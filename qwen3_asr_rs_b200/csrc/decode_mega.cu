@@ -5,11 +5,10 @@
 // down} + lm_head).  As separate kernels each phase pays launch latency and a cold weight stream;
 // with device-wide barriers each phase pays an atomic + spin + re-read.
 // Here one CTA per SM stays resident for the whole step:
-//   * a producer warp streams this CTA's slice of EVERY weight matrix, in phase order, into a
-//     shared-memory ring with cp.async.bulk (TMA bulk copy) + mbarrier transaction counts, and the
-//     K/V rows of earlier positions into a staging tile.  None of these addresses depend on
-//     activations, so the producer runs AHEAD across phase boundaries: HBM stays busy while
-//     consumers wait for activations.
+//   * a producer warp streams this CTA's slice of EVERY weight matrix and the K/V rows of earlier
+//     positions, in consumption order, into a shared-memory ring with cp.async.bulk (TMA bulk copy) +
+//     mbarrier transaction counts.  None of these addresses depend on activations, so the producer
+//     runs AHEAD across phase boundaries: HBM stays busy while consumers wait for activations.
 //   * 8 consumer warps do the fp32 GEMV from shared memory (activation vector held in registers,
 //     bf16 -> fp32 up-cast is exact, fp32 FMA accumulate).
 //   * activations are exchanged between CTAs WITHOUT barriers: every published fp32 value travels
@@ -47,59 +46,9 @@ struct Params {
     // tagged exchange buffers ({value, tag} words)
     uint2* qkv_ll; uint2* part_ll; uint2* attn_ll; uint2* x_ll; uint2* act_ll;
     long long* dbg;              // optional timeline [2][DBG_SLOTS] of clock64 (CTA 0 and CTA G-1), else null
-    int pf_ahead;                // L2 prefetch distance in ring chunks (0 = off)
 };
 
-// The shared-memory ring only buffers a few microseconds of the weight stream (128 KB at an SM's ~25 GB/s share of H100
-// HBM), and a ring slot can only be refilled once its rows have been consumed: the refill of the slots a phase has just
-// released must land before the phase after next needs them.  With the all-gathers re-reading only their missing words
-// (ll_gather, mega_common.cuh) a refill from DRAM can arrive too late for the GEMV turns.  So the producer also runs an L2
-// prefetch cursor `pf_ahead` ring chunks ahead of the ring (ASRB_MEGA_PF overrides): the refill then comes from L2.  A
-// cursor far ahead gets its prefetched lines evicted before use.
-static constexpr int PF_AHEAD = 2;
-
-template <int H, int QD, int I>
-struct ChunkCursor {
-    int l, ph, r; Slice s; bool done;
-    const DecLayerW* ltab;
-    __device__ void load(const Params& p) {
-        if (l >= p.L) { if (l == p.L && ph == 0) s = make_slice(p.lm_head, p.V, H, 1); else { done = true; return; } }
-        else {
-            const DecLayerW w = ltab[l];
-            s = ph == 0 ? make_slice(w.wqkv, QD + 2 * p.KVD, H, 1) : ph == 1 ? make_slice(w.wo, H, QD, 1)
-              : ph == 2 ? make_slice(w.wgu, 2 * I, H, 2) : make_slice(w.wdown, H, I, 1);
-        }
-        r = s.r0;
-    }
-    __device__ void init(const Params& p, const DecLayerW* table) { ltab = table; l = 0; ph = 0; done = false; load(p); }
-    __device__ bool next(const Params& p, const bf16*& src, uint32_t& bytes) {
-        while (!done && r >= s.r1) {
-            if (l >= p.L) { done = true; break; }
-            if (++ph == 4) { ph = 0; ++l; }
-            load(p);
-        }
-        if (done) return false;
-        const int rows = min(s.rpc, s.r1 - r);
-        src = s.W + (size_t)r * s.K; bytes = (uint32_t)rows * s.K * 2;
-        r += s.rpc;
-        return true;
-    }
-};
-
-// producer: issue all chunks of a slice into the ring; every issued chunk advances the L2 prefetch cursor
-template <class Cursor>
-__device__ __forceinline__ void produce(const Slice& s, const Ring& ring, uint32_t& q, Cursor& pf, const Params& p) {
-    for (int r = s.r0; r < s.r1; r += s.rpc, ++q) {
-        int rows = min(s.rpc, s.r1 - r);
-        uint32_t slot = q % ring.nslot, par = (q / ring.nslot) & 1;
-        mbar_wait(&ring.empty[slot], par ^ 1);
-        uint32_t bytes = (uint32_t)rows * s.K * 2;
-        mbar_expect_tx(&ring.full[slot], bytes);
-        bulk_g2s(ring.slots + (size_t)slot * SLOT_BYTES, s.W + (size_t)r * s.K, bytes, &ring.full[slot]);
-        const bf16* psrc; uint32_t pbytes;
-        if (p.pf_ahead > 0 && pf.next(p, psrc, pbytes)) l2_prefetch(psrc, pbytes);
-    }
-}
+static_assert(KV_KEYS * HD * 4 == SLOT_BYTES, "K / V tiles travel through the weight ring: one tile per slot");
 
 // GEMV row mapping: a row of K bf16 weights is contracted by one warp; lane `lane` holds the activations of elements
 // (c * 32 + lane) * 8 .. +8 for every 256-element chunk c in registers.
@@ -509,17 +458,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     Ring ring;
     ring.slots = smem;
     ring.nslot = NS;
-    uint8_t* kv_smem = smem + (size_t)NS * SLOT_BYTES;              // [K tile | V tile]
-    float* xs = reinterpret_cast<float*>(kv_smem + 2 * KV_TILE_BYTES);
+    float* xs = reinterpret_cast<float*>(smem + (size_t)NS * SLOT_BYTES);
     float* xres = xs + XS_FLOATS;                                      // [XRES_MAX] residual rows owned by this CTA
     float* pbuf = xres + XRES_MAX;                                     // [2][PARAM_FLOATS] per-layer small vectors (double buffer)
     float* ropes = pbuf + 2 * PARAM_FLOATS;                            // [128] cos | sin of this step's position
     DecLayerW* ltab = reinterpret_cast<DecLayerW*>(ropes + 128);       // [MAX_LAYERS]
     uint64_t* bars = reinterpret_cast<uint64_t*>(ltab + MAX_LAYERS);
     ring.full = bars; ring.empty = bars + NSLOT_MAX;
-    uint64_t* kv_full = bars + 2 * NSLOT_MAX; uint64_t* kv_empty = kv_full + 1;
-    uint64_t* p_full = kv_empty + 1; uint64_t* p_empty = p_full + 2;   // [2] each
-    float* red = reinterpret_cast<float*>(bars + 2 * NSLOT_MAX + 6);      // [64]
+    uint64_t* p_full = bars + 2 * NSLOT_MAX; uint64_t* p_empty = p_full + 2;   // [2] each
+    float* red = reinterpret_cast<float*>(bars + 2 * NSLOT_MAX + 4);      // [64]
     int* ired = reinterpret_cast<int*>(red + 64);                      // [64]
     float* part = reinterpret_cast<float*>(ired + 64);                 // [2][8 warps][8 rows] K-split partials (consume_ksplit)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -529,7 +476,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
 
     if (tid == 0) {
         for (int i = 0; i < NS; ++i) { mbar_init(&ring.full[i], 1); mbar_init(&ring.empty[i], NCONS_WARPS); }
-        mbar_init(kv_full, 1); mbar_init(kv_empty, NCONS_WARPS);
         for (int i = 0; i < 2; ++i) { mbar_init(&p_full[i], 1); mbar_init(&p_empty[i], NCONS_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -550,21 +496,25 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     const bool att_cta = (int)blockIdx.x < p.nkv * p.nsplit;
     const int att_g = blockIdx.x / p.nsplit, att_sp = blockIdx.x % p.nsplit, att_j0 = att_sp * KV_KEYS;
     const int n_old = att_cta ? max(0, min(pos - att_j0, KV_KEYS)) : 0;
-    uint32_t kvq = 0;
     uint32_t q = 0;
     if (is_producer) {
+        // ONE stream in consumption order through ONE ring: per layer the [q|k|v] rows, this CTA's K tile and V tile of
+        // the earlier positions (one slot each, when its split holds any), the o_proj, gate/up and down_proj rows; then the
+        // lm_head.  The copies carry an L2 evict_first hint: every line is read once per step.  (Prefetching further ahead
+        // into L2 measured slower on the H100 at any distance: see DESIGN.md section 4.1.)
         if (lane == 0) {
-            ChunkCursor<H, QD, I> pf;
-            pf.init(p, ltab);
-            {   // start the HBM stream immediately: the first PF_AHEAD chunks go to L2 now
-                const bf16* psrc; uint32_t pbytes;
-                for (int i = 0; i < p.pf_ahead; ++i) if (pf.next(p, psrc, pbytes)) l2_prefetch(psrc, pbytes);
-            }
+            const uint64_t pol = l2_evict_first_policy();
+            auto issue = [&](const void* src, uint32_t bytes) __attribute__((always_inline)) {
+                const uint32_t slot = q % NS, par = (q / NS) & 1;
+                mbar_wait(&ring.empty[slot], par ^ 1);
+                mbar_expect_tx(&ring.full[slot], bytes);
+                bulk_g2s_hint(ring.slots + (size_t)slot * SLOT_BYTES, src, bytes, &ring.full[slot], pol);
+                ++q;
+            };
+            auto issue_slice = [&](const Slice& s) __attribute__((always_inline)) {
+                for (int r = s.r0; r < s.r1; r += s.rpc) issue(s.W + (size_t)r * s.K, (uint32_t)min(s.rpc, s.r1 - r) * s.K * 2);
+            };
             const size_t kv_row = ((size_t)att_g * p.max_ctx + att_j0) * HD;
-            if (n_old > 0) {   // K/V tiles of the first two layers
-                l2_prefetch(p.kcache + kv_row, (uint32_t)n_old * HD * 4);
-                l2_prefetch(p.vcache + kv_row, (uint32_t)n_old * HD * 4);
-            }
             for (int l = 0; l <= p.L; ++l) {
                 {   // small per-layer vectors -> pbuf[l & 1] (layer L = final norm only)
                     float* pb = pbuf + (l & 1) * PARAM_FLOATS;
@@ -583,31 +533,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
                     }
                 }
                 const DecLayerW w = ltab[l];
-                produce(make_slice(w.wqkv, QD + 2 * p.KVD, H, 1), ring, q, pf, p);
-                if (n_old > 0) {   // K/V rows of earlier positions do not depend on this step: prefetch them too
-                    const uint32_t bytes = (uint32_t)n_old * HD * 4;
-                    if (l + 1 < p.L) {
-                        l2_prefetch(p.kcache + (size_t)(l + 1) * p.cache_layer_stride + kv_row, bytes);
-                        l2_prefetch(p.vcache + (size_t)(l + 1) * p.cache_layer_stride + kv_row, bytes);
-                    }
-                    mbar_wait(kv_empty, (kvq & 1) ^ 1);
-                    mbar_expect_tx(kv_full, 2 * bytes);
+                issue_slice(make_slice(w.wqkv, QD + 2 * p.KVD, H, 1));
+                if (n_old > 0) {
                     const size_t off = (size_t)l * p.cache_layer_stride + kv_row;
-                    bulk_g2s(kv_smem, p.kcache + off, bytes, kv_full);
-                    bulk_g2s(kv_smem + KV_TILE_BYTES, p.vcache + off, bytes, kv_full);
-                    ++kvq;
+                    issue(p.kcache + off, (uint32_t)n_old * HD * 4);
+                    issue(p.vcache + off, (uint32_t)n_old * HD * 4);
                 }
-                produce(make_slice(w.wo, H, QD, 1), ring, q, pf, p);
-                produce(make_slice(w.wgu, 2 * I, H, 2), ring, q, pf, p);
-                produce(make_slice(w.wdown, H, I, 1), ring, q, pf, p);
+                issue_slice(make_slice(w.wo, H, QD, 1));
+                issue_slice(make_slice(w.wgu, 2 * I, H, 2));
+                issue_slice(make_slice(w.wdown, H, I, 1));
             }
-            produce(make_slice(p.lm_head, p.V, H, 1), ring, q, pf, p);
-            {   // warm L2 with the head of the NEXT step's stream (same addresses every step)
-                ChunkCursor<H, QD, I> nx;
-                nx.init(p, ltab);
-                const bf16* psrc; uint32_t pbytes;
-                for (int i = 0; i < p.pf_ahead; ++i) if (nx.next(p, psrc, pbytes)) l2_prefetch(psrc, pbytes);
-            }
+            issue_slice(make_slice(p.lm_head, p.V, H, 1));
         }
         return;
     }
@@ -667,8 +603,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
                 float* osum = ml + 8;                 // [warps][2][128] per-warp partial outputs (group == 2 path)
                 float* wml = osum + NCONS_WARPS * 2 * HD;   // [warps][2][2] per-warp (max, sum)
                 float* snew = wml + NCONS_WARPS * 4;  // [group] score of the current token's key per head (merging CTA)
-                float* Ks = reinterpret_cast<float*>(kv_smem);
-                float* Vs = reinterpret_cast<float*>(kv_smem + KV_TILE_BYTES);
+                // the producer streams this split's K tile and V tile right after the [q|k|v] rows
+                const uint32_t ksl = q % ring.nslot, vsl = (q + 1) % ring.nslot;
+                const float* Ks = reinterpret_cast<const float*>(ring.slots + (size_t)ksl * SLOT_BYTES);
+                const float* Vs = reinterpret_cast<const float*>(ring.slots + (size_t)vsl * SLOT_BYTES);
                 MEGA_FINE(24);
                 cons_sync();                          // xs (phase-1 activations) no longer needed by any warp; q/k/v words are
                                                       // polled directly below (few readers per word)
@@ -681,7 +619,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
                     for (int i = 0; i < 4; ++i) vn[lane + 32 * i] = vv[i];
                 }
                 MEGA_FINE(25);
-                mbar_wait(kv_full, kvq & 1);          // prefetched K/V tiles have landed
+                mbar_wait(&ring.full[ksl], (q / ring.nslot) & 1);
+                mbar_wait(&ring.full[vsl], ((q + 1) / ring.nslot) & 1);
                 cons_sync();
                 MEGA_FINE(26);
                 if (merger) {
@@ -813,11 +752,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
                         if (d < 2) ll_store(rec + HD + d, ml[hq * 2 + d], tl | PH_PART);
                     }
                 }
-                {                                     // hand the K/V staging buffer back to the producer
+                {                                     // hand the K / V slots back to the producer
                     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(kv_empty);
-                    ++kvq;
+                    if (lane == 0) { mbar_arrive(&ring.empty[ksl]); mbar_arrive(&ring.empty[vsl]); }
+                    q += 2;
                 }
                 MEGA_FINE(30);
                 MEGA_GT(1);
@@ -985,12 +924,12 @@ static long long* g_last_dbg = nullptr;   // debug only (ASRB_MEGA_DEBUG): timel
 
 static int mega_xs_floats(int I) { return std::max(I, mega::XS_MIN) + 64; }
 static size_t mega_smem_bytes(int H, int I, int nslot) {
-    return (size_t)nslot * mega::SLOT_BYTES + 2 * mega::KV_TILE_BYTES +
+    return (size_t)nslot * mega::SLOT_BYTES +
            (mega_xs_floats(I) + mega::XRES_MAX + 2 * (2 * H + 2 * mega::HD) + 128) * 4 + mega::MAX_LAYERS * sizeof(DecLayerW) +
-           (2 * mega::NSLOT_MAX + 6) * 8 + 64 * 4 + 64 * 4 + 128 * 4 + 64;
+           (2 * mega::NSLOT_MAX + 4) * 8 + 64 * 4 + 64 * 4 + 128 * 4 + 64;
 }
 // instantiations: (hidden, q_dim, intermediate) -> ring depth
-static int mega_nslot(const asrb_dims& c) { return c.hidden_size > 1024 ? 3 : 4; }
+static int mega_nslot(const asrb_dims& c) { return c.hidden_size > 1024 ? 5 : 6; }
 
 template <int H, int QD, int I> static bool dims_match(const asrb_dims& c) {
     return c.hidden_size == H && c.num_attention_heads * c.head_dim == QD && c.intermediate_size == I;
@@ -1033,9 +972,9 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
     const int nsplit = std::min(mega::MAX_SPLITS, std::min(G / c.num_key_value_heads, (max_ctx + mega::KV_KEYS - 1) / mega::KV_KEYS));
     const size_t smem = mega_smem_bytes(c.hidden_size, c.intermediate_size, mega_nslot(c));
     const void* fn = nullptr;
-    if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 4>;          // Qwen3-ASR-0.6B
-    else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 3>;     // Qwen3-ASR-1.7B
-    else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 4>;                                             // test config
+    if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6>;          // Qwen3-ASR-0.6B
+    else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5>;     // Qwen3-ASR-1.7B
+    else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6>;                                             // test config
     ASRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // The kernel handles one sequence.  A batch runs as B launches on the stream (weights are re-streamed per sequence:
     // 2.0 k tokens/s at any batch size, still ~1.8x the per-phase path at batch 8); a sequence that has finished
@@ -1061,8 +1000,6 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
         p.act_ll = w; w += c.intermediate_size;
         p.dbg = mb.dbg;
         g_last_dbg = mb.dbg;
-        static const int pf_env = [] { const char* e = getenv("ASRB_MEGA_PF"); return e ? atoi(e) : mega::PF_AHEAD; }();
-        p.pf_ahead = pf_env;
         // tags must stay monotonic for red.max publication: long before the 24-bit epoch wraps, wipe the exchange buffers
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {
             ASRB_CUDA_CHECK(cudaMemsetAsync(mb.part, 0, mb.part_bytes, st));

@@ -10,9 +10,8 @@ static constexpr int NCONS_WARPS = 8;
 static constexpr int NCONS = NCONS_WARPS * 32;          // 256 consumer threads
 static constexpr int NTHREADS = NCONS + 32;             // + 1 producer warp
 static constexpr int SLOT_BYTES = 32 * 1024;           // 16 rows of K = 1024: one row per half-warp and pass
-static constexpr int NSLOT_MAX = 4;                     // weight ring: 4 x 32 KB in flight per SM (3 for the 1.7B dims: larger vectors)
-static constexpr int KV_KEYS = 64;                      // keys per attention split (K and V tiles staged in smem)
-static constexpr int KV_TILE_BYTES = KV_KEYS * 128 * 4; // 32 KB each for K and V (fp32 cache)
+static constexpr int NSLOT_MAX = 6;                     // weight ring: 6 x 32 KB per SM (5 for the 1.7B dims: larger vectors)
+static constexpr int KV_KEYS = 64;                      // keys per attention split (the K and V tiles are one ring slot each)
 static constexpr int XS_MIN = 3072;                     // activation vector / attention scratch: max(I, XS_MIN) + 64 floats
 static constexpr int XRES_MAX = 64;
 static constexpr int MAX_LAYERS = 32;                   // layer table staged in shared memory                     // residual rows owned by one CTA (H / gridDim.x, rounded up)
@@ -49,6 +48,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+// L2 policy for data read exactly once per step: its lines are the first to go when L2 needs room
+__device__ __forceinline__ uint64_t l2_evict_first_policy() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ void bulk_g2s_hint(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void cons_sync() { asm volatile("bar.sync 1, %0;" ::"n"(NCONS) : "memory"); }
 
@@ -144,10 +153,6 @@ __device__ __forceinline__ Slice make_slice(const bf16* W, int N, int K, int rst
     s.rpc = SLOT_BYTES / (K * 2);
     s.rpc &= ~1;                        // keep (gate, up) pairs together
     return s;
-}
-
-__device__ __forceinline__ void l2_prefetch(const void* src, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
 }
 
 }  // namespace mega
