@@ -122,26 +122,8 @@ __device__ __forceinline__ void mma_tile(uint32_t arow, int akey, int ac0, uint3
         for (int k = 0; k < 4; ++k) acc[nt][k] += acc1[nt][k] + acc2[nt][k];
 }
 
-// ---- self-validating 4-byte exchange words (the all-to-all vectors: x after o_proj / down_proj, attention output,
-// SwiGLU activations).  A word is the fp32 value itself; 0xFFFFFFFF (a NaN pattern no result is ever published with)
-// means "not written yet".  Publication = one fire-and-forget red.and (performed at L2 at once, like red.max of the
-// tagged words); the gather polls 16-byte quads until none of the 4 words is the sentinel -- half the L2 traffic of
-// {value, tag} words, and that traffic (one CTA per SM x every vector x NB sequences) is what bounds the batched step.
-// Every (layer, vector) has its own region, and there are two such sets: step s uses set s & 1 and, at its start,
-// re-arms (stores the sentinel into) the words THIS CTA wrote into the other set during step s - 1.  The kernel
-// boundary orders that re-arm before any publication of step s + 1 into it, so a poll can only ever see the sentinel or
-// the current step's value.
-static constexpr uint32_t SX_EMPTY = 0xFFFFFFFFu;
-__device__ __forceinline__ void sx_store(uint32_t* p, float v) {
-    uint32_t b = __float_as_uint(v);
-    if (b == SX_EMPTY) b = 0x7FFFFFFFu;                   // (another NaN)
-    asm volatile("red.relaxed.gpu.global.and.b32 [%0], %1;" ::"l"(p), "r"(b) : "memory");
-}
-__device__ __forceinline__ uint4 sx_load4(const uint32_t* p) {
-    uint4 v;
-    asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-    return v;
-}
+// (the all-to-all vectors travel as self-validating 4-byte words: SX_EMPTY, sx_store, sx_load4 in mega_common.cuh;
+//  the multiplier of their traffic here is NB sequences)
 
 // per-head RMSNorm + RoPE of one 128-vector by one warp (lane holds d = lane, +32, +64, +96); input = tagged words
 __device__ __forceinline__ void head_norm_rope_b(const uint2* __restrict__ src, uint32_t tag, const float* __restrict__ nw,

@@ -11,11 +11,15 @@
 //     runs AHEAD across phase boundaries: HBM stays busy while consumers wait for activations.
 //   * 8 consumer warps do the fp32 GEMV from shared memory (activation vector held in registers,
 //     bf16 -> fp32 up-cast is exact, fp32 FMA accumulate).
-//   * activations are exchanged between CTAs WITHOUT barriers: every published fp32 value travels
-//     in an 8-byte {value, tag} word (tag = launch epoch/layer/phase), published with one 64-bit
-//     fire-and-forget `red.max` (performed at L2 immediately; the tag grows monotonically so max acts as
-//     an exchange) and polled with 128-bit relaxed loads until the tags match -- data and "ready" flag
-//     arrive in the same L2 round trip (the low-latency protocol of collective libraries, on-chip).
+//   * activations are exchanged between CTAs WITHOUT barriers, and data and "ready" flag arrive in the
+//     same L2 round trip (the low-latency protocol of collective libraries, on-chip).  The vectors every
+//     CTA reads in full (x after o_proj and after down_proj, attention output, SwiGLU activations) travel
+//     as self-validating 4-byte words (the fp32 value itself, 0xFFFFFFFF = not written yet), published
+//     with one fire-and-forget `red.and` and polled as 16-byte quads; two sets of per-layer regions
+//     alternate between launches (mega_common.cuh).  The few-reader q/k/v rows and attention partials
+//     travel in 8-byte {value, tag} words (tag = launch epoch/layer/phase), published with one 64-bit
+//     `red.max` (performed at L2 immediately; the tag grows monotonically so max acts as an exchange)
+//     and polled until the tags match.
 //   * attention (QK-RMSNorm + RoPE + KV append + softmax.V) is split over kv-heads x 64-key tiles;
 //     the tile-0 CTA of each kv-head merges the partials and publishes the head outputs.
 //   * the last CTA to finish the lm_head performs the greedy bookkeeping (argmax, EOS, append,
@@ -42,9 +46,10 @@ struct Params {
     int nsplit;
     float* part_val; int* part_idx;     // [gridDim.x]
     int* pos; int* done; int* next_id; int* ids_out; int* n_out; int max_new;
-    unsigned* bar;               // [0] finish ticket, [1] launch epoch (starts at 1; 0 marks never-written words)
-    // tagged exchange buffers ({value, tag} words)
-    uint2* qkv_ll; uint2* part_ll; uint2* attn_ll; uint2* x_ll; uint2* act_ll;
+    unsigned* bar;               // [0] finish ticket, [1] launch epoch (starts at 1; 0 marks never-written words),
+                                 // [3] executed launches of this kernel (selects the set of self-validating words)
+    uint2* qkv_ll; uint2* part_ll;      // tagged exchange buffers ({value, tag} words)
+    uint32_t* sx;                // self-validating words [2 sets][L][x_o H | x_d H | attn QD | act I]
     long long* dbg;              // optional timeline [2][DBG_SLOTS] of clock64 (CTA 0 and CTA G-1), else null
 };
 
@@ -179,18 +184,20 @@ __device__ __forceinline__ float warp_reduce8(const float (&a)[8], int lane) {
     return v;
 }
 
-enum { ME_STORE = 0, ME_RESID = 1, ME_SWIGLU = 2, ME_ARGMAX = 3 };
+enum { ME_STORE = 0, ME_SWIGLU = 1, ME_ARGMAX = 2 };
 
 // Residual GEMVs (o_proj, down_proj: a handful of rows per CTA, long K): all 8 warps split K of EVERY row instead of one
 // warp per row.  A thread owns the 16-byte weight groups tid, tid + 256, ... of each row (its 8 activations per group come
 // straight from xs), keeps one partial per row (8 independent FMA chains), the warp reduces its 8 partials with one
 // transposed reduction (9 shuffles), the 8 warp partials of a row are summed in a fixed order by one thread, which applies
-// the residual and publishes.  Rows are taken 8 at a time; a group spans two ring slots when a slot holds fewer than 8.
+// the residual and publishes to `out`.  Rows are taken 8 at a time; a group spans two ring slots when a slot holds fewer
+// than 8.
 // (The one-warp-per-row form left 1 of 8 warps idle and paid the load -> unpack -> FMA -> 5-shuffle latency chain once per
-// row with nothing to overlap it.)
+// row with nothing to overlap it.  Feeding each thread's activations straight from the exchange words into registers,
+// without the copy into xs and its barrier, measured 4.5 % slower per step on the H100: see DESIGN.md section 4.1.)
 template <int K>
-__device__ __forceinline__ void consume_ksplit(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
-                                               uint32_t tag, float* xres, float* part) {
+__device__ __forceinline__ void consume_ksplit(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint32_t* out,
+                                               float* xres, float* part) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     constexpr int NU = K / 8;                                  // 16-byte groups per row
     constexpr int J = (NU + NCONS - 1) / NCONS;
@@ -250,7 +257,7 @@ __device__ __forceinline__ void consume_ksplit(const Slice& s, const Ring& ring,
                 for (int w8 = 1; w8 < NCONS_WARPS; ++w8) t += pb[w8 * 8 + tid];
                 const int row = r + g0 + tid;
                 const float nv = xres[row - s.r0] + t; xres[row - s.r0] = nv;
-                ll_store(out + row, nv, tag);
+                sx_store(out + row, nv);
             }
         }
         r += R; q += pair ? 2 : 1;
@@ -260,7 +267,7 @@ __device__ __forceinline__ void consume_ksplit(const Slice& s, const Ring& ring,
 // K <= 1024 GEMVs (qkv, gate/up, lm_head of the 0.6B dims): four rows per warp and turn, two ring slots (32 rows) per turn.
 template <int K, int EPI>
 __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
-                                             uint32_t tag, float& best_v, int& best_i,
+                                             uint32_t tag, uint32_t* sxo, float& best_v, int& best_i,
                                              const float* norm_w, float norm_r, long long* fine) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int fi = 0;
@@ -297,7 +304,7 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
             const int row = r + i0 + j;
             if (EPI == ME_SWIGLU) {                // rows (gate, up, gate, up): lanes 0 / 16 hold a gate, lanes 8 / 24 its up row
                 const float up = __shfl_xor_sync(0xffffffffu, v, 8);
-                if ((lane & 15) == 0 && j < nv) ll_store(out + (row >> 1), silu(v) * up, tag);
+                if ((lane & 15) == 0 && j < nv) sx_store(sxo + (row >> 1), silu(v) * up);
             } else if (EPI == ME_STORE) {
                 if ((lane & 7) == 0 && j < nv) ll_store(out + row, v, tag);
             } else {                               // ME_ARGMAX: rows arrive in increasing order per lane, strict > keeps the first maximum
@@ -314,15 +321,13 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
 }
 
 // consumer: process all chunks of a slice.  `xs` holds the (already normalised) activation vector.
-// Results are published as tagged words to `out` (ME_STORE / ME_SWIGLU), added to the CTA-local
-// residual rows `xres` and published (ME_RESID), or folded into the running argmax (ME_ARGMAX).
+// Results are published as tagged words to `out` (ME_STORE), as self-validating words to `sxo` (ME_SWIGLU), or folded
+// into the running argmax (ME_ARGMAX).
 template <int K, int EPI>
 __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
-                                        uint32_t tag, float* xres, float& best_v, int& best_i,
-                                        const float* norm_w = nullptr, float norm_r = 1.f, long long* fine = nullptr,
-                                        float* part = nullptr) {
-    if constexpr (EPI == ME_RESID) { consume_ksplit<K>(s, ring, q, xs, out, tag, xres, part); return; }
-    else if constexpr (K <= 1024) { consume_quad<K, EPI>(s, ring, q, xs, out, tag, best_v, best_i, norm_w, norm_r, fine); return; }
+                                        uint32_t tag, uint32_t* sxo, float& best_v, int& best_i,
+                                        const float* norm_w = nullptr, float norm_r = 1.f, long long* fine = nullptr) {
+    if constexpr (K <= 1024) { consume_quad<K, EPI>(s, ring, q, xs, out, tag, sxo, best_v, best_i, norm_w, norm_r, fine); return; }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int fi = 0;
 #define CF() do { if (fine && threadIdx.x == 0 && fi < 24) fine[fi++] = clock64(); } while (0)
@@ -365,7 +370,7 @@ __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32
                     v0 = row_dot_smem<K>(base + (size_t)(ub * 2) * (K / 8), xs, lane);
                     v1 = row_dot_smem<K>(base + (size_t)(ub * 2 + 1) * (K / 8), xs, lane);
                 }
-                if (lane == 0) ll_store(out + (row >> 1), silu(v0) * v1, tag);
+                if (lane == 0) sx_store(sxo + (row >> 1), silu(v0) * v1);
             } else {
                 bool act; int row; float v0;
                 if (DUAL) {
@@ -381,8 +386,6 @@ __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32
                 }
                 if (EPI == ME_STORE) {
                     if (act) ll_store(out + row, v0, tag);
-                } else if (EPI == ME_RESID) {
-                    if (act) { const float nv = xres[row - s.r0] + v0; xres[row - s.r0] = nv; ll_store(out + row, nv, tag); }
                 } else {
                     if (act && v0 > best_v) { best_v = v0; best_i = row; }
                 }
@@ -396,6 +399,57 @@ __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32
     CF();
 #undef CF
     if (!XREG) cons_sync();                        // xs was read in place: nobody may overwrite it before this point
+}
+
+// all consumer threads: gather the N self-validating words at `src` into xs (xs_swz layout) and return this thread's sum of
+// squares of elements 2i, 2i + 1 for i = tid, tid + NCONS, ... in that order (the partial sums norm_scale reduces).
+// Warp w polls exactly the quads that hold its threads' pairs -- quads 16 w + (0..15) + NCONS / 2 * u, lane taking
+// u = 2 k + (lane >> 4) -- so the squares are read back from xs after a __syncwarp, without a CTA barrier.
+template <int N>
+__device__ __forceinline__ float sx_gather(const uint32_t* src, float* xs) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int NQ = N / 4;
+    constexpr int KQ = (NQ + NCONS - 1) / NCONS;              // quads per thread
+    int qi[KQ];
+    uint4 v[KQ];
+#pragma unroll
+    for (int k = 0; k < KQ; ++k) {
+        qi[k] = 16 * warp + (lane & 15) + (NCONS / 2) * (2 * k + (lane >> 4));
+        v[k] = make_uint4(SX_EMPTY, SX_EMPTY, SX_EMPTY, SX_EMPTY);
+    }
+    bool ok;
+    do {                                                       // only the quads still missing are re-read
+        ok = true;
+#pragma unroll
+        for (int k = 0; k < KQ; ++k)
+            if (qi[k] < NQ && !sx_ready(v[k])) v[k] = sx_load4(src + 4 * qi[k]);
+#pragma unroll
+        for (int k = 0; k < KQ; ++k)
+            if (qi[k] < NQ) ok = ok && sx_ready(v[k]);
+    } while (!ok);
+#pragma unroll
+    for (int k = 0; k < KQ; ++k)
+        if (qi[k] < NQ) *reinterpret_cast<uint4*>(xs + xs_swz(4 * qi[k])) = v[k];
+    __syncwarp();
+    float ss = 0.f;
+#pragma unroll
+    for (int i = tid; i < N / 2; i += NCONS) {
+        const float2 x = *reinterpret_cast<const float2*>(xs + xs_swz(2 * i));
+        ss = fmaf(x.x, x.x, ss); ss = fmaf(x.y, x.y, ss);
+    }
+    return ss;
+}
+
+// all consumer threads: copy the N self-validating words at `src` into xs (xs_swz layout), the input of o_proj / down_proj.
+// A thread spins on one quad at a time: a single load in flight per thread while the words are not yet published keeps
+// the polling traffic of 132 CTAs low (measured faster than re-polling all of a thread's missing quads per round).
+template <int N>
+__device__ __forceinline__ void sx_copy(const uint32_t* src, float* xs) {
+    for (int j = threadIdx.x; j < N / 4; j += NCONS) {
+        uint4 v;
+        do { v = sx_load4(src + 4 * j); } while (!sx_ready(v));
+        *reinterpret_cast<uint4*>(xs + xs_swz(4 * j)) = v;
+    }
 }
 
 // RMSNorm scale of the vector sitting in xs from the per-thread partial sums of squares; the scaling itself is
@@ -496,6 +550,28 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     const bool att_cta = (int)blockIdx.x < p.nkv * p.nsplit;
     const int att_g = blockIdx.x / p.nsplit, att_sp = blockIdx.x % p.nsplit, att_j0 = att_sp * KV_KEYS;
     const int n_old = att_cta ? max(0, min(pos - att_j0, KV_KEYS)) : 0;
+    const bool merger = att_cta && att_sp == 0;     // merges the attention partials of kv head att_g and publishes its outputs
+    // residual rows owned by this CTA (same row partition for o_proj and down_proj), and its gate/up units
+    const Slice xsl = make_slice(nullptr, H, QD, 1), sl_gu = make_slice(nullptr, 2 * I, H, 2);
+
+    // self-validating words of this launch: set = parity of bar[3], the count of executed launches of THIS kernel (the
+    // launch epoch bar[1] also advances on batched steps, which would break the strict alternation the re-arm relies on)
+    constexpr size_t SXL = 2 * H + QD + I;          // words per (set, layer): x_o | x_d | attn | act
+    const unsigned sstep = __ldcg(p.bar + 3);
+    uint32_t* const sx_cur = p.sx + (size_t)(sstep & 1u) * p.L * SXL;
+    // Re-arm of layer l of the other set (consumer threads): exactly the words this CTA publishes, from the slices and head
+    // mapping its publishing code uses -- its residual rows of x_o and x_d (consume_ksplit over sl_o / sl_dn, the rows of
+    // xsl), the act rows of its gate/up units, and as merging CTA the group x 128 attention outputs of its kv head.  Every
+    // word of a set is published in every executed step (pos >= 1, so split 0 of every kv head always merges), so the
+    // re-arms of all CTAs cover the whole set.
+    auto rearm = [&](int l) __attribute__((always_inline)) {
+        uint32_t* const base = p.sx + (size_t)((sstep & 1u) ^ 1u) * p.L * SXL + (size_t)l * SXL;
+        const int xrows = xsl.r1 - xsl.r0, a0 = sl_gu.r0 / 2, arows = sl_gu.r1 / 2 - a0;
+        const int nattn = merger ? p.group * HD : 0;
+        for (int i = tid; i < xrows; i += NCONS) { base[xsl.r0 + i] = SX_EMPTY; base[H + xsl.r0 + i] = SX_EMPTY; }
+        for (int i = tid; i < nattn; i += NCONS) base[2 * H + att_g * p.group * HD + i] = SX_EMPTY;
+        for (int i = tid; i < arows; i += NCONS) base[2 * H + QD + a0 + i] = SX_EMPTY;
+    };
     uint32_t q = 0;
     if (is_producer) {
         // ONE stream in consumption order through ONE ring: per layer the [q|k|v] rows, this CTA's K tile and V tile of
@@ -560,28 +636,30 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     // tag = launch epoch (unique per executed step, survives new utterances that revisit the same positions)
     const unsigned epoch = __ldcg(p.bar + 1);
     const uint32_t tag_base = (epoch & 0xffffffu) << 8;
-    // residual rows owned by this CTA (same row partition for o_proj and down_proj)
-    const Slice xsl = make_slice(nullptr, H, QD, 1);
     // slice geometry does not depend on the layer: computed once, only the weight pointer changes
-    Slice sl_qkv = make_slice(nullptr, QD + 2 * p.KVD, H, 1), sl_o = make_slice(nullptr, H, QD, 1),
-          sl_gu = make_slice(nullptr, 2 * I, H, 2), sl_dn = make_slice(nullptr, H, I, 1);
+    Slice sl_qkv = make_slice(nullptr, QD + 2 * p.KVD, H, 1), sl_o = make_slice(nullptr, H, QD, 1), sl_dn = make_slice(nullptr, H, I, 1);
     for (int i = tid; i < xsl.r1 - xsl.r0; i += NCONS) xres[i] = __ldcg(p.x + xsl.r0 + i);
+    for (int l = 0; l < p.L; ++l) rearm(l);
 
     for (int l = 0; l < p.L; ++l) {
         const DecLayerW w = ltab[l];
         const uint32_t tl = tag_base | ((uint32_t)l << 3);
         const float* pb = pbuf + (l & 1) * PARAM_FLOATS;               // ln_in | ln_post | q_norm | k_norm of this layer
+        uint32_t* const sx_xo = sx_cur + (size_t)l * SXL;
+        uint32_t* const sx_xd = sx_xo + H;
+        uint32_t* const sx_attn = sx_xo + 2 * H;
+        uint32_t* const sx_act = sx_xo + 2 * H + QD;
         mbar_wait(&p_full[l & 1], (l >> 1) & 1);
         // ---- phase 1: RMSNorm + [q|k|v] GEMV ----
         float nr;
         {
             float ss = 0.f;
             if (l == 0) { for (int i = tid; i < H; i += NCONS) { const float v = __ldcg(p.x + i); xs[xs_swz(i)] = v; ss = fmaf(v, v, ss); } }
-            else { MEGA_FINE(0); MEGA_FINE(1); ss = ll_gather(p.x_ll, H, (tag_base | ((uint32_t)(l - 1) << 3)) | PH_XD, xs); MEGA_FINE(2); }
+            else { MEGA_FINE(0); MEGA_FINE(1); ss = sx_gather<H>(sx_xd - SXL, xs); MEGA_FINE(2); }     // x_d of layer l - 1
             nr = norm_scale(ss, H, p.eps, red);
             MEGA_FINE(3);
         }
-        consume<H, ME_STORE>(sl_qkv, ring, q, xs, p.qkv_ll, tl | PH_QKV, xres, best_v, best_i, pb, nr);
+        consume<H, ME_STORE>(sl_qkv, ring, q, xs, p.qkv_ll, tl | PH_QKV, nullptr, best_v, best_i, pb, nr);
         MEGA_FINE(4);
         MEGA_GT(0);
         MEGA_MARK();
@@ -592,8 +670,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
             // merging CTA (split 0 of the kv head), which also appends it to the cache.
             const int nloc = n_old;
             const int nact = min(p.nsplit, (pos + KV_KEYS - 1) / KV_KEYS);      // splits holding at least one cached key
-            const bool merger = att_cta && att_sp == 0;                         // pos >= 1: split 0 always has cached keys
-            if (nloc > 0) {
+            if (nloc > 0) {                                                     // pos >= 1: split 0 always has cached keys
                 const int g = att_g;
                 float* qs = xs;                       // [group][128]
                 float* kn = qs + p.group * HD;        // [128]
@@ -810,7 +887,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
                             for (int u = 0; u < RB; ++u)
                                 if (u0 + u < nact) O = fmaf(__shfl_sync(0xffffffffu, f, u0 + u), __uint_as_float(ov[u].x), O);
                         }
-                        ll_store(p.attn_ll + (size_t)(g * p.group + hq) * HD + d, O / Lsum, tl | PH_ATTN);
+                        sx_store(sx_attn + (size_t)(g * p.group + hq) * HD + d, O / Lsum);
                     }
                 }
                 MEGA_FINE(31);
@@ -820,29 +897,29 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
         MEGA_MARK();
         // ---- phase 3: o_proj GEMV + residual ----
         MEGA_FINE(32);
-        ll_gather(p.attn_ll, QD, tl | PH_ATTN, xs);
+        sx_copy<QD>(sx_attn, xs);
         MEGA_FINE(33);
         MEGA_GT(2);
         cons_sync();
-        consume<QD, ME_RESID>(sl_o, ring, q, xs, p.x_ll, tl | PH_XO, xres, best_v, best_i, nullptr, 1.f, nullptr, part);
+        consume_ksplit<QD>(sl_o, ring, q, xs, sx_xo, xres, part);
         MEGA_FINE(34);
         MEGA_MARK();
         // ---- phase 4: RMSNorm + gate/up GEMV + SiLU*mul ----
         cons_sync();
         {
             MEGA_FINE(8); MEGA_FINE(9);
-            const float ss = ll_gather(p.x_ll, H, tl | PH_XO, xs); MEGA_FINE(10);
+            const float ss = sx_gather<H>(sx_xo, xs); MEGA_FINE(10);
             nr = norm_scale(ss, H, p.eps, red); MEGA_FINE(11);
         }
-        consume<H, ME_SWIGLU>(sl_gu, ring, q, xs, p.act_ll, tl | PH_ACT, xres, best_v, best_i, pb + H, nr, (dbg_row && l == 5) ? dbg_row + 440 : nullptr);
+        consume<H, ME_SWIGLU>(sl_gu, ring, q, xs, nullptr, 0u, sx_act, best_v, best_i, pb + H, nr, (dbg_row && l == 5) ? dbg_row + 440 : nullptr);
         MEGA_FINE(12);
         MEGA_FINE(13);
         MEGA_MARK();
         // ---- phase 5: down GEMV + residual ----
         MEGA_FINE(16); MEGA_FINE(17);
-        ll_gather(p.act_ll, I, tl | PH_ACT, xs); MEGA_FINE(18);
+        sx_copy<I>(sx_act, xs); MEGA_FINE(18);
         cons_sync();
-        consume<I, ME_RESID>(sl_dn, ring, q, xs, p.x_ll, tl | PH_XD, xres, best_v, best_i, nullptr, 1.f, nullptr, part);
+        consume_ksplit<I>(sl_dn, ring, q, xs, sx_xd, xres, part);
         MEGA_FINE(19);
         MEGA_FINE(20);
         MEGA_MARK();
@@ -852,11 +929,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     // ---- final RMSNorm + tied lm_head GEMV + argmax ----
     float nrf;
     {
-        const float ss = ll_gather(p.x_ll, H, (tag_base | ((uint32_t)(p.L - 1) << 3)) | PH_XD, xs);
+        const float ss = sx_gather<H>(sx_cur + (size_t)(p.L - 1) * SXL + H, xs);     // x_d of the last layer
         mbar_wait(&p_full[p.L & 1], (p.L >> 1) & 1);
         nrf = norm_scale(ss, H, p.eps, red);
     }
-    consume<H, ME_ARGMAX>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, xres, best_v, best_i,
+    consume<H, ME_ARGMAX>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i,
                           pbuf + (p.L & 1) * PARAM_FLOATS, nrf);
     MEGA_MARK();
     // candidates live in lanes 0, 8, 16, 24 of every warp (the four rows of a turn; lanes 0 / 16 in the two-row form):
@@ -907,6 +984,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
             tok_s = tok;
             p.bar[0] = 0;                        // every CTA has taken its ticket: reset for the next launch
             p.bar[1] = p.bar[1] + 1;             // new epoch: words published by this step can never match again
+            p.bar[3] = p.bar[3] + 1;             // executed launches of this kernel: the next one uses the other set
         }
         cons_sync();
         const int tok = tok_s;
@@ -955,16 +1033,20 @@ bool decode_mega_supported(const Model& m, int B, int ctx) {
 size_t decode_mega_part_floats(const Model& m) {
     const asrb_dims& c = m.d.c;
     const int group = c.num_attention_heads / c.num_key_value_heads;
-    const size_t words = (size_t)m.d.qkv_dim + (size_t)m.ctx->sm_count * group * mega::PSTRIDE + m.d.q_dim + c.hidden_size +
-                         c.intermediate_size + 64;
+    const size_t words = (size_t)m.d.qkv_dim + (size_t)m.ctx->sm_count * group * mega::PSTRIDE + 64;
     return 2 * words + 64;
+}
+// bytes of the self-validating exchange words: [2 sets][L][x_o H | x_d H | attn QD | act I] uint32
+size_t decode_mega_sx_bytes(const Model& m) {
+    const asrb_dims& c = m.d.c;
+    return 2 * (size_t)c.num_hidden_layers * (2 * (size_t)c.hidden_size + m.d.q_dim + c.intermediate_size) * sizeof(uint32_t);
 }
 
 void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* kcache, float* vcache,
                              size_t cache_layer_stride, size_t cache_seq_stride, int max_ctx, int ctx_now, const MegaBufs& mb,
                              cudaStream_t st, int64_t* launches) {
     ASRB_REQUIRE(decode_mega_supported(m, B, ctx_now), ASRB_ERR_STATE, "fused decode step not supported for this model/batch/context");
-    ASRB_REQUIRE(m.d_dec_layers && mb.bar && mb.part, ASRB_ERR_STATE, "fused decode step buffers missing");
+    ASRB_REQUIRE(m.d_dec_layers && mb.bar && mb.part && mb.sx_seq, ASRB_ERR_STATE, "fused decode step buffers missing");
     const asrb_dims& c = m.d.c;
     const int G = m.ctx->sm_count;
     const int group = c.num_attention_heads / c.num_key_value_heads;
@@ -978,7 +1060,8 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
     ASRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // The kernel handles one sequence.  A batch runs as B launches on the stream (weights are re-streamed per sequence:
     // 2.0 k tokens/s at any batch size, still ~1.8x the per-phase path at batch 8); a sequence that has finished
-    // returns at once.  Exchange buffers are shared: launches are serialised by the stream and tagged by epoch.
+    // returns at once.  Exchange buffers are shared: launches are serialised by the stream, the tagged words carry the
+    // epoch and the self-validating words switch sets with every executed launch.
     for (int sb = 0; sb < B; ++sb) {
         mega::Params p{};
         p.layers = m.d_dec_layers; p.lm_head = m.lm_head; p.embed = m.embed; p.final_norm = m.final_norm_sw;
@@ -994,13 +1077,12 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
         p.bar = mb.bar;
         uint2* w = reinterpret_cast<uint2*>(mb.part);            // 16-byte aligned sub-buffers (even word counts)
         p.qkv_ll = w; w += m.d.qkv_dim;
-        p.part_ll = w; w += (size_t)G * group * mega::PSTRIDE;
-        p.attn_ll = w; w += m.d.q_dim;
-        p.x_ll = w; w += c.hidden_size;
-        p.act_ll = w; w += c.intermediate_size;
+        p.part_ll = w;
+        p.sx = mb.sx_seq;
         p.dbg = mb.dbg;
         g_last_dbg = mb.dbg;
-        // tags must stay monotonic for red.max publication: long before the 24-bit epoch wraps, wipe the exchange buffers
+        // tags must stay monotonic for red.max publication: long before the 24-bit epoch wraps, wipe the tagged exchange
+        // buffers (the self-validating words live elsewhere and are left alone: to them 0 would be a published 0.0)
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {
             ASRB_CUDA_CHECK(cudaMemsetAsync(mb.part, 0, mb.part_bytes, st));
             const unsigned one = 1;

@@ -188,8 +188,10 @@ void launch_decode_step_phases(const Model& m, const DecodeBufs& b, int B, float
 // final-norm + lm_head + argmax on arbitrary rows of a residual stream (prefill last rows);
 // also performs the greedy bookkeeping of src/inference.rs:161-170 (EOS check, append, embed)
 struct MegaBufs { unsigned* bar = nullptr; float* part = nullptr; long long* dbg = nullptr; size_t part_bytes = 0; unsigned* steps_issued = nullptr;
-                  uint32_t* sx = nullptr; size_t sx_bytes = 0; int* sx_nb = nullptr; };   // sx: decode_batch.cu's self-validating words   // per-session state of the fused step
+                  uint32_t* sx = nullptr; size_t sx_bytes = 0; int* sx_nb = nullptr;   // sx: decode_batch.cu's self-validating words   // per-session state of the fused step
+                  uint32_t* sx_seq = nullptr; };   // decode_mega.cu's self-validating words (outside `part`: never wiped to 0)
 size_t decode_mega_part_floats(const Model& m);
+size_t decode_mega_sx_bytes(const Model& m);
 size_t decode_batch_part_floats(const Model& m);
 size_t decode_batch_sx_bytes(const Model& m);   // decode_batch.cu: NB sequences per fused launch
 bool decode_batch_supported(const Model& m, int B, int ctx);

@@ -1,5 +1,6 @@
 // mega_common.cuh -- device helpers shared by the fused decode steps (decode_mega.cu: one sequence per launch,
-// decode_batch.cu: NB sequences per launch): mbarrier / bulk-copy PTX, the tagged-word exchange, the weight ring.
+// decode_batch.cu: NB sequences per launch): mbarrier / bulk-copy PTX, the tagged and the self-validating exchange
+// words, the weight ring.
 #pragma once
 #include "internal.h"
 
@@ -20,8 +21,8 @@ static constexpr int PSTRIDE = HD + 2;                  // partial record: o[128
 static constexpr int DBG_SLOTS = 1024;
 static constexpr int MAX_SPLITS = 18;                   // 64-key attention splits per kv head (also bounded by SMs / kv heads: 16 for the 0.6B dims on 132 SMs)
 
-// phases (3 bits of the tag)
-enum { PH_QKV = 1, PH_PART = 2, PH_ATTN = 3, PH_XO = 4, PH_ACT = 5, PH_XD = 6 };
+// phases of the tagged words (3 bits of the tag)
+enum { PH_QKV = 1, PH_PART = 2 };
 
 // ---- PTX helpers ------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -71,11 +72,6 @@ __device__ __forceinline__ void ll_store(uint2* p, float v, uint32_t tag) {
     const unsigned long long val = ((unsigned long long)tag << 32) | (unsigned long long)__float_as_uint(v);
     asm volatile("red.relaxed.gpu.global.max.u64 [%0], %1;" ::"l"(p), "l"(val) : "memory");
 }
-__device__ __forceinline__ uint4 ll_load2(const uint2* p) {      // two consecutive words (16-byte aligned)
-    uint4 v;
-    asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-    return v;
-}
 __device__ __forceinline__ float ll_poll1(const uint2* p, uint32_t tag) {
     uint2 v;
     do {
@@ -96,47 +92,34 @@ __device__ __forceinline__ void ll_poll4(const uint2* p, int stride, uint32_t ta
 #pragma unroll
     for (int i = 0; i < 4; ++i) out[i] = __uint_as_float(v[i].x);
 }
+// ---- self-validating 4-byte exchange words (the all-to-all vectors: x after o_proj / down_proj, attention output,
+// SwiGLU activations).  A word is the fp32 value itself; 0xFFFFFFFF (a NaN pattern no result is ever published with)
+// means "not written yet".  Publication = one fire-and-forget red.and (performed at L2 at once, like red.max of the
+// tagged words); a gather polls 16-byte quads until none of the 4 words is the sentinel -- half the L2 traffic of
+// {value, tag} words, and that traffic (one CTA per SM x every vector) is what bounds the all-gathers.
+// Every (layer, vector) has its own region, and there are two such sets: step s uses set s & 1 and, at its start,
+// re-arms (stores the sentinel into) the words THIS CTA wrote into the other set during step s - 1.  The kernel
+// boundary orders that re-arm before any publication of step s + 1 into it, so a poll can only ever see the sentinel or
+// the current step's value.  Each kernel counts its own executed steps for the set parity.
+static constexpr uint32_t SX_EMPTY = 0xFFFFFFFFu;
+__device__ __forceinline__ void sx_store(uint32_t* p, float v) {
+    uint32_t b = __float_as_uint(v);
+    if (b == SX_EMPTY) b = 0x7FFFFFFFu;                   // (another NaN)
+    asm volatile("red.relaxed.gpu.global.and.b32 [%0], %1;" ::"l"(p), "r"(b) : "memory");
+}
+__device__ __forceinline__ uint4 sx_load4(const uint32_t* p) {
+    uint4 v;
+    asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ bool sx_ready(const uint4& v) {
+    return v.x != SX_EMPTY && v.y != SX_EMPTY && v.z != SX_EMPTY && v.w != SX_EMPTY;
+}
+
 // Activation vectors in shared memory are stored with 16-byte group k at k ^ ((k >> 3) & 1).  The GEMV register loads
 // read, per lane, the two groups of 8 consecutive elements (32-byte lane stride): unswizzled, lanes i and i+4 of every
 // quarter warp hit the same banks (2-way conflict on every LDS.128).
 __device__ __forceinline__ int xs_swz(int e) { const int k = e >> 2; return ((k ^ ((k >> 3) & 1)) << 2) | (e & 3); }
-// all consumer threads: gather n (even) tagged values into shared memory; returns this thread's sum of squares
-__device__ __forceinline__ float ll_gather(const uint2* buf, int n, uint32_t tag, float* xs) {
-    float ss = 0.f;
-    const int pairs = n >> 1;
-    constexpr int U = 8;                                           // independent 16-byte loads in flight per thread
-    for (int i0 = threadIdx.x; i0 < pairs; i0 += U * NCONS) {
-        uint4 v[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) v[u] = make_uint4(0u, 0u, 0u, 0u);      // tag 0 is never published (epochs start at 1)
-        bool ok;
-        do {
-            ok = true;
-            // only the pairs still missing are re-read (the registers themselves say which): every CTA reads every word, so
-            // a full re-poll costs n x 8 B x gridDim.x of L2 bandwidth per round -- 3.6 MB for the 3072 SwiGLU activations
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const int i = i0 + u * NCONS;
-                if (i < pairs && !(v[u].y == tag && v[u].w == tag)) v[u] = ll_load2(buf + 2 * i);
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const int i = i0 + u * NCONS;
-                if (i < pairs) ok = ok && (v[u].y == tag) && (v[u].w == tag);
-            }
-        } while (!ok);
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const int i = i0 + u * NCONS;
-            if (i < pairs) {
-                const float a = __uint_as_float(v[u].x), b = __uint_as_float(v[u].z);
-                *reinterpret_cast<float2*>(xs + xs_swz(2 * i)) = make_float2(a, b);
-                ss = fmaf(a, a, ss); ss = fmaf(b, b, ss);
-            }
-        }
-    }
-    return ss;
-}
 
 struct Ring {
     uint8_t* slots; uint64_t* full; uint64_t* empty;

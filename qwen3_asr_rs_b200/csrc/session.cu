@@ -199,6 +199,11 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
                 } else cudaGetLastError();
             }
         }
+        {   // single-sequence fused step (batch 1 included): self-validating exchange words, all "not written yet"
+            const size_t bytes = decode_mega_sx_bytes(*m);
+            s->mega.sx_seq = (uint32_t*)salloc<uint8_t>(s, bytes);
+            ASRB_CUDA_CHECK(cudaMemset(s->mega.sx_seq, 0xFF, bytes));
+        }
         if (getenv("ASRB_MEGA_DEBUG")) s->mega.dbg = salloc<long long>(s, decode_mega_dbg_slots(), true);
         ASRB_CUDA_CHECK(cudaMallocHost(&s->h_done, Bm * sizeof(int)));
         ASRB_CUDA_CHECK(cudaMallocHost(&s->h_nout, Bm * sizeof(int)));
