@@ -168,8 +168,19 @@ ASRB_API int asrb_session_device_ids(asrb_session* s, const int32_t** ids_dev, c
  * writes min(n, 5) values */
 ASRB_API int asrb_session_stats(asrb_session* s, int64_t* out, int n);
 /* knobs: "gemm" = "tc"|"simt", "decode" = "mega"|"phases", "batch_step" = "1"|"0", "planes" = "1"|"2"|"3",
- * "resident" = "1"|"0" (1: the samples uploaded by the previous call are reused, no H2D) */
+ * "resident" = "1"|"0" (1: the samples uploaded by the previous call are reused, no H2D),
+ * "logprobs" = "1"|"0" (1: every greedy step also records the log-probability of the token it selects, read with
+ * asrb_last_logprobs; same ids, same decode paths; the value in effect at the prefill applies to the whole run) */
 ASRB_API int asrb_session_set_option(asrb_session* s, const char* key, const char* value);
+
+/* Per-token log-probabilities of the last run (asrb_generate / asrb_transcribe_ids / asrb_transcribe_ingested, or
+ * asrb_prefill + asrb_decode_step), recorded when the option "logprobs" was "1" for its prefill and every step:
+ *   logprobs_out      [batch][max_new_tokens]: log p(ids[b][i]) = logit - logsumexp(logits) under the fp32 logits
+ *                     that selected the token (<= 0); NaN at and beyond lens_out[b]
+ *   eos_logprob_out   [batch] or NULL: the same for the EOS token that ended sequence b, NaN if it stopped at
+ *                     max_new_tokens
+ * Returns ASRB_ERR_STATE when the last run did not record them (option off, or switched after the prefill). */
+ASRB_API int asrb_last_logprobs(asrb_session* s, int max_new_tokens, float* logprobs_out, float* eos_logprob_out);
 
 /* debug (ASRB_MEGA_DEBUG=1): clock64 timeline of the last fused decode step, CTA 0 then CTA G-1;
  * returns the number of slots per CTA (0 if disabled) */

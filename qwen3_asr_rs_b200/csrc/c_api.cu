@@ -24,6 +24,7 @@ void session_transcribe_ids(Session* s, const float* const* samples, const int64
 void session_last_timings(Session* s, float* ms6, int64_t* kernels, int64_t* steps);
 void session_set_option(Session* s, const char* key, const char* value);
 void session_stats(Session* s, int64_t* out, int n);
+void session_last_logprobs(Session* s, int max_new_tokens, float* out, float* eos_out);
 void session_ingest_pcm(Session* s, const void* const* pcm, const int64_t* n_frames, const int32_t* channels, const int32_t* rate,
                         const int32_t* format, int batch, int64_t* n_samples_out);
 void session_ingested_read(Session* s, int b, float* out);
@@ -187,6 +188,9 @@ int asrb_session_stats(asrb_session* s, int64_t* out, int n) {
 }
 int asrb_session_set_option(asrb_session* s, const char* key, const char* value) {
     return guarded([&] { NONNULL(s); session_set_option(s->s, key, value); });
+}
+int asrb_last_logprobs(asrb_session* s, int max_new_tokens, float* logprobs_out, float* eos_logprob_out) {
+    return guarded([&] { NONNULL(s); NONNULL(logprobs_out); session_last_logprobs(s->s, max_new_tokens, logprobs_out, eos_logprob_out); });
 }
 
 int asrb_debug_mega_timeline(long long* out, int cap) {

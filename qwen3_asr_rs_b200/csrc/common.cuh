@@ -98,6 +98,20 @@ __device__ __forceinline__ float block_max(float v, float* scratch) {
     return r;
 }
 
+// ---- log-sum-exp partial records (max m, s = sum_j exp(l_j - m)) beside the greedy argmax ----------------
+// s rescaled from max m to max M >= m; an empty record (m = -inf, s = 0) stays 0, and m == M skips the exp
+__device__ __forceinline__ float lse_rescale(float s, float m, float M) { return m == M ? s : s * expf(m - M); }
+// fold logit v of `row` into a running (argmax, sum): strict > keeps the first maximum, as the plain argmax does
+__device__ __forceinline__ void lse_fold(float v, int row, float& best_v, int& best_i, float& best_s) {
+    if (v > best_v) { best_s = lse_rescale(best_s, best_v, v) + 1.f; best_v = v; best_i = row; }
+    else best_s += expf(v - best_v);
+}
+// merge two records (m, s), (om, os) into (max, rescaled sum); symmetric, so both lanes of a shuffle agree bitwise
+__device__ __forceinline__ float lse_merge(float m, float s, float om, float os) {
+    const float M = fmaxf(m, om);
+    return lse_rescale(s, m, M) + lse_rescale(os, om, M);
+}
+
 // order-preserving float <-> int key (for atomicMax on floats of either sign)
 __device__ __host__ __forceinline__ int float_to_ordered(float f) {
 #ifdef __CUDA_ARCH__

@@ -19,7 +19,8 @@
 namespace asrb {
 
 static constexpr int DG_THREADS = 256, DG_WARPS = 8;
-enum { DE_STORE = 0, DE_RESID = 1, DE_SWIGLU = 2, DE_ARGMAX = 3 };
+// DE_ARGMAX_LSE: DE_ARGMAX + per-CTA sum of exp(logit - max) (part_sum), the partial record of the token log-probability
+enum { DE_STORE = 0, DE_RESID = 1, DE_SWIGLU = 2, DE_ARGMAX = 3, DE_ARGMAX_LSE = 4 };
 
 struct GemvParams {
     const bf16* W; int N, K;
@@ -29,6 +30,7 @@ struct GemvParams {
     float* logits; int ldl;                         // ARGMAX: optional full logits
     float* part_val; int* part_idx;                 // ARGMAX: [B][gridDim.x]
     int B;
+    float* part_sum;                                // ARGMAX_LSE: [B][gridDim.x]
 };
 
 template <int MAXB, bool PRE_NORM, int EPI>
@@ -37,6 +39,7 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p) {
     __shared__ float red[32];
     __shared__ float bestv[DG_WARPS][MAXB];
     __shared__ int besti[DG_WARPS][MAXB];
+    constexpr bool ARGMAX = EPI == DE_ARGMAX || EPI == DE_ARGMAX_LSE, LSE = EPI == DE_ARGMAX_LSE;
     const int K = p.K, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     for (int b = 0; b < MAXB; ++b) {
         if (b < p.B) {
@@ -59,8 +62,9 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p) {
     const int per_cta = (units + gridDim.x - 1) / gridDim.x;
     const int u0 = blockIdx.x * per_cta, u1 = min(units, u0 + per_cta);
     float bv[MAXB]; int bi[MAXB];
+    float bs[LSE ? MAXB : 1];                     // LSE: sum of exp(logit - bv[b]) over this warp's rows
 #pragma unroll
-    for (int b = 0; b < MAXB; ++b) { bv[b] = -INFINITY; bi[b] = 0x7fffffff; }
+    for (int b = 0; b < MAXB; ++b) { bv[b] = -INFINITY; bi[b] = 0x7fffffff; if constexpr (LSE) bs[b] = 0.f; }
     for (int u = u0 + warp; u < u1; u += DG_WARPS) {
         float acc[RSTEP][MAXB];
 #pragma unroll
@@ -96,9 +100,10 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p) {
                 if (EPI == DE_STORE) p.out[(size_t)b * p.ldo + u] = acc[0][b];
                 if (EPI == DE_RESID) p.out[(size_t)b * p.ldo + u] += acc[0][b];
                 if (EPI == DE_SWIGLU) p.out[(size_t)b * p.ldo + u] = silu(acc[0][b]) * acc[RSTEP - 1][b];
-                if (EPI == DE_ARGMAX) {
+                if (ARGMAX) {
                     if (p.logits) p.logits[(size_t)b * p.ldl + u] = acc[0][b];
-                    if (acc[0][b] > bv[b]) { bv[b] = acc[0][b]; bi[b] = u; }   // rows ascend per warp: first max wins
+                    if constexpr (LSE) lse_fold(acc[0][b], u, bv[b], bi[b], bs[b]);
+                    else if (acc[0][b] > bv[b]) { bv[b] = acc[0][b]; bi[b] = u; }   // rows ascend per warp: first max wins
                 }
             }
         }
@@ -113,6 +118,22 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p) {
                 if (bestv[w][tid] > v || (bestv[w][tid] == v && besti[w][tid] < idx)) { v = bestv[w][tid]; idx = besti[w][tid]; }
             p.part_val[(size_t)tid * gridDim.x + blockIdx.x] = v;
             p.part_idx[(size_t)tid * gridDim.x + blockIdx.x] = idx;
+        }
+    }
+    if constexpr (LSE) {
+        __shared__ float bests[DG_WARPS][MAXB];
+        if (lane == 0)
+            for (int b = 0; b < MAXB; ++b) { bestv[warp][b] = bv[b]; besti[warp][b] = bi[b]; bests[warp][b] = bs[b]; }
+        __syncthreads();
+        if (tid < p.B) {
+            float v = -INFINITY; int idx = 0x7fffffff;
+            for (int w = 0; w < DG_WARPS; ++w)
+                if (bestv[w][tid] > v || (bestv[w][tid] == v && besti[w][tid] < idx)) { v = bestv[w][tid]; idx = besti[w][tid]; }
+            float sum = 0.f;                     // the warps' sums rescaled to the CTA maximum, in warp order
+            for (int w = 0; w < DG_WARPS; ++w) sum += lse_rescale(bests[w][tid], bestv[w][tid], v);
+            p.part_val[(size_t)tid * gridDim.x + blockIdx.x] = v;
+            p.part_idx[(size_t)tid * gridDim.x + blockIdx.x] = idx;
+            p.part_sum[(size_t)tid * gridDim.x + blockIdx.x] = sum;
         }
     }
 }
@@ -212,12 +233,16 @@ __global__ void __launch_bounds__(128) dec_attn_kernel(const float* __restrict__
 
 // ---------------------------------------------------------------------------------------------
 // greedy bookkeeping (inference.rs:161-170): finish the argmax, EOS check, append, embed.
+// LOGPROB: also merge the (max, sum of exponentials) records and store the selected token's log-probability in
+// lp_out (appended token) or eos_lp (EOS).
 // grid = B blocks.
 // ---------------------------------------------------------------------------------------------
+template <bool LOGPROB>
 __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __restrict__ part_idx, int n_part,
                               int* __restrict__ done, int* __restrict__ pos, int* __restrict__ next_id,
                               int* __restrict__ ids_out, int* __restrict__ n_out, int max_new,
-                              const bf16* __restrict__ embed, int hidden, float* __restrict__ x) {
+                              const bf16* __restrict__ embed, int hidden, float* __restrict__ x,
+                              const float* __restrict__ part_sum, float* __restrict__ lp_out, float* __restrict__ eos_lp) {
     __shared__ float sv[32];
     __shared__ int si[32];
     __shared__ int tok_s;
@@ -235,11 +260,34 @@ __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __r
     }
     if (lane == 0) { sv[warp] = v; si[warp] = idx; }
     __syncthreads();
+    float lp = 0.f;
+    if constexpr (LOGPROB) {
+        // S = sum_c s_c exp(m_c - M) over the n_part records, M = the maximum logit: each thread its records in index
+        // order, then a fixed tree over lanes and warps; logprob = -log S
+        __shared__ float ss[32];
+        const int nw = (blockDim.x + 31) / 32;
+        float M = sv[0];
+        for (int w = 1; w < nw; ++w) M = fmaxf(M, sv[w]);
+        float sum = 0.f;
+        for (int i = tid; i < n_part; i += blockDim.x) sum += lse_rescale(part_sum[(size_t)b * n_part + i], part_val[(size_t)b * n_part + i], M);
+        sum = warp_sum(sum);
+        if (lane == 0) ss[warp] = sum;
+        __syncthreads();
+        if (tid == 0) {
+            float S = 0.f;
+            for (int w = 0; w < nw; ++w) S += ss[w];
+            lp = -logf(S);
+        }
+    }
     if (tid == 0) {
         int nw = (blockDim.x + 31) / 32;
         for (int w = 1; w < nw; ++w)
             if (sv[w] > v || (sv[w] == v && si[w] < idx)) { v = sv[w]; idx = si[w]; }
         int tok = idx;
+        if constexpr (LOGPROB) {
+            if (tok == 151643 || tok == 151645) eos_lp[b] = lp;
+            else if (n_out[b] < max_new) lp_out[(size_t)b * max_new + n_out[b]] = lp;
+        }
         if (tok == 151643 || tok == 151645 || n_out[b] >= max_new) {   // EOS ids, inference.rs:154
             done[b] = 1; next_id[b] = -1; tok = -1;
         } else {
@@ -258,8 +306,12 @@ __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __r
 }
 
 void launch_greedy(const Model& m, const DecodeBufs& b, int B, cudaStream_t st, int64_t* launches) {
-    greedy_kernel<<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
-                                     b.max_new, m.embed, m.d.c.hidden_size, b.x);
+    if (b.logprobs)
+        greedy_kernel<true><<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
+                                               b.max_new, m.embed, m.d.c.hidden_size, b.x, b.part_sum, b.lp_out, b.eos_lp);
+    else
+        greedy_kernel<false><<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
+                                                b.max_new, m.embed, m.d.c.hidden_size, b.x, nullptr, nullptr, nullptr);
     ASRB_CUDA_CHECK(cudaGetLastError());
     if (launches) *launches += 1;
 }
@@ -270,6 +322,7 @@ static DecodeBufs offset_bufs(const DecodeBufs& b, int b0, const Model& m) {
     o.x = b.x + (size_t)b0 * c.hidden_size; o.qkv = b.qkv + (size_t)b0 * m.d.qkv_dim; o.attn = b.attn + (size_t)b0 * m.d.q_dim;
     o.act = b.act + (size_t)b0 * c.intermediate_size; o.logits = b.logits ? b.logits + (size_t)b0 * c.vocab_size : nullptr;
     o.part_val = b.part_val + (size_t)b0 * b.n_part; o.part_idx = b.part_idx + (size_t)b0 * b.n_part;
+    o.part_sum = b.part_sum ? b.part_sum + (size_t)b0 * b.n_part : nullptr;
     o.pos = b.pos + b0; o.done = b.done + b0; o.next_id = b.next_id + b0; o.ids_out = b.ids_out + (size_t)b0 * b.max_new; o.n_out = b.n_out + b0;
     return o;
 }
@@ -286,7 +339,8 @@ void launch_lmhead_argmax(const Model& m, const float* x_rows, const int* d_row_
         p.norm_w = m.final_norm; p.eps = (float)c.rms_norm_eps;
         p.logits = write_logits ? ob.logits : nullptr; p.ldl = c.vocab_size;
         p.part_val = ob.part_val; p.part_idx = ob.part_idx; p.B = nb;
-        run_gemv<true, DE_ARGMAX>(p, b.n_part, st);
+        if (b.logprobs) { p.part_sum = ob.part_sum; run_gemv<true, DE_ARGMAX_LSE>(p, b.n_part, st); }
+        else run_gemv<true, DE_ARGMAX>(p, b.n_part, st);
         if (launches) *launches += 1;
     }
 }

@@ -57,6 +57,10 @@ struct Params {
     uint32_t* sx;                        // self-validating 4-byte words [2 sets][L][XO | XD | ATTN | ACT][NB][rows]
     long long* dbg;              // optional timeline [2][DBG_SLOTS] of clock64 (CTA 0 and CTA G-1), else null
     int flags;                   // bit 0: L2 prefetch of the next layer's K/V tiles
+    // LOGPROB instantiations only (appended: the offsets above stay those of the default instantiations)
+    float* part_sum;             // [nb][n_part] sum of exp(logit - part_val) over the CTA's lm_head rows
+    float* lp_out;               // [nb][max_new] log-probability of each appended token
+    float* eos_lp;               // [nb] log-probability of the EOS token that ends the sequence
 };
 
 __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
@@ -147,7 +151,9 @@ __device__ __forceinline__ void head_norm_rope_b(const uint2* __restrict__ src, 
 
 enum { BE_STORE = 0, BE_SWIGLU = 1, BE_ARGMAX = 2 };
 
-template <int H, int QD, int I, int NB, int NS, int KVK>
+// LOGPROB: the lm_head also keeps (max, sum of exponentials) per (tile row, sequence), and the last CTA records the
+// log-probability of each selected token (p.lp_out / p.eos_lp)
+template <int H, int QD, int I, int NB, int NS, int KVK, bool LOGPROB>
 __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params p) {   // 9 warps are allocated as 12 (granularity 4): 168 registers
     static_assert(NB % 8 == 0 && NB <= 16, "NB must be 8 or 16");
     static_assert(H % 256 == 0 && QD % H == 0 && I % H == 0, "chunking needs QD, I multiples of H, H multiple of 256");
@@ -290,6 +296,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
         xres[b * MAXROWS + r] = __ldcg(p.x + (size_t)b * H + xsl.r0 + r);
     }
     float best_v = -INFINITY; int best_i = 0x7fffffff;      // lm_head: running argmax of (tile row tid / NB, sequence tid % NB)
+    float best_s = 0.f;                                      // LOGPROB: its sum of exp(logit - best_v)
     // merging CTA: which (sequence, kv head), and which record slots will be written for it -- slot u holds a record iff a
     // run starts at split u, i.e. u == 0 or item base + u opens its owner's range.  Positions do not change within the
     // step, so this is computed once, not per layer (the owner search is a dozen integer divisions per slot).
@@ -482,6 +489,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
                     } else if (epi == BE_SWIGLU) {
                         const float up = __shfl_down_sync(0xffffffffu, v, NB);     // rows 2j (gate) and 2j + 1 (up): NB threads apart
                         if (valid && !(rr & 1)) sx_store(sxo + (size_t)sq * I + (row >> 1), silu(v) * up);
+                    } else if constexpr (LOGPROB) {
+                        if (valid) lse_fold(v, row, best_v, best_i, best_s);      // rows ascend per thread: ties keep the first
                     } else {
                         if (valid && (v > best_v || (v == best_v && row < best_i))) { best_v = v; best_i = row; }
                     }
@@ -791,7 +800,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
     MARK();
     // every thread tid < 16 NB holds the best row of (tile row tid / NB, sequence tid % NB): merge the 16 tile rows per sequence
     cons_sync();
-    if (tid < 16 * NB) { bestv[tid] = best_v; besti[tid] = best_i; }
+    // LOGPROB: the sums go to the activation planes, which nothing reads once the lm_head tiles are contracted
+    float* bests = xs;                                       // [16 rows][NB]
+    if (tid < 16 * NB) { bestv[tid] = best_v; besti[tid] = best_i; if constexpr (LOGPROB) bests[tid] = best_s; }
     cons_sync();
     int& is_last = misc[0];
     if (tid < nb) {
@@ -801,6 +812,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
             if (cv > v || (cv == v && ci < idx)) { v = cv; idx = ci; }
         }
         p.part_val[(size_t)tid * p.n_part + blockIdx.x] = v; p.part_idx[(size_t)tid * p.n_part + blockIdx.x] = idx;
+        if constexpr (LOGPROB) {                             // the 16 tile rows' sums rescaled to the CTA maximum, in row order
+            float sum = 0.f;
+            for (int wq = 0; wq < 16; ++wq) sum += lse_rescale(bests[wq * NB + tid], bestv[wq * NB + tid], v);
+            p.part_sum[(size_t)tid * p.n_part + blockIdx.x] = sum;
+        }
         __threadfence();
     }
     cons_sync();
@@ -827,6 +843,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
         }
         int tok = idx;
         const int n = p.n_out[b];
+        if constexpr (LOGPROB) {
+            // S = sum_c s_c exp(m_c - M) over the G records (M = v, the maximum: every lane holds it after the butterfly),
+            // each lane its records in index order, then a fixed butterfly; logprob = -log S
+            float sum = 0.f;
+            for (int i = lane; i < (int)G; i += 32)
+                sum += lse_rescale(__ldcg(p.part_sum + (size_t)b * p.n_part + i), __ldcg(p.part_val + (size_t)b * p.n_part + i), v);
+            const float lp = -logf(warp_sum(sum));
+            if (lane == 0) {
+                if (tok == 151643 || tok == 151645) p.eos_lp[b] = lp;
+                else if (n < p.max_new) p.lp_out[(size_t)b * p.max_new + n] = lp;
+            }
+        }
         if (tok == 151643 || tok == 151645 || n >= p.max_new) {
             if (lane == 0) { p.done[b] = 1; p.next_id[b] = -1; }
             tok = -1;
@@ -913,12 +941,20 @@ void launch_decode_step_batch(const Model& m, const DecodeBufs& b, int B, float*
         const BatchCfg k = batch_cfg(nb);
         const size_t smem = batch_smem_bytes(c.hidden_size, k);
         const void* fn = nullptr;
-        if (bdims_match<1024, 2048, 3072>(c))
-            fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64>
-                           : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64>;
+        if (b.logprobs) {
+            if (bdims_match<1024, 2048, 3072>(c))
+                fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, true>
+                               : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, true>;
+            else
+                fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, true>
+                               : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, true>;
+        }
+        else if (bdims_match<1024, 2048, 3072>(c))
+            fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, false>
+                           : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, false>;
         else
-            fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64>
-                           : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64>;
+            fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, false>
+                           : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, false>;
         ASRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         megab::Params p{};
         p.layers = m.d_dec_layers_b; p.lm_head = m.lm_head_b; p.embed = m.embed; p.final_norm = m.final_norm;
@@ -942,6 +978,9 @@ void launch_decode_step_batch(const Model& m, const DecodeBufs& b, int B, float*
         }
         p.dbg = mb.dbg;
         g_last_dbg_batch = mb.dbg;
+        if (b.logprobs) {
+            p.part_sum = b.part_sum + (size_t)b0 * b.n_part; p.lp_out = b.lp_out + (size_t)b0 * b.max_new; p.eos_lp = b.eos_lp + b0;
+        }
         { static const int fl = getenv("ASRB_BATCH_FLAGS") ? atoi(getenv("ASRB_BATCH_FLAGS")) : 0; p.flags = fl; }   // bit 0 (K/V L2 prefetch): measured slower, off
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {   // tags must stay monotonic: wipe long before the epoch wraps
             ASRB_CUDA_CHECK(cudaMemsetAsync(mb.part, 0, mb.part_bytes, st));

@@ -51,6 +51,10 @@ struct Params {
     uint2* qkv_ll; uint2* part_ll;      // tagged exchange buffers ({value, tag} words)
     uint32_t* sx;                // self-validating words [2 sets][L][x_o H | x_d H | attn QD | act I]
     long long* dbg;              // optional timeline [2][DBG_SLOTS] of clock64 (CTA 0 and CTA G-1), else null
+    // LOGPROB instantiations only (appended: the offsets above stay those of the default instantiations)
+    float* part_sum;             // [gridDim.x] sum of exp(logit - part_val) over the CTA's lm_head rows
+    float* lp_out;               // [max_new] log-probability of each appended token
+    float* eos_lp;               // log-probability of the EOS token that ends the sequence
 };
 
 static_assert(KV_KEYS * HD * 4 == SLOT_BYTES, "K / V tiles travel through the weight ring: one tile per slot");
@@ -265,9 +269,9 @@ __device__ __forceinline__ void consume_ksplit(const Slice& s, const Ring& ring,
 }
 
 // K <= 1024 GEMVs (qkv, gate/up, lm_head of the 0.6B dims): four rows per warp and turn, two ring slots (32 rows) per turn.
-template <int K, int EPI>
+template <int K, int EPI, bool LOGPROB>
 __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
-                                             uint32_t tag, uint32_t* sxo, float& best_v, int& best_i,
+                                             uint32_t tag, uint32_t* sxo, float& best_v, int& best_i, float& best_s,
                                              const float* norm_w, float norm_r, long long* fine) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int fi = 0;
@@ -307,6 +311,8 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
                 if ((lane & 15) == 0 && j < nv) sx_store(sxo + (row >> 1), silu(v) * up);
             } else if (EPI == ME_STORE) {
                 if ((lane & 7) == 0 && j < nv) ll_store(out + row, v, tag);
+            } else if constexpr (LOGPROB) {        // ME_ARGMAX + running sum of exponentials (the lanes that keep best_v)
+                if ((lane & 7) == 0 && j < nv) lse_fold(v, row, best_v, best_i, best_s);
             } else {                               // ME_ARGMAX: rows arrive in increasing order per lane, strict > keeps the first maximum
                 if ((lane & 7) == 0 && j < nv && v > best_v) { best_v = v; best_i = row; }
             }
@@ -322,12 +328,12 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
 
 // consumer: process all chunks of a slice.  `xs` holds the (already normalised) activation vector.
 // Results are published as tagged words to `out` (ME_STORE), as self-validating words to `sxo` (ME_SWIGLU), or folded
-// into the running argmax (ME_ARGMAX).
-template <int K, int EPI>
+// into the running argmax (ME_ARGMAX; with LOGPROB also into the running sum of exponentials `best_s`).
+template <int K, int EPI, bool LOGPROB = false>
 __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
-                                        uint32_t tag, uint32_t* sxo, float& best_v, int& best_i,
+                                        uint32_t tag, uint32_t* sxo, float& best_v, int& best_i, float& best_s,
                                         const float* norm_w = nullptr, float norm_r = 1.f, long long* fine = nullptr) {
-    if constexpr (K <= 1024) { consume_quad<K, EPI>(s, ring, q, xs, out, tag, sxo, best_v, best_i, norm_w, norm_r, fine); return; }
+    if constexpr (K <= 1024) { consume_quad<K, EPI, LOGPROB>(s, ring, q, xs, out, tag, sxo, best_v, best_i, best_s, norm_w, norm_r, fine); return; }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int fi = 0;
 #define CF() do { if (fine && threadIdx.x == 0 && fi < 24) fine[fi++] = clock64(); } while (0)
@@ -386,6 +392,8 @@ __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32
                 }
                 if (EPI == ME_STORE) {
                     if (act) ll_store(out + row, v0, tag);
+                } else if constexpr (LOGPROB) {
+                    if (act) lse_fold(v0, row, best_v, best_i, best_s);
                 } else {
                     if (act && v0 > best_v) { best_v = v0; best_i = row; }
                 }
@@ -504,7 +512,9 @@ __device__ __forceinline__ void head_norm_rope(const uint2* __restrict__ src, ui
         if (dbg_row && tid == 0 && dbg_i < DBG_SLOTS) dbg_row[dbg_i++] = clock64();                    \
     } while (0)
 
-template <int H, int QD, int I, int NS>
+// LOGPROB: the lm_head also keeps (max, sum of exponentials) per lane, and the last CTA records the log-probability of
+// the selected token (p.lp_out / p.eos_lp)
+template <int H, int QD, int I, int NS, bool LOGPROB>
 __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p) {
     constexpr int XS_FLOATS = (I > XS_MIN ? I : XS_MIN) + 64;
     extern __shared__ __align__(128) uint8_t smem[];
@@ -633,6 +643,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     const float* sn = ropes + half;
     const unsigned G = gridDim.x;
     float best_v = -INFINITY; int best_i = 0x7fffffff;
+    float best_s = 0.f;                               // LOGPROB: sum of exp(logit - best_v) over the rows this lane folded
     // tag = launch epoch (unique per executed step, survives new utterances that revisit the same positions)
     const unsigned epoch = __ldcg(p.bar + 1);
     const uint32_t tag_base = (epoch & 0xffffffu) << 8;
@@ -659,7 +670,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
             nr = norm_scale(ss, H, p.eps, red);
             MEGA_FINE(3);
         }
-        consume<H, ME_STORE>(sl_qkv, ring, q, xs, p.qkv_ll, tl | PH_QKV, nullptr, best_v, best_i, pb, nr);
+        consume<H, ME_STORE>(sl_qkv, ring, q, xs, p.qkv_ll, tl | PH_QKV, nullptr, best_v, best_i, best_s, pb, nr);
         MEGA_FINE(4);
         MEGA_GT(0);
         MEGA_MARK();
@@ -911,7 +922,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
             const float ss = sx_gather<H>(sx_xo, xs); MEGA_FINE(10);
             nr = norm_scale(ss, H, p.eps, red); MEGA_FINE(11);
         }
-        consume<H, ME_SWIGLU>(sl_gu, ring, q, xs, nullptr, 0u, sx_act, best_v, best_i, pb + H, nr, (dbg_row && l == 5) ? dbg_row + 440 : nullptr);
+        consume<H, ME_SWIGLU>(sl_gu, ring, q, xs, nullptr, 0u, sx_act, best_v, best_i, best_s, pb + H, nr, (dbg_row && l == 5) ? dbg_row + 440 : nullptr);
         MEGA_FINE(12);
         MEGA_FINE(13);
         MEGA_MARK();
@@ -933,18 +944,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
         mbar_wait(&p_full[p.L & 1], (p.L >> 1) & 1);
         nrf = norm_scale(ss, H, p.eps, red);
     }
-    consume<H, ME_ARGMAX>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i,
-                          pbuf + (p.L & 1) * PARAM_FLOATS, nrf);
+    consume<H, ME_ARGMAX, LOGPROB>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i, best_s,
+                                   pbuf + (p.L & 1) * PARAM_FLOATS, nrf);
     MEGA_MARK();
     // candidates live in lanes 0, 8, 16, 24 of every warp (the four rows of a turn; lanes 0 / 16 in the two-row form):
     // merge them, lane 0 publishes the warp's best
 #pragma unroll
     for (int o = 8; o <= 16; o <<= 1) {
         const float ov = __shfl_xor_sync(0xffffffffu, best_v, o); const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
+        if constexpr (LOGPROB) best_s = lse_merge(best_v, best_s, ov, __shfl_xor_sync(0xffffffffu, best_s, o));
         if (ov > best_v || (ov == best_v && oi < best_i)) { best_v = ov; best_i = oi; }
     }
     cons_sync();
-    if (lane == 0) { red[warp] = best_v; ired[warp] = best_i; }
+    if (lane == 0) { red[warp] = best_v; ired[warp] = best_i; if constexpr (LOGPROB) red[NCONS_WARPS + warp] = best_s; }
     cons_sync();
     int& is_last = ired[63];
     if (tid == 0) {
@@ -952,6 +964,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
         for (int wq = 0; wq < NCONS_WARPS; ++wq)
             if (red[wq] > v || (red[wq] == v && ired[wq] < idx)) { v = red[wq]; idx = ired[wq]; }
         p.part_val[blockIdx.x] = v; p.part_idx[blockIdx.x] = idx;
+        if constexpr (LOGPROB) {             // the warps' sums rescaled to the CTA maximum, in warp order
+            float sum = 0.f;
+            for (int wq = 0; wq < NCONS_WARPS; ++wq) sum += lse_rescale(red[NCONS_WARPS + wq], red[wq], v);
+            p.part_sum[blockIdx.x] = sum;
+        }
         __threadfence();
         unsigned t = atomicAdd(p.bar, 1u);
         is_last = (t == G - 1);
@@ -973,12 +990,33 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
         }
         if (lane == 0) { red[warp] = v; ired[warp] = idx; }
         cons_sync();
+        float lp = 0.f;
+        if constexpr (LOGPROB) {
+            // S = sum_c s_c exp(m_c - M) over the G records, M = the step's maximum logit (= that of the selected token):
+            // each thread its records in index order, then the warps in a fixed tree; logprob = -log S
+            float M = red[0];
+            for (int wq = 1; wq < NCONS_WARPS; ++wq) M = fmaxf(M, red[wq]);
+            float sum = 0.f;
+            for (int i = tid; i < (int)G; i += NCONS) sum += lse_rescale(__ldcg(p.part_sum + i), __ldcg(p.part_val + i), M);
+            sum = warp_sum(sum);
+            if (lane == 0) red[NCONS_WARPS + warp] = sum;
+            cons_sync();
+            if (tid == 0) {
+                float S = 0.f;
+                for (int wq = 0; wq < NCONS_WARPS; ++wq) S += red[NCONS_WARPS + wq];
+                lp = -logf(S);
+            }
+        }
         int& tok_s = ired[62];
         if (tid == 0) {
             for (int wq = 1; wq < NCONS_WARPS; ++wq)
                 if (red[wq] > v || (red[wq] == v && ired[wq] < idx)) { v = red[wq]; idx = ired[wq]; }
             int tok = idx;
             const int n = *p.n_out;
+            if constexpr (LOGPROB) {
+                if (tok == 151643 || tok == 151645) *p.eos_lp = lp;
+                else if (n < p.max_new) p.lp_out[n] = lp;
+            }
             if (tok == 151643 || tok == 151645 || n >= p.max_new) { *p.done = 1; *p.next_id = -1; tok = -1; }
             else { p.ids_out[n] = tok; *p.n_out = n + 1; *p.pos = pos + 1; *p.next_id = tok; }
             tok_s = tok;
@@ -1054,9 +1092,14 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
     const int nsplit = std::min(mega::MAX_SPLITS, std::min(G / c.num_key_value_heads, (max_ctx + mega::KV_KEYS - 1) / mega::KV_KEYS));
     const size_t smem = mega_smem_bytes(c.hidden_size, c.intermediate_size, mega_nslot(c));
     const void* fn = nullptr;
-    if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6>;          // Qwen3-ASR-0.6B
-    else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5>;     // Qwen3-ASR-1.7B
-    else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6>;                                             // test config
+    if (b.logprobs) {
+        if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, true>;
+        else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, true>;
+        else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, true>;
+    }
+    else if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, false>;   // Qwen3-ASR-0.6B
+    else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, false>;   // Qwen3-ASR-1.7B
+    else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, false>;                                           // test config
     ASRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // The kernel handles one sequence.  A batch runs as B launches on the stream (weights are re-streamed per sequence:
     // 2.0 k tokens/s at any batch size, still ~1.8x the per-phase path at batch 8); a sequence that has finished
@@ -1081,6 +1124,7 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
         p.sx = mb.sx_seq;
         p.dbg = mb.dbg;
         g_last_dbg = mb.dbg;
+        if (b.logprobs) { p.part_sum = b.part_sum; p.lp_out = b.lp_out + (size_t)sb * b.max_new; p.eos_lp = b.eos_lp + sb; }
         // tags must stay monotonic for red.max publication: long before the 24-bit epoch wraps, wipe the tagged exchange
         // buffers (the self-validating words live elsewhere and are left alone: to them 0 would be a published 0.0)
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {

@@ -181,6 +181,11 @@ struct DecodeBufs {
     int* ids_out;    // [B][max_new]
     int* n_out;      // [B]
     int max_new;
+    // per-token log-probabilities (session option "logprobs"): buffers allocated when the option is first enabled
+    bool logprobs;   // launch the LOGPROB kernel variants
+    float* part_sum; // [B][n_part] sum of exp(logit - part_val) per argmax partial
+    float* lp_out;   // [B][max_new] log-probability of each appended token
+    float* eos_lp;   // [B] log-probability of the EOS token that ended the sequence (NaN until then)
 };
 void launch_decode_step_phases(const Model& m, const DecodeBufs& b, int B, float* kcache, float* vcache,
                                size_t cache_layer_stride, size_t cache_seq_stride, int max_ctx,

@@ -5,6 +5,7 @@
 // by small index arrays uploaded once per call.
 #include <algorithm>
 #include <cstring>
+#include <limits>
 #include "internal.h"
 
 namespace asrb {
@@ -73,6 +74,9 @@ struct Session {
     std::vector<int64_t> ingested_n;    // 16 kHz samples per utterance produced by the last asrb_ingest_pcm (empty: none pending)
     int64_t launches = 0, decode_steps = 0;
     int greedy_done = 0;   // greedy applications since prefill (tokens appended or EOS), bounds max_new
+    // per-token log-probabilities: option "logprobs" (db.logprobs selects the kernel variants); lp_valid = the prefill
+    // and every step since ran with it on, i.e. db.lp_out / db.eos_lp describe the current run
+    bool lp_valid = false;
     ~Session();
 };
 
@@ -442,6 +446,11 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.pos, di + (pos0 - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
     ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.done, 0, B * sizeof(int), st));
     ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.n_out, 0, B * sizeof(int), st));
+    s->lp_valid = s->db.logprobs;          // latched here: a run records log-probabilities only if it starts with the option on
+    if (s->db.logprobs) {                  // all NaN (0xFFFFFFFF): no EOS seen, nothing appended
+        ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.eos_lp, 0xFF, B * sizeof(float), st));
+        ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.lp_out, 0xFF, (size_t)B * s->max_new * sizeof(float), st));
+    }
 
     launch_embed_inject(m.embed, c.hidden_size, s->d_ids, s->d_audio_row, s->audio, totS, s->hid, st);
     s->launches += 1;
@@ -537,6 +546,7 @@ void session_decode_step(Session* s, int64_t* next_ids_out, float* logits) {
     ASRB_REQUIRE(s->stage >= 3, ASRB_ERR_STATE, "decode_step called before prefill");
     Model& m = *s->m; const int B = s->B;
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
+    s->lp_valid = s->lp_valid && s->db.logprobs;
     // the id selected by the previous greedy application is the one this iteration consumes
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->h_next, s->db.next_id, B * sizeof(int), cudaMemcpyDeviceToHost, s->st));
     forward_step(s, logits != nullptr);
@@ -551,12 +561,13 @@ void session_generate(Session* s, int max_new_tokens, int32_t* ids_out, int32_t*
     ASRB_REQUIRE(max_new_tokens >= 1 && max_new_tokens <= s->max_new, ASRB_ERR_INVALID, "max_new_tokens exceeds session capacity");
     Model& m = *s->m; const int B = s->B; cudaStream_t st = s->st;
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
+    s->lp_valid = s->lp_valid && s->db.logprobs;     // switched off after the prefill: this run's record is incomplete
     // Token 0 was selected at the end of prefill; each further token costs one forward + greedy.  The
     // reference also runs `forward` after the last appended token and discards its logits
     // (inference.rs:160-200); that wasted forward is not issued here.
     const int steps = std::max(0, max_new_tokens - s->greedy_done);
     auto ensure_graph = [&]() {   // per-phase path: ~142 launches per step -> replay them as one CUDA graph
-        const int mode_key = s->decode_mode * (s->max_batch + 1) + B;     // unique per (mode, batch)
+        const int mode_key = ((int)s->db.logprobs * 2 + s->decode_mode) * (s->max_batch + 1) + B;     // unique per (logprobs, mode, batch)
         if (s->step_graph == nullptr || s->graph_mode != mode_key) {
             if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
             cudaGraph_t g = nullptr;
@@ -630,6 +641,27 @@ void session_device_ids(Session* s, const int32_t** ids, const int32_t** lens, i
     *ids = s->db.ids_out; *lens = s->db.n_out; *stride = s->max_new; *batch = s->B;
 }
 
+// log-probabilities of the last run (prefill + generate / decode steps): [batch][max_new_tokens], NaN at and beyond the
+// sequence's length; eos_out[b] = that of the EOS token that ended sequence b, NaN if it did not end on EOS
+void session_last_logprobs(Session* s, int max_new_tokens, float* out, float* eos_out) {
+    ASRB_REQUIRE(s->stage >= 3 && s->lp_valid, ASRB_ERR_STATE,
+                 "last_logprobs: the last run did not record log-probabilities (set option logprobs=1 before the prefill)");
+    ASRB_REQUIRE(max_new_tokens >= 1, ASRB_ERR_INVALID, "max_new_tokens must be >= 1");
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    const int B = s->B;
+    std::vector<float> lp((size_t)B * s->max_new), eos((size_t)B);
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->h_nout, s->db.n_out, B * sizeof(int), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(lp.data(), s->db.lp_out, lp.size() * sizeof(float), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(eos.data(), s->db.eos_lp, eos.size() * sizeof(float), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    const float nan = std::numeric_limits<float>::quiet_NaN();
+    for (int b = 0; b < B; ++b) {
+        const int n = std::min(s->h_nout[b], max_new_tokens);
+        for (int i = 0; i < max_new_tokens; ++i) out[(size_t)b * max_new_tokens + i] = i < n ? lp[(size_t)b * s->max_new + i] : nan;
+        if (eos_out) eos_out[b] = eos[b];
+    }
+}
+
 void session_stats(Session* s, int64_t* out, int n) {
     const int64_t v[5] = {s->n_batch_steps, s->n_mega_steps, s->n_phase_steps, g_gemm_simt_fallbacks.load(), g_gemm_tc_launches.load()};
     for (int i = 0; i < n && i < 5; ++i) out[i] = v[i];
@@ -652,6 +684,16 @@ void session_set_option(Session* s, const char* key, const char* value) {
         s->nplanes = p;
     } else if (k == "resident") {
         s->resident = (v == "1");
+    } else if (k == "logprobs") {
+        ASRB_REQUIRE(v == "1" || v == "0", ASRB_ERR_INVALID, "logprobs must be 1|0");
+        DecodeBufs& b = s->db;
+        if (v == "1" && !b.lp_out) {      // first enabled: a session that never records keeps its allocations unchanged
+            ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+            b.part_sum = salloc<float>(s, (size_t)s->max_batch * b.n_part);
+            b.lp_out = salloc<float>(s, (size_t)s->max_batch * s->max_new);
+            b.eos_lp = salloc<float>(s, s->max_batch);
+        }
+        b.logprobs = (v == "1");
     } else throw Error(ASRB_ERR_INVALID, "unknown option: " + k);
 }
 

@@ -42,12 +42,21 @@ def _dims_struct(cfg: AsrConfig) -> _lib.AsrbDims:
     return d
 
 
+def avg_logprob(token_logprobs: Sequence[float], eos_logprob: Optional[float]) -> Optional[float]:
+    """Mean log-probability of an utterance: over the generated tokens, plus the EOS token when generation ended on it
+    (Whisper's `avg_logprob`); None when there is nothing to average."""
+    vals = list(token_logprobs) + ([eos_logprob] if eos_logprob is not None else [])
+    return sum(vals) / len(vals) if vals else None
+
+
 @dataclass
 class TranscribeResult:           # inference.rs:270-274
     text: str
     language: str
     raw_output: str
     ids: List[int]
+    token_logprobs: Optional[List[float]] = None    # transcribe(logprobs=True): log p of each id
+    avg_logprob: Optional[float] = None             # avg_logprob(token_logprobs, EOS log p)
 
 
 @dataclass
@@ -56,6 +65,8 @@ class TranscribeIds:
     stage_ms: Dict[str, float]    # device time per stage (CUDA events)
     kernels_launched: int
     decode_steps: int
+    logprobs: Optional[List[List[float]]] = None         # logprobs=True: natural-log probability of each id
+    eos_logprobs: Optional[List[Optional[float]]] = None  # ... of the EOS id that ended the utterance (None: stopped at max_new_tokens)
 
 
 class AsrInference:
@@ -200,24 +211,61 @@ class AsrInference:
                 mx = max(mx, len(a))
         return keep, (C.POINTER(C.c_int64) * batch)(*ptrs), (C.c_int32 * batch)(*lens), mx
 
+    # ---- per-token log-probabilities (session option "logprobs") ----------------------------
+    def _record_logprobs(self, s, on: bool) -> None:
+        """Switch recording on for one call (True) or back to the engine's configured value (False)."""
+        if self._options.get("logprobs") != "1":
+            _lib.check(self._lib.asrb_session_set_option(s, b"logprobs", b"1" if on else b"0"))
+
+    def last_logprobs(self, max_new_tokens: int):
+        """asrb_last_logprobs: (per-utterance log-probabilities of the ids of the last run, EOS log-probability or None).
+        Raises AsrbError (ASRB_ERR_STATE) when the last run did not record them."""
+        if self._session is None:
+            raise _lib.AsrbError(4, "no session: nothing has run yet")
+        cap = self._cap[0]                                   # the library writes one row per utterance of the last run
+        lp = np.full((cap, max_new_tokens), np.nan, dtype=np.float32)
+        eos = np.full(cap, np.nan, dtype=np.float32)
+        _lib.check(self._lib.asrb_last_logprobs(self._session, int(max_new_tokens), lp.ctypes.data_as(C.POINTER(C.c_float)),
+                                                eos.ctypes.data_as(C.POINTER(C.c_float))))
+        B = getattr(self, "_B", cap)
+        rows = []
+        for r in lp[:B]:                                     # each row: the finite prefix (NaN from the utterance's length on)
+            nan = np.flatnonzero(np.isnan(r))
+            rows.append([float(v) for v in r[: nan[0] if len(nan) else len(r)]])
+        return rows, [None if np.isnan(e) else float(e) for e in eos[:B]]
+
+    def _finish(self, s, B: int, ids, n, max_new_tokens: int, logprobs: bool) -> TranscribeIds:
+        ms = (C.c_float * 6)()
+        k, st = C.c_int64(), C.c_int64()
+        _lib.check(self._lib.asrb_last_timings(s, ms, C.byref(k), C.byref(st)))
+        names = ("h2d", "mel", "encoder", "prefill", "decode", "total")
+        r = TranscribeIds([ids[b, : n[b]].tolist() for b in range(B)], dict(zip(names, ms)), k.value, st.value)
+        self._B = B
+        if logprobs:
+            r.logprobs, r.eos_logprobs = self.last_logprobs(max_new_tokens)
+        return r
+
     # ---- the hot path ----------------------------------------------------------------
     def transcribe_ids(self, clips: Sequence[np.ndarray], language_ids: Optional[Sequence] = None,
-                       max_new_tokens: int = MAX_NEW_TOKENS) -> TranscribeIds:
-        """transcribe() steps 2-8 for a batch: host f32 samples in, host token ids out."""
+                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False) -> TranscribeIds:
+        """transcribe() steps 2-8 for a batch: host f32 samples in, host token ids out (and, with `logprobs`, the
+        log-probability of every id and of the ending EOS, from the kernels that selected them)."""
         B = len(clips)
         arrs, ptrs, lens = self._pack_samples(clips)
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
         s = self._ensure_session(B, max(a.shape[0] for a in arrs), mx, max_new_tokens)
         ids = np.zeros((B, max_new_tokens), dtype=np.int32)
         n = np.zeros(B, dtype=np.int32)
-        _lib.check(self._lib.asrb_transcribe_ids(
-            s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
-            ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
-        ms = (C.c_float * 6)()
-        k, st = C.c_int64(), C.c_int64()
-        _lib.check(self._lib.asrb_last_timings(s, ms, C.byref(k), C.byref(st)))
-        names = ("h2d", "mel", "encoder", "prefill", "decode", "total")
-        return TranscribeIds([ids[b, : n[b]].tolist() for b in range(B)], dict(zip(names, ms)), k.value, st.value)
+        if logprobs:
+            self._record_logprobs(s, True)
+        try:
+            _lib.check(self._lib.asrb_transcribe_ids(
+                s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
+                ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
+            return self._finish(s, B, ids, n, max_new_tokens, logprobs)
+        finally:
+            if logprobs:
+                self._record_logprobs(s, False)
 
     # ---- GPU-side audio ingest (step 1, src/audio.rs:162-245) -------------------------------------------
     _PCM_FMT = {"int16": 0, "float32": 1, "int32": 2}
@@ -250,41 +298,48 @@ class AsrInference:
         return out
 
     def transcribe_pcm(self, pcms: Sequence, rates: Sequence[int], language_ids: Optional[Sequence] = None,
-                       max_new_tokens: int = MAX_NEW_TOKENS) -> TranscribeIds:
-        """transcribe() steps 1-8 for a batch with step 1 on the GPU: raw PCM in, token ids out."""
+                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False) -> TranscribeIds:
+        """transcribe() steps 1-8 for a batch with step 1 on the GPU: raw PCM in, token ids out (`logprobs`: as in
+        transcribe_ids)."""
         B = len(pcms)
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
         s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens)
         ids = np.zeros((B, max_new_tokens), dtype=np.int32)
         n = np.zeros(B, dtype=np.int32)
-        _lib.check(self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens),
-                                                      ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
-        ms = (C.c_float * 6)()
-        k, st = C.c_int64(), C.c_int64()
-        _lib.check(self._lib.asrb_last_timings(s, ms, C.byref(k), C.byref(st)))
-        names = ("h2d", "mel", "encoder", "prefill", "decode", "total")
-        return TranscribeIds([ids[b, : n[b]].tolist() for b in range(B)], dict(zip(names, ms)), k.value, st.value)
+        if logprobs:
+            self._record_logprobs(s, True)
+        try:
+            _lib.check(self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens),
+                                                          ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
+            return self._finish(s, B, ids, n, max_new_tokens, logprobs)
+        finally:
+            if logprobs:
+                self._record_logprobs(s, False)
 
     def transcribe(self, audio_path: str, language: Optional[str] = None,
-                   max_new_tokens: int = MAX_NEW_TOKENS, gpu_ingest: bool = True) -> TranscribeResult:
+                   max_new_tokens: int = MAX_NEW_TOKENS, gpu_ingest: bool = True, logprobs: bool = False) -> TranscribeResult:
         """AsrInference::transcribe (inference.rs:89-213): step 1 (WAV payload -> mono 16 kHz; on the GPU by default,
         `gpu_ingest=False` = the host loader) -> steps 2-8 on the GPU -> step 9 (detokenise + parse, host; needs
-        tokenizer.json, else raw_output is the id list as text)."""
+        tokenizer.json, else raw_output is the id list as text).  `logprobs`: also fill token_logprobs / avg_logprob."""
         from .audio import load_wav, read_wav_pcm
         from .text import language_prompt_ids, parse_asr_output
         lang_ids = language_prompt_ids(self.tokenizer, language)
         if gpu_ingest:
             pcm, rate = read_wav_pcm(audio_path)
             r = self.transcribe_pcm([pcm], [rate], language_ids=[lang_ids] if lang_ids is not None else None,
-                                    max_new_tokens=max_new_tokens)
+                                    max_new_tokens=max_new_tokens, logprobs=logprobs)
         else:
             samples = load_wav(audio_path, MEL_SAMPLE_RATE)
             r = self.transcribe_ids([samples], language_ids=[lang_ids] if lang_ids is not None else None,
-                                    max_new_tokens=max_new_tokens)
+                                    max_new_tokens=max_new_tokens, logprobs=logprobs)
         ids = r.ids[0]
         raw = self.tokenizer.decode(ids) if self.tokenizer is not None else " ".join(str(i) for i in ids)
         lang, text = parse_asr_output(raw, language is not None) if self.tokenizer is not None else ("unknown", raw)
-        return TranscribeResult(text=text, language=lang, raw_output=raw, ids=ids)
+        res = TranscribeResult(text=text, language=lang, raw_output=raw, ids=ids)
+        if logprobs:
+            res.token_logprobs = r.logprobs[0]
+            res.avg_logprob = avg_logprob(r.logprobs[0], r.eos_logprobs[0])
+        return res
 
     # ---- stage-level calls (the calls transcribe() makes; used by the parity tests) ----
     def mel(self, clips: Sequence[np.ndarray], max_new_tokens: int = 64, max_lang: int = 16) -> List[np.ndarray]:

@@ -65,5 +65,6 @@ extern "C" {
     pub fn asrb_session_device_ids(s: *mut asrb_session, ids_dev: *mut *const i32, lens_dev: *mut *const i32, row_stride: *mut c_int, batch: *mut c_int) -> c_int;
     pub fn asrb_session_stats(s: *mut asrb_session, out: *mut i64, n: c_int) -> c_int;
     pub fn asrb_session_set_option(s: *mut asrb_session, key: *const c_char, value: *const c_char) -> c_int;
+    pub fn asrb_last_logprobs(s: *mut asrb_session, max_new_tokens: c_int, logprobs_out: *mut f32, eos_logprob_out: *mut f32) -> c_int;
     pub fn asrb_debug_mega_timeline(out: *mut c_longlong, cap: c_int) -> c_int;
 }

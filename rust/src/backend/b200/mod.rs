@@ -85,4 +85,25 @@ impl B200Engine {
         })?;
         Ok(ids[..n as usize].iter().map(|&t| t as i64).collect())
     }
+
+    /// `transcribe_ids` that also returns the natural-log probability of every generated id and of the EOS id that
+    /// ended the sequence (`None` when it stopped at `max_new_tokens`), computed by the decode kernels from the same
+    /// fp32 logits that selected the ids (`asrb_last_logprobs`).  The ids are those `transcribe_ids` returns.
+    pub fn transcribe_ids_with_logprobs(&self, samples: &[f32], lang_ids: Option<&[i64]>) -> Result<(Vec<i64>, Vec<f32>, Option<f32>)> {
+        let session = self.session_for(samples.len())?;
+        let key = CString::new("logprobs")?;
+        let on = CString::new("1")?;
+        let off = CString::new("0")?;
+        check(unsafe { ffi::asrb_session_set_option(session, key.as_ptr(), on.as_ptr()) })?;
+        let run = (|| -> Result<(Vec<i64>, Vec<f32>, Option<f32>)> {
+            let ids = self.transcribe_ids(samples, lang_ids)?;
+            let mut lp = vec![0f32; self.max_new_tokens];
+            let mut eos = 0f32;
+            check(unsafe { ffi::asrb_last_logprobs(session, self.max_new_tokens as i32, lp.as_mut_ptr(), &mut eos) })?;
+            lp.truncate(ids.len());
+            Ok((ids, lp, if eos.is_nan() { None } else { Some(eos) }))
+        })();
+        check(unsafe { ffi::asrb_session_set_option(session, key.as_ptr(), off.as_ptr()) })?;
+        run
+    }
 }
