@@ -170,7 +170,10 @@ ASRB_API int asrb_session_stats(asrb_session* s, int64_t* out, int n);
 /* knobs: "gemm" = "tc"|"simt", "decode" = "mega"|"phases", "batch_step" = "1"|"0", "planes" = "1"|"2"|"3",
  * "resident" = "1"|"0" (1: the samples uploaded by the previous call are reused, no H2D),
  * "logprobs" = "1"|"0" (1: every greedy step also records the log-probability of the token it selects, read with
- * asrb_last_logprobs; same ids, same decode paths; the value in effect at the prefill applies to the whole run) */
+ * asrb_last_logprobs; same ids, same decode paths; the value in effect at the prefill applies to the whole run),
+ * "top_logprobs" = "0".."8" (k >= 1: every greedy step also records its k best candidates, read with
+ * asrb_last_top_logprobs, and the log-probabilities asrb_last_logprobs reads; same ids, same decode paths; the value in
+ * effect at the prefill applies to the whole run) */
 ASRB_API int asrb_session_set_option(asrb_session* s, const char* key, const char* value);
 
 /* Per-token log-probabilities of the last run (asrb_generate / asrb_transcribe_ids / asrb_transcribe_ingested, or
@@ -181,6 +184,18 @@ ASRB_API int asrb_session_set_option(asrb_session* s, const char* key, const cha
  *                     max_new_tokens
  * Returns ASRB_ERR_STATE when the last run did not record them (option off, or switched after the prefill). */
 ASRB_API int asrb_last_logprobs(asrb_session* s, int max_new_tokens, float* logprobs_out, float* eos_logprob_out);
+
+/* Top-k alternatives of the last run, recorded when the option "top_logprobs" was k_rec >= 1 for its prefill and every
+ * step.  Candidates are the best logits of the step under (logit descending, id ascending), the order the greedy argmax
+ * uses; candidate j's value is its log-probability under the same fp32 logits: (l_j - max) + lp_0, where lp_0 is the
+ * value asrb_last_logprobs reports for the selected token.
+ *   ids_out / logprobs_out          [batch][max_new_tokens][k]: candidates of the step that selected ids[b][i], best first
+ *                                   (entry 0 = ids[b][i]); -1 / NaN at and beyond lens_out[b]
+ *   eos_ids_out / eos_logprobs_out  [batch][k] or NULL: the same for the step that selected the EOS ending sequence b
+ *                                   (entry 0 = that EOS id); -1 / NaN if it stopped at max_new_tokens
+ * ASRB_ERR_STATE when the last run did not record them; ASRB_ERR_INVALID when k < 1 or k > k_rec. */
+ASRB_API int asrb_last_top_logprobs(asrb_session* s, int max_new_tokens, int k, int32_t* ids_out, float* logprobs_out,
+                                    int32_t* eos_ids_out, float* eos_logprobs_out);
 
 /* debug (ASRB_MEGA_DEBUG=1): clock64 timeline of the last fused decode step, CTA 0 then CTA G-1;
  * returns the number of slots per CTA (0 if disabled) */

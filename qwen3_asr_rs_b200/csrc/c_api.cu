@@ -25,6 +25,8 @@ void session_last_timings(Session* s, float* ms6, int64_t* kernels, int64_t* ste
 void session_set_option(Session* s, const char* key, const char* value);
 void session_stats(Session* s, int64_t* out, int n);
 void session_last_logprobs(Session* s, int max_new_tokens, float* out, float* eos_out);
+void session_last_top_logprobs(Session* s, int max_new_tokens, int k, int32_t* ids_out, float* lp_out, int32_t* eos_ids_out,
+                               float* eos_lp_out);
 void session_ingest_pcm(Session* s, const void* const* pcm, const int64_t* n_frames, const int32_t* channels, const int32_t* rate,
                         const int32_t* format, int batch, int64_t* n_samples_out);
 void session_ingested_read(Session* s, int b, float* out);
@@ -191,6 +193,13 @@ int asrb_session_set_option(asrb_session* s, const char* key, const char* value)
 }
 int asrb_last_logprobs(asrb_session* s, int max_new_tokens, float* logprobs_out, float* eos_logprob_out) {
     return guarded([&] { NONNULL(s); NONNULL(logprobs_out); session_last_logprobs(s->s, max_new_tokens, logprobs_out, eos_logprob_out); });
+}
+int asrb_last_top_logprobs(asrb_session* s, int max_new_tokens, int k, int32_t* ids_out, float* logprobs_out,
+                           int32_t* eos_ids_out, float* eos_logprobs_out) {
+    return guarded([&] {
+        NONNULL(s); NONNULL(ids_out); NONNULL(logprobs_out);
+        session_last_top_logprobs(s->s, max_new_tokens, k, ids_out, logprobs_out, eos_ids_out, eos_logprobs_out);
+    });
 }
 
 int asrb_debug_mega_timeline(long long* out, int cap) {

@@ -112,6 +112,64 @@ __device__ __forceinline__ float lse_merge(float m, float s, float om, float os)
     return lse_rescale(s, m, M) + lse_rescale(os, om, M);
 }
 
+// ---- top-k candidate lists beside the greedy argmax -----------------------------------------------------
+// TK_MAX (logit, id) pairs kept sorted best first under the argmax's total order: logit descending, then id ascending.
+// Ids are distinct across the rows folded anywhere, so the top TK_MAX of any union is one set whatever the merge order.
+// Empty entries are (-inf, 0x7fffffff).  All indices are compile-time: the lists stay in registers.
+constexpr int TK_MAX = 8;
+struct TopK { float v[TK_MAX]; int i[TK_MAX]; };
+__device__ __forceinline__ bool tk_before(float a, int ai, float b, int bi) { return a > b || (a == b && ai < bi); }
+__device__ __forceinline__ void tk_init(TopK& t) {
+#pragma unroll
+    for (int j = 0; j < TK_MAX; ++j) { t.v[j] = -INFINITY; t.i[j] = 0x7fffffff; }
+}
+// fold logit v of `row`: one compare unless it beats the tail, then it bubbles into place and the tail drops out
+__device__ __forceinline__ void tk_insert(TopK& t, float v, int row) {
+    if (!tk_before(v, row, t.v[TK_MAX - 1], t.i[TK_MAX - 1])) return;
+#pragma unroll
+    for (int j = 0; j < TK_MAX; ++j)
+        if (tk_before(v, row, t.v[j], t.i[j])) { const float tv = t.v[j]; const int ti = t.i[j]; t.v[j] = v; t.i[j] = row; v = tv; row = ti; }
+}
+// t <- top TK_MAX of t and u (both sorted): the better of t[j] and u[TK_MAX-1-j] is a bitonic sequence holding the top
+// TK_MAX of the union, which three half-cleaner stages sort
+__device__ __forceinline__ void tk_merge(TopK& t, const TopK& u) {
+#pragma unroll
+    for (int j = 0; j < TK_MAX; ++j)
+        if (!tk_before(t.v[j], t.i[j], u.v[TK_MAX - 1 - j], u.i[TK_MAX - 1 - j])) { t.v[j] = u.v[TK_MAX - 1 - j]; t.i[j] = u.i[TK_MAX - 1 - j]; }
+#pragma unroll
+    for (int d = TK_MAX / 2; d > 0; d >>= 1)
+#pragma unroll
+        for (int j = 0; j < TK_MAX; ++j)
+            if ((j & d) == 0 && tk_before(t.v[j + d], t.i[j + d], t.v[j], t.i[j])) {
+                const float tv = t.v[j]; const int ti = t.i[j];
+                t.v[j] = t.v[j + d]; t.i[j] = t.i[j + d]; t.v[j + d] = tv; t.i[j + d] = ti;
+            }
+}
+// merge with the list of lane ^ o (both lanes end with the same list)
+__device__ __forceinline__ void tk_merge_xor(TopK& t, int o) {
+    TopK u;
+#pragma unroll
+    for (int j = 0; j < TK_MAX; ++j) { u.v[j] = __shfl_xor_sync(0xffffffffu, t.v[j], o); u.i[j] = __shfl_xor_sync(0xffffffffu, t.i[j], o); }
+    tk_merge(t, u);
+}
+__device__ __forceinline__ void tk_store(const TopK& t, float* v, int* i) {
+#pragma unroll
+    for (int j = 0; j < TK_MAX; ++j) { v[j] = t.v[j]; i[j] = t.i[j]; }
+}
+// merge a list published by another thread of this CTA (shared memory) or, with L2 loads, by another CTA
+__device__ __forceinline__ void tk_merge_from(TopK& t, const float* v, const int* i, bool l2) {
+    TopK u;
+#pragma unroll
+    for (int j = 0; j < TK_MAX; ++j) { u.v[j] = l2 ? __ldcg(v + j) : v[j]; u.i[j] = l2 ? __ldcg(i + j) : i[j]; }
+    tk_merge(t, u);
+}
+// the step's record: entry j = (l_j - l_0) + lp where l_0 is the maximum logit and lp = -log S the selected token's
+// log-probability; entry 0 is lp itself, bitwise
+__device__ __forceinline__ void tk_write(const TopK& t, float lp, int* ids, float* lps) {
+#pragma unroll
+    for (int j = 0; j < TK_MAX; ++j) { ids[j] = t.i[j]; lps[j] = j == 0 ? lp : (t.v[j] - t.v[0]) + lp; }
+}
+
 // order-preserving float <-> int key (for atomicMax on floats of either sign)
 __device__ __host__ __forceinline__ int float_to_ordered(float f) {
 #ifdef __CUDA_ARCH__

@@ -235,14 +235,19 @@ __global__ void __launch_bounds__(128) dec_attn_kernel(const float* __restrict__
 // greedy bookkeeping (inference.rs:161-170): finish the argmax, EOS check, append, embed.
 // LOGPROB: also merge the (max, sum of exponentials) records and store the selected token's log-probability in
 // lp_out (appended token) or eos_lp (EOS).
+// TOPK (with LOGPROB): also select the TK_MAX best (logit, id) pairs of the step's logits [B][vocab] (written by the
+// lm_head GEMV) and store them in tk_ids / tk_lp [B][max_new][TK_MAX] or the EOS rows tk_eos_ids / tk_eos_lp [B][TK_MAX].
 // grid = B blocks.
 // ---------------------------------------------------------------------------------------------
-template <bool LOGPROB>
+template <bool LOGPROB, bool TOPK = false>
 __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __restrict__ part_idx, int n_part,
                               int* __restrict__ done, int* __restrict__ pos, int* __restrict__ next_id,
                               int* __restrict__ ids_out, int* __restrict__ n_out, int max_new,
                               const bf16* __restrict__ embed, int hidden, float* __restrict__ x,
-                              const float* __restrict__ part_sum, float* __restrict__ lp_out, float* __restrict__ eos_lp) {
+                              const float* __restrict__ part_sum, float* __restrict__ lp_out, float* __restrict__ eos_lp,
+                              const float* __restrict__ logits, int vocab, int* __restrict__ tk_ids, float* __restrict__ tk_lp,
+                              int* __restrict__ tk_eos_ids, float* __restrict__ tk_eos_lp) {
+    static_assert(!TOPK || LOGPROB, "the candidates' log-probabilities need the sum of exponentials");
     __shared__ float sv[32];
     __shared__ int si[32];
     __shared__ int tok_s;
@@ -279,6 +284,23 @@ __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __r
             lp = -logf(S);
         }
     }
+    TopK tk;
+    if constexpr (TOPK) {
+        // each thread its rows (ascending), a butterfly per warp, then thread 0 merges the warps' lists
+        __shared__ float tkv[32 * TK_MAX];
+        __shared__ int tki[32 * TK_MAX];
+        tk_init(tk);
+        const float* lg = logits + (size_t)b * vocab;
+        for (int i = tid; i < vocab; i += blockDim.x) tk_insert(tk, lg[i], i);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) tk_merge_xor(tk, o);
+        if (lane == 0) tk_store(tk, tkv + warp * TK_MAX, tki + warp * TK_MAX);
+        __syncthreads();
+        if (tid == 0) {
+            const int nw = (blockDim.x + 31) / 32;
+            for (int w = 1; w < nw; ++w) tk_merge_from(tk, tkv + w * TK_MAX, tki + w * TK_MAX, false);
+        }
+    }
     if (tid == 0) {
         int nw = (blockDim.x + 31) / 32;
         for (int w = 1; w < nw; ++w)
@@ -287,6 +309,13 @@ __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __r
         if constexpr (LOGPROB) {
             if (tok == 151643 || tok == 151645) eos_lp[b] = lp;
             else if (n_out[b] < max_new) lp_out[(size_t)b * max_new + n_out[b]] = lp;
+        }
+        if constexpr (TOPK) {
+            if (tok == 151643 || tok == 151645) tk_write(tk, lp, tk_eos_ids + (size_t)b * TK_MAX, tk_eos_lp + (size_t)b * TK_MAX);
+            else if (n_out[b] < max_new) {
+                const size_t o = ((size_t)b * max_new + n_out[b]) * TK_MAX;
+                tk_write(tk, lp, tk_ids + o, tk_lp + o);
+            }
         }
         if (tok == 151643 || tok == 151645 || n_out[b] >= max_new) {   // EOS ids, inference.rs:154
             done[b] = 1; next_id[b] = -1; tok = -1;
@@ -306,12 +335,18 @@ __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __r
 }
 
 void launch_greedy(const Model& m, const DecodeBufs& b, int B, cudaStream_t st, int64_t* launches) {
-    if (b.logprobs)
+    if (b.topk)     // the lm_head wrote the logits (launch_lmhead_argmax): one CTA per sequence selects the candidates
+        greedy_kernel<true, true><<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
+                                                     b.max_new, m.embed, m.d.c.hidden_size, b.x, b.part_sum, b.lp_out, b.eos_lp,
+                                                     b.logits, m.d.c.vocab_size, b.tk_ids, b.tk_lp, b.tk_eos_ids, b.tk_eos_lp);
+    else if (b.logprobs)
         greedy_kernel<true><<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
-                                               b.max_new, m.embed, m.d.c.hidden_size, b.x, b.part_sum, b.lp_out, b.eos_lp);
+                                               b.max_new, m.embed, m.d.c.hidden_size, b.x, b.part_sum, b.lp_out, b.eos_lp,
+                                               nullptr, 0, nullptr, nullptr, nullptr, nullptr);
     else
         greedy_kernel<false><<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
-                                                b.max_new, m.embed, m.d.c.hidden_size, b.x, nullptr, nullptr, nullptr);
+                                                b.max_new, m.embed, m.d.c.hidden_size, b.x, nullptr, nullptr, nullptr,
+                                                nullptr, 0, nullptr, nullptr, nullptr, nullptr);
     ASRB_CUDA_CHECK(cudaGetLastError());
     if (launches) *launches += 1;
 }
@@ -337,7 +372,7 @@ void launch_lmhead_argmax(const Model& m, const float* x_rows, const int* d_row_
         p.W = m.lm_head; p.N = c.vocab_size; p.K = c.hidden_size;
         p.x = d_row_idx ? x_rows : x_rows + (size_t)b0 * c.hidden_size; p.ldx = c.hidden_size; p.row_idx = d_row_idx ? d_row_idx + b0 : nullptr;
         p.norm_w = m.final_norm; p.eps = (float)c.rms_norm_eps;
-        p.logits = write_logits ? ob.logits : nullptr; p.ldl = c.vocab_size;
+        p.logits = (write_logits || b.topk) ? ob.logits : nullptr; p.ldl = c.vocab_size;   // TOPK: greedy_kernel reads them
         p.part_val = ob.part_val; p.part_idx = ob.part_idx; p.B = nb;
         if (b.logprobs) { p.part_sum = ob.part_sum; run_gemv<true, DE_ARGMAX_LSE>(p, b.n_part, st); }
         else run_gemv<true, DE_ARGMAX>(p, b.n_part, st);

@@ -61,6 +61,10 @@ struct Params {
     float* part_sum;             // [nb][n_part] sum of exp(logit - part_val) over the CTA's lm_head rows
     float* lp_out;               // [nb][max_new] log-probability of each appended token
     float* eos_lp;               // [nb] log-probability of the EOS token that ends the sequence
+    // TOPK instantiations only (appended as well)
+    float* tk_part_val; int* tk_part_idx;   // [nb][n_part][TK_MAX] each CTA's best (logit, id) candidates per sequence
+    int* tk_ids; float* tk_lp;              // [nb][max_new][TK_MAX] candidates of each appended token's step, best first
+    int* tk_eos_ids; float* tk_eos_lp;      // [nb][TK_MAX] those of the step that selects EOS
 };
 
 __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
@@ -153,7 +157,10 @@ enum { BE_STORE = 0, BE_SWIGLU = 1, BE_ARGMAX = 2 };
 
 // LOGPROB: the lm_head also keeps (max, sum of exponentials) per (tile row, sequence), and the last CTA records the
 // log-probability of each selected token (p.lp_out / p.eos_lp)
-template <int H, int QD, int I, int NB, int NS, int KVK, bool LOGPROB>
+// TOPK (with LOGPROB): each (tile row, sequence) thread also keeps its best TK_MAX (logit, id) pairs; they are merged
+// per sequence across tile rows and CTAs, and the last CTA records each step's candidates (p.tk_ids / p.tk_lp, or the
+// EOS rows)
+template <int H, int QD, int I, int NB, int NS, int KVK, bool LOGPROB, bool TOPK = false>
 __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params p) {   // 9 warps are allocated as 12 (granularity 4): 168 registers
     static_assert(NB % 8 == 0 && NB <= 16, "NB must be 8 or 16");
     static_assert(H % 256 == 0 && QD % H == 0 && I % H == 0, "chunking needs QD, I multiples of H, H multiple of 256");
@@ -166,6 +173,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
     constexpr int KV_TILE = KVK * HD * 4;
     constexpr int GROUP = 2;                    // q heads per kv head (checked on the host)
     constexpr int XS_FLOATS = (3 * PSTR / 4 > ATT_SCRATCH) ? 3 * PSTR / 4 : ATT_SCRATCH;   // activation planes; attention scratch aliases them
+    static_assert(!TOPK || LOGPROB, "the candidates' log-probabilities need the sum of exponentials");
+    static_assert(16 * NB * (1 + 2 * TK_MAX) <= XS_FLOATS, "lm_head merge records must fit the activation planes");
     extern __shared__ __align__(128) uint8_t smem[];
     Ring ring;
     ring.slots = smem; ring.nslot = NS;
@@ -297,6 +306,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
     }
     float best_v = -INFINITY; int best_i = 0x7fffffff;      // lm_head: running argmax of (tile row tid / NB, sequence tid % NB)
     float best_s = 0.f;                                      // LOGPROB: its sum of exp(logit - best_v)
+    TopK tk;                                                 // TOPK: its best rows
+    if constexpr (TOPK) tk_init(tk);
     // merging CTA: which (sequence, kv head), and which record slots will be written for it -- slot u holds a record iff a
     // run starts at split u, i.e. u == 0 or item base + u opens its owner's range.  Positions do not change within the
     // step, so this is computed once, not per layer (the owner search is a dozen integer divisions per slot).
@@ -490,7 +501,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
                         const float up = __shfl_down_sync(0xffffffffu, v, NB);     // rows 2j (gate) and 2j + 1 (up): NB threads apart
                         if (valid && !(rr & 1)) sx_store(sxo + (size_t)sq * I + (row >> 1), silu(v) * up);
                     } else if constexpr (LOGPROB) {
-                        if (valid) lse_fold(v, row, best_v, best_i, best_s);      // rows ascend per thread: ties keep the first
+                        if (valid) {
+                            lse_fold(v, row, best_v, best_i, best_s);     // rows ascend per thread: ties keep the first
+                            if constexpr (TOPK) tk_insert(tk, v, row);
+                        }
                     } else {
                         if (valid && (v > best_v || (v == best_v && row < best_i))) { best_v = v; best_i = row; }
                     }
@@ -802,7 +816,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
     cons_sync();
     // LOGPROB: the sums go to the activation planes, which nothing reads once the lm_head tiles are contracted
     float* bests = xs;                                       // [16 rows][NB]
+    float* tkv = xs + 16 * NB;                               // TOPK: [16 rows][NB][TK_MAX] candidate values, then ids
+    int* tki = reinterpret_cast<int*>(tkv + 16 * NB * TK_MAX);
     if (tid < 16 * NB) { bestv[tid] = best_v; besti[tid] = best_i; if constexpr (LOGPROB) bests[tid] = best_s; }
+    if constexpr (TOPK) if (tid < 16 * NB) tk_store(tk, tkv + tid * TK_MAX, tki + tid * TK_MAX);
     cons_sync();
     int& is_last = misc[0];
     if (tid < nb) {
@@ -816,6 +833,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
             float sum = 0.f;
             for (int wq = 0; wq < 16; ++wq) sum += lse_rescale(bests[wq * NB + tid], bestv[wq * NB + tid], v);
             p.part_sum[(size_t)tid * p.n_part + blockIdx.x] = sum;
+        }
+        if constexpr (TOPK) {                                // the CTA's TK_MAX best of the sequence's 16 tile rows
+            tk_init(tk);
+            for (int wq = 0; wq < 16; ++wq) tk_merge_from(tk, tkv + (wq * NB + tid) * TK_MAX, tki + (wq * NB + tid) * TK_MAX, false);
+            const size_t o = ((size_t)tid * p.n_part + blockIdx.x) * TK_MAX;
+            tk_store(tk, p.tk_part_val + o, p.tk_part_idx + o);
         }
         __threadfence();
     }
@@ -853,6 +876,24 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
             if (lane == 0) {
                 if (tok == 151643 || tok == 151645) p.eos_lp[b] = lp;
                 else if (n < p.max_new) p.lp_out[(size_t)b * p.max_new + n] = lp;
+            }
+            if constexpr (TOPK) {
+                // the TK_MAX best of the G CTA lists: each lane merges its CTAs', then a butterfly (every lane ends
+                // with the same list, the exact top of one set whatever the order)
+                tk_init(tk);
+                for (int i = lane; i < (int)G; i += 32) {
+                    const size_t o = ((size_t)b * p.n_part + i) * TK_MAX;
+                    tk_merge_from(tk, p.tk_part_val + o, p.tk_part_idx + o, true);
+                }
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) tk_merge_xor(tk, o);
+                if (lane == 0) {
+                    if (tok == 151643 || tok == 151645) tk_write(tk, lp, p.tk_eos_ids + (size_t)b * TK_MAX, p.tk_eos_lp + (size_t)b * TK_MAX);
+                    else if (n < p.max_new) {
+                        const size_t o = ((size_t)b * p.max_new + n) * TK_MAX;
+                        tk_write(tk, lp, p.tk_ids + o, p.tk_lp + o);
+                    }
+                }
             }
         }
         if (tok == 151643 || tok == 151645 || n >= p.max_new) {
@@ -941,7 +982,15 @@ void launch_decode_step_batch(const Model& m, const DecodeBufs& b, int B, float*
         const BatchCfg k = batch_cfg(nb);
         const size_t smem = batch_smem_bytes(c.hidden_size, k);
         const void* fn = nullptr;
-        if (b.logprobs) {
+        if (b.topk) {
+            if (bdims_match<1024, 2048, 3072>(c))
+                fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, true, true>
+                               : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, true, true>;
+            else
+                fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, true, true>
+                               : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, true, true>;
+        }
+        else if (b.logprobs) {
             if (bdims_match<1024, 2048, 3072>(c))
                 fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, true>
                                : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, true>;
@@ -980,6 +1029,11 @@ void launch_decode_step_batch(const Model& m, const DecodeBufs& b, int B, float*
         g_last_dbg_batch = mb.dbg;
         if (b.logprobs) {
             p.part_sum = b.part_sum + (size_t)b0 * b.n_part; p.lp_out = b.lp_out + (size_t)b0 * b.max_new; p.eos_lp = b.eos_lp + b0;
+        }
+        if (b.topk) {
+            p.tk_part_val = b.tk_part_val + (size_t)b0 * b.n_part * TK_MAX; p.tk_part_idx = b.tk_part_idx + (size_t)b0 * b.n_part * TK_MAX;
+            p.tk_ids = b.tk_ids + (size_t)b0 * b.max_new * TK_MAX; p.tk_lp = b.tk_lp + (size_t)b0 * b.max_new * TK_MAX;
+            p.tk_eos_ids = b.tk_eos_ids + (size_t)b0 * TK_MAX; p.tk_eos_lp = b.tk_eos_lp + (size_t)b0 * TK_MAX;
         }
         { static const int fl = getenv("ASRB_BATCH_FLAGS") ? atoi(getenv("ASRB_BATCH_FLAGS")) : 0; p.flags = fl; }   // bit 0 (K/V L2 prefetch): measured slower, off
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {   // tags must stay monotonic: wipe long before the epoch wraps

@@ -55,6 +55,10 @@ struct Params {
     float* part_sum;             // [gridDim.x] sum of exp(logit - part_val) over the CTA's lm_head rows
     float* lp_out;               // [max_new] log-probability of each appended token
     float* eos_lp;               // log-probability of the EOS token that ends the sequence
+    // TOPK instantiations only (appended as well)
+    float* tk_part_val; int* tk_part_idx;   // [gridDim.x][TK_MAX] the CTA's best (logit, id) candidates
+    int* tk_ids; float* tk_lp;              // [max_new][TK_MAX] candidates of each appended token's step, best first
+    int* tk_eos_ids; float* tk_eos_lp;      // [TK_MAX] those of the step that selects EOS
 };
 
 static_assert(KV_KEYS * HD * 4 == SLOT_BYTES, "K / V tiles travel through the weight ring: one tile per slot");
@@ -269,10 +273,10 @@ __device__ __forceinline__ void consume_ksplit(const Slice& s, const Ring& ring,
 }
 
 // K <= 1024 GEMVs (qkv, gate/up, lm_head of the 0.6B dims): four rows per warp and turn, two ring slots (32 rows) per turn.
-template <int K, int EPI, bool LOGPROB>
+template <int K, int EPI, bool LOGPROB, bool TOPK>
 __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
                                              uint32_t tag, uint32_t* sxo, float& best_v, int& best_i, float& best_s,
-                                             const float* norm_w, float norm_r, long long* fine) {
+                                             const float* norm_w, float norm_r, long long* fine, TopK* tk) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int fi = 0;
 #define CF() do { if (fine && threadIdx.x == 0 && fi < 24) fine[fi++] = clock64(); } while (0)
@@ -312,7 +316,10 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
             } else if (EPI == ME_STORE) {
                 if ((lane & 7) == 0 && j < nv) ll_store(out + row, v, tag);
             } else if constexpr (LOGPROB) {        // ME_ARGMAX + running sum of exponentials (the lanes that keep best_v)
-                if ((lane & 7) == 0 && j < nv) lse_fold(v, row, best_v, best_i, best_s);
+                if ((lane & 7) == 0 && j < nv) {
+                    lse_fold(v, row, best_v, best_i, best_s);
+                    if constexpr (TOPK) tk_insert(*tk, v, row);           // TOPK: + the lane's best TK_MAX rows
+                }
             } else {                               // ME_ARGMAX: rows arrive in increasing order per lane, strict > keeps the first maximum
                 if ((lane & 7) == 0 && j < nv && v > best_v) { best_v = v; best_i = row; }
             }
@@ -328,12 +335,14 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
 
 // consumer: process all chunks of a slice.  `xs` holds the (already normalised) activation vector.
 // Results are published as tagged words to `out` (ME_STORE), as self-validating words to `sxo` (ME_SWIGLU), or folded
-// into the running argmax (ME_ARGMAX; with LOGPROB also into the running sum of exponentials `best_s`).
-template <int K, int EPI, bool LOGPROB = false>
+// into the running argmax (ME_ARGMAX; with LOGPROB also into the running sum of exponentials `best_s`, with TOPK also
+// into the sorted candidate list `*tk`).
+template <int K, int EPI, bool LOGPROB = false, bool TOPK = false>
 __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
                                         uint32_t tag, uint32_t* sxo, float& best_v, int& best_i, float& best_s,
-                                        const float* norm_w = nullptr, float norm_r = 1.f, long long* fine = nullptr) {
-    if constexpr (K <= 1024) { consume_quad<K, EPI, LOGPROB>(s, ring, q, xs, out, tag, sxo, best_v, best_i, best_s, norm_w, norm_r, fine); return; }
+                                        const float* norm_w = nullptr, float norm_r = 1.f, long long* fine = nullptr,
+                                        TopK* tk = nullptr) {
+    if constexpr (K <= 1024) { consume_quad<K, EPI, LOGPROB, TOPK>(s, ring, q, xs, out, tag, sxo, best_v, best_i, best_s, norm_w, norm_r, fine, tk); return; }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int fi = 0;
 #define CF() do { if (fine && threadIdx.x == 0 && fi < 24) fine[fi++] = clock64(); } while (0)
@@ -393,7 +402,10 @@ __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32
                 if (EPI == ME_STORE) {
                     if (act) ll_store(out + row, v0, tag);
                 } else if constexpr (LOGPROB) {
-                    if (act) lse_fold(v0, row, best_v, best_i, best_s);
+                    if (act) {
+                        lse_fold(v0, row, best_v, best_i, best_s);
+                        if constexpr (TOPK) tk_insert(*tk, v0, row);
+                    }
                 } else {
                     if (act && v0 > best_v) { best_v = v0; best_i = row; }
                 }
@@ -514,7 +526,9 @@ __device__ __forceinline__ void head_norm_rope(const uint2* __restrict__ src, ui
 
 // LOGPROB: the lm_head also keeps (max, sum of exponentials) per lane, and the last CTA records the log-probability of
 // the selected token (p.lp_out / p.eos_lp)
-template <int H, int QD, int I, int NS, bool LOGPROB>
+// TOPK (with LOGPROB): each folding lane also keeps its best TK_MAX (logit, id) pairs; they are merged across lanes,
+// warps and CTAs, and the last CTA records the step's candidates (p.tk_ids / p.tk_lp, or the EOS row)
+template <int H, int QD, int I, int NS, bool LOGPROB, bool TOPK = false>
 __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p) {
     constexpr int XS_FLOATS = (I > XS_MIN ? I : XS_MIN) + 64;
     extern __shared__ __align__(128) uint8_t smem[];
@@ -644,6 +658,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     const unsigned G = gridDim.x;
     float best_v = -INFINITY; int best_i = 0x7fffffff;
     float best_s = 0.f;                               // LOGPROB: sum of exp(logit - best_v) over the rows this lane folded
+    static_assert(!TOPK || LOGPROB, "the candidates' log-probabilities need the sum of exponentials");
+    TopK tk;                                          // TOPK: this lane's best rows
+    if constexpr (TOPK) tk_init(tk);
     // tag = launch epoch (unique per executed step, survives new utterances that revisit the same positions)
     const unsigned epoch = __ldcg(p.bar + 1);
     const uint32_t tag_base = (epoch & 0xffffffu) << 8;
@@ -944,8 +961,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
         mbar_wait(&p_full[p.L & 1], (p.L >> 1) & 1);
         nrf = norm_scale(ss, H, p.eps, red);
     }
-    consume<H, ME_ARGMAX, LOGPROB>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i, best_s,
-                                   pbuf + (p.L & 1) * PARAM_FLOATS, nrf);
+    consume<H, ME_ARGMAX, LOGPROB, TOPK>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i, best_s,
+                                         pbuf + (p.L & 1) * PARAM_FLOATS, nrf, nullptr, &tk);
     MEGA_MARK();
     // candidates live in lanes 0, 8, 16, 24 of every warp (the four rows of a turn; lanes 0 / 16 in the two-row form):
     // merge them, lane 0 publishes the warp's best
@@ -954,9 +971,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
         const float ov = __shfl_xor_sync(0xffffffffu, best_v, o); const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
         if constexpr (LOGPROB) best_s = lse_merge(best_v, best_s, ov, __shfl_xor_sync(0xffffffffu, best_s, o));
         if (ov > best_v || (ov == best_v && oi < best_i)) { best_v = ov; best_i = oi; }
+        if constexpr (TOPK) tk_merge_xor(tk, o);
     }
     cons_sync();
+    // TOPK: the warps' lists go to xs ([NCONS_WARPS][TK_MAX] values, then ids), free once the lm_head has read it
+    float* tkv = xs; int* tki = reinterpret_cast<int*>(xs + NCONS_WARPS * TK_MAX);
     if (lane == 0) { red[warp] = best_v; ired[warp] = best_i; if constexpr (LOGPROB) red[NCONS_WARPS + warp] = best_s; }
+    if constexpr (TOPK) if (lane == 0) tk_store(tk, tkv + warp * TK_MAX, tki + warp * TK_MAX);
     cons_sync();
     int& is_last = ired[63];
     if (tid == 0) {
@@ -968,6 +989,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
             float sum = 0.f;
             for (int wq = 0; wq < NCONS_WARPS; ++wq) sum += lse_rescale(red[NCONS_WARPS + wq], red[wq], v);
             p.part_sum[blockIdx.x] = sum;
+        }
+        if constexpr (TOPK) {                // the CTA's TK_MAX best of its warps' lists
+            for (int wq = 1; wq < NCONS_WARPS; ++wq) tk_merge_from(tk, tkv + wq * TK_MAX, tki + wq * TK_MAX, false);
+            tk_store(tk, p.tk_part_val + (size_t)blockIdx.x * TK_MAX, p.tk_part_idx + (size_t)blockIdx.x * TK_MAX);
         }
         __threadfence();
         unsigned t = atomicAdd(p.bar, 1u);
@@ -1007,6 +1032,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
                 lp = -logf(S);
             }
         }
+        if constexpr (TOPK) {
+            // the step's TK_MAX best of the G CTA lists: each thread merges its CTAs', then a butterfly per warp and
+            // thread 0 the warps' lists (the exact top of one set: the order of the merges does not matter)
+            tk_init(tk);
+            for (int i = tid; i < (int)G; i += NCONS) tk_merge_from(tk, p.tk_part_val + (size_t)i * TK_MAX, p.tk_part_idx + (size_t)i * TK_MAX, true);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) tk_merge_xor(tk, o);
+            if (lane == 0) tk_store(tk, tkv + warp * TK_MAX, tki + warp * TK_MAX);
+            cons_sync();
+            if (tid == 0)
+                for (int wq = 1; wq < NCONS_WARPS; ++wq) tk_merge_from(tk, tkv + wq * TK_MAX, tki + wq * TK_MAX, false);
+        }
         int& tok_s = ired[62];
         if (tid == 0) {
             for (int wq = 1; wq < NCONS_WARPS; ++wq)
@@ -1016,6 +1053,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
             if constexpr (LOGPROB) {
                 if (tok == 151643 || tok == 151645) *p.eos_lp = lp;
                 else if (n < p.max_new) p.lp_out[n] = lp;
+            }
+            if constexpr (TOPK) {
+                if (tok == 151643 || tok == 151645) tk_write(tk, lp, p.tk_eos_ids, p.tk_eos_lp);
+                else if (n < p.max_new) tk_write(tk, lp, p.tk_ids + (size_t)n * TK_MAX, p.tk_lp + (size_t)n * TK_MAX);
             }
             if (tok == 151643 || tok == 151645 || n >= p.max_new) { *p.done = 1; *p.next_id = -1; tok = -1; }
             else { p.ids_out[n] = tok; *p.n_out = n + 1; *p.pos = pos + 1; *p.next_id = tok; }
@@ -1092,7 +1133,12 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
     const int nsplit = std::min(mega::MAX_SPLITS, std::min(G / c.num_key_value_heads, (max_ctx + mega::KV_KEYS - 1) / mega::KV_KEYS));
     const size_t smem = mega_smem_bytes(c.hidden_size, c.intermediate_size, mega_nslot(c));
     const void* fn = nullptr;
-    if (b.logprobs) {
+    if (b.topk) {
+        if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, true, true>;
+        else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, true, true>;
+        else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, true, true>;
+    }
+    else if (b.logprobs) {
         if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, true>;
         else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, true>;
         else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, true>;
@@ -1125,6 +1171,11 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
         p.dbg = mb.dbg;
         g_last_dbg = mb.dbg;
         if (b.logprobs) { p.part_sum = b.part_sum; p.lp_out = b.lp_out + (size_t)sb * b.max_new; p.eos_lp = b.eos_lp + sb; }
+        if (b.topk) {
+            p.tk_part_val = b.tk_part_val; p.tk_part_idx = b.tk_part_idx;
+            p.tk_ids = b.tk_ids + (size_t)sb * b.max_new * TK_MAX; p.tk_lp = b.tk_lp + (size_t)sb * b.max_new * TK_MAX;
+            p.tk_eos_ids = b.tk_eos_ids + (size_t)sb * TK_MAX; p.tk_eos_lp = b.tk_eos_lp + (size_t)sb * TK_MAX;
+        }
         // tags must stay monotonic for red.max publication: long before the 24-bit epoch wraps, wipe the tagged exchange
         // buffers (the self-validating words live elsewhere and are left alone: to them 0 would be a published 0.0)
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {

@@ -186,6 +186,15 @@ struct DecodeBufs {
     float* part_sum; // [B][n_part] sum of exp(logit - part_val) per argmax partial
     float* lp_out;   // [B][max_new] log-probability of each appended token
     float* eos_lp;   // [B] log-probability of the EOS token that ended the sequence (NaN until then)
+    // top-k alternatives (session option "top_logprobs" >= 1, which also sets `logprobs`): allocated when first enabled;
+    // the kernels always keep TK_MAX candidates per step, best first (-1 / NaN until written)
+    bool topk;          // launch the TOPK kernel variants
+    float* tk_part_val; // [B][n_part][TK_MAX] per-CTA candidate logits
+    int* tk_part_idx;   // [B][n_part][TK_MAX] their ids
+    int* tk_ids;        // [B][max_new][TK_MAX] candidates of the step that selected each appended token
+    float* tk_lp;       // [B][max_new][TK_MAX] their log-probabilities
+    int* tk_eos_ids;    // [B][TK_MAX] candidates of the step that selected the EOS token ending the sequence
+    float* tk_eos_lp;   // [B][TK_MAX]
 };
 void launch_decode_step_phases(const Model& m, const DecodeBufs& b, int B, float* kcache, float* vcache,
                                size_t cache_layer_stride, size_t cache_seq_stride, int max_ctx,

@@ -77,6 +77,9 @@ struct Session {
     // per-token log-probabilities: option "logprobs" (db.logprobs selects the kernel variants); lp_valid = the prefill
     // and every step since ran with it on, i.e. db.lp_out / db.eos_lp describe the current run
     bool lp_valid = false;
+    // top-k alternatives: option "top_logprobs" (top_k >= 1 sets db.topk and db.logprobs); tk_valid = the k the prefill
+    // and every step since ran with (0: none), i.e. db.tk_* describe the current run for k <= tk_valid
+    bool opt_logprobs = false; int top_k = 0, tk_valid = 0;
     ~Session();
 };
 
@@ -451,6 +454,14 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
         ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.eos_lp, 0xFF, B * sizeof(float), st));
         ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.lp_out, 0xFF, (size_t)B * s->max_new * sizeof(float), st));
     }
+    s->tk_valid = s->top_k;
+    if (s->db.topk) {                      // ids -1, values NaN (0xFFFFFFFF): nothing recorded yet
+        const size_t rows = (size_t)B * s->max_new * TK_MAX;
+        ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.tk_ids, 0xFF, rows * sizeof(int), st));
+        ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.tk_lp, 0xFF, rows * sizeof(float), st));
+        ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.tk_eos_ids, 0xFF, (size_t)B * TK_MAX * sizeof(int), st));
+        ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.tk_eos_lp, 0xFF, (size_t)B * TK_MAX * sizeof(float), st));
+    }
 
     launch_embed_inject(m.embed, c.hidden_size, s->d_ids, s->d_audio_row, s->audio, totS, s->hid, st);
     s->launches += 1;
@@ -547,6 +558,7 @@ void session_decode_step(Session* s, int64_t* next_ids_out, float* logits) {
     Model& m = *s->m; const int B = s->B;
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
     s->lp_valid = s->lp_valid && s->db.logprobs;
+    if (s->tk_valid != s->top_k) s->tk_valid = 0;
     // the id selected by the previous greedy application is the one this iteration consumes
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->h_next, s->db.next_id, B * sizeof(int), cudaMemcpyDeviceToHost, s->st));
     forward_step(s, logits != nullptr);
@@ -562,12 +574,13 @@ void session_generate(Session* s, int max_new_tokens, int32_t* ids_out, int32_t*
     Model& m = *s->m; const int B = s->B; cudaStream_t st = s->st;
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
     s->lp_valid = s->lp_valid && s->db.logprobs;     // switched off after the prefill: this run's record is incomplete
+    if (s->tk_valid != s->top_k) s->tk_valid = 0;    // top_logprobs changed after the prefill: likewise
     // Token 0 was selected at the end of prefill; each further token costs one forward + greedy.  The
     // reference also runs `forward` after the last appended token and discards its logits
     // (inference.rs:160-200); that wasted forward is not issued here.
     const int steps = std::max(0, max_new_tokens - s->greedy_done);
     auto ensure_graph = [&]() {   // per-phase path: ~142 launches per step -> replay them as one CUDA graph
-        const int mode_key = ((int)s->db.logprobs * 2 + s->decode_mode) * (s->max_batch + 1) + B;     // unique per (logprobs, mode, batch)
+        const int mode_key = (((int)s->db.topk * 2 + (int)s->db.logprobs) * 2 + s->decode_mode) * (s->max_batch + 1) + B;   // unique per (topk, logprobs, mode, batch)
         if (s->step_graph == nullptr || s->graph_mode != mode_key) {
             if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
             cudaGraph_t g = nullptr;
@@ -662,9 +675,66 @@ void session_last_logprobs(Session* s, int max_new_tokens, float* out, float* eo
     }
 }
 
+// top-k alternatives of the last run: [batch][max_new_tokens][k] ids and log-probabilities, best first, -1 / NaN at and
+// beyond the sequence's length; eos rows [batch][k] those of the step that selected the EOS ending sequence b
+void session_last_top_logprobs(Session* s, int max_new_tokens, int k, int32_t* ids_out, float* lp_out, int32_t* eos_ids_out,
+                               float* eos_lp_out) {
+    ASRB_REQUIRE(s->stage >= 3 && s->tk_valid > 0, ASRB_ERR_STATE,
+                 "last_top_logprobs: the last run did not record alternatives (set option top_logprobs before the prefill)");
+    ASRB_REQUIRE(max_new_tokens >= 1, ASRB_ERR_INVALID, "max_new_tokens must be >= 1");
+    ASRB_REQUIRE(k >= 1 && k <= s->tk_valid, ASRB_ERR_INVALID, "k must be in [1, top_logprobs of the last run]");
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    const int B = s->B;
+    std::vector<int32_t> ids((size_t)B * s->max_new * TK_MAX), eids((size_t)B * TK_MAX);
+    std::vector<float> lp(ids.size()), elp(eids.size());
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->h_nout, s->db.n_out, B * sizeof(int), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(ids.data(), s->db.tk_ids, ids.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(lp.data(), s->db.tk_lp, lp.size() * sizeof(float), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(eids.data(), s->db.tk_eos_ids, eids.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(elp.data(), s->db.tk_eos_lp, elp.size() * sizeof(float), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    const float nan = std::numeric_limits<float>::quiet_NaN();
+    for (int b = 0; b < B; ++b) {
+        const int n = std::min(s->h_nout[b], max_new_tokens);
+        for (int i = 0; i < max_new_tokens; ++i)
+            for (int j = 0; j < k; ++j) {
+                const size_t o = ((size_t)b * max_new_tokens + i) * k + j, src = ((size_t)b * s->max_new + i) * TK_MAX + j;
+                ids_out[o] = i < n ? ids[src] : -1;
+                lp_out[o] = i < n ? lp[src] : nan;
+            }
+        for (int j = 0; j < k; ++j) {
+            if (eos_ids_out) eos_ids_out[(size_t)b * k + j] = eids[(size_t)b * TK_MAX + j];
+            if (eos_lp_out) eos_lp_out[(size_t)b * k + j] = elp[(size_t)b * TK_MAX + j];
+        }
+    }
+}
+
 void session_stats(Session* s, int64_t* out, int n) {
     const int64_t v[5] = {s->n_batch_steps, s->n_mega_steps, s->n_phase_steps, g_gemm_simt_fallbacks.load(), g_gemm_tc_launches.load()};
     for (int i = 0; i < n && i < 5; ++i) out[i] = v[i];
+}
+
+// options "logprobs" / "top_logprobs" -> kernel variants; buffers are allocated when first needed, so a session that
+// never records keeps its allocations unchanged
+static void apply_record_options(Session* s) {
+    DecodeBufs& b = s->db;
+    b.logprobs = s->opt_logprobs || s->top_k > 0;    // the candidates' values need the selected token's log-probability
+    b.topk = s->top_k > 0;
+    if (b.logprobs && !b.lp_out) {
+        ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+        b.part_sum = salloc<float>(s, (size_t)s->max_batch * b.n_part);
+        b.lp_out = salloc<float>(s, (size_t)s->max_batch * s->max_new);
+        b.eos_lp = salloc<float>(s, s->max_batch);
+    }
+    if (b.topk && !b.tk_ids) {
+        ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+        b.tk_part_val = salloc<float>(s, (size_t)s->max_batch * b.n_part * TK_MAX);
+        b.tk_part_idx = salloc<int>(s, (size_t)s->max_batch * b.n_part * TK_MAX);
+        b.tk_ids = salloc<int>(s, (size_t)s->max_batch * s->max_new * TK_MAX);
+        b.tk_lp = salloc<float>(s, (size_t)s->max_batch * s->max_new * TK_MAX);
+        b.tk_eos_ids = salloc<int>(s, (size_t)s->max_batch * TK_MAX);
+        b.tk_eos_lp = salloc<float>(s, (size_t)s->max_batch * TK_MAX);
+    }
 }
 
 void session_set_option(Session* s, const char* key, const char* value) {
@@ -686,14 +756,12 @@ void session_set_option(Session* s, const char* key, const char* value) {
         s->resident = (v == "1");
     } else if (k == "logprobs") {
         ASRB_REQUIRE(v == "1" || v == "0", ASRB_ERR_INVALID, "logprobs must be 1|0");
-        DecodeBufs& b = s->db;
-        if (v == "1" && !b.lp_out) {      // first enabled: a session that never records keeps its allocations unchanged
-            ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
-            b.part_sum = salloc<float>(s, (size_t)s->max_batch * b.n_part);
-            b.lp_out = salloc<float>(s, (size_t)s->max_batch * s->max_new);
-            b.eos_lp = salloc<float>(s, s->max_batch);
-        }
-        b.logprobs = (v == "1");
+        s->opt_logprobs = (v == "1");
+        apply_record_options(s);
+    } else if (k == "top_logprobs") {
+        ASRB_REQUIRE(v.size() == 1 && v[0] >= '0' && v[0] < '0' + 1 + TK_MAX, ASRB_ERR_INVALID, "top_logprobs must be 0..8");
+        s->top_k = v[0] - '0';
+        apply_record_options(s);
     } else throw Error(ASRB_ERR_INVALID, "unknown option: " + k);
 }
 

@@ -13,7 +13,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -49,6 +49,13 @@ def avg_logprob(token_logprobs: Sequence[float], eos_logprob: Optional[float]) -
     return sum(vals) / len(vals) if vals else None
 
 
+def check_top_logprobs(top_logprobs) -> int:
+    """The `top_logprobs` argument as an int in 0..8 (0: off), else ValueError."""
+    if not isinstance(top_logprobs, (int, np.integer)) or isinstance(top_logprobs, bool) or not 0 <= top_logprobs <= 8:
+        raise ValueError(f"top_logprobs must be an int in 0..8, got {top_logprobs!r}")
+    return int(top_logprobs)
+
+
 @dataclass
 class TranscribeResult:           # inference.rs:270-274
     text: str
@@ -57,6 +64,9 @@ class TranscribeResult:           # inference.rs:270-274
     ids: List[int]
     token_logprobs: Optional[List[float]] = None    # transcribe(logprobs=True): log p of each id
     avg_logprob: Optional[float] = None             # avg_logprob(token_logprobs, EOS log p)
+    # transcribe(top_logprobs=k): per id, the k best candidates of its step as (id, log p), best first (entry 0 = the id)
+    top_logprobs: Optional[List[List[Tuple[int, float]]]] = None
+    eos_top_logprobs: Optional[List[Tuple[int, float]]] = None   # ... of the step that selected EOS (None: stopped by the cap)
 
 
 @dataclass
@@ -67,6 +77,10 @@ class TranscribeIds:
     decode_steps: int
     logprobs: Optional[List[List[float]]] = None         # logprobs=True: natural-log probability of each id
     eos_logprobs: Optional[List[Optional[float]]] = None  # ... of the EOS id that ended the utterance (None: stopped at max_new_tokens)
+    # top_logprobs=k: per utterance, per id, the k best candidates of the step that selected it as (id, log p), best first
+    top_logprobs: Optional[List[List[List[Tuple[int, float]]]]] = None
+    # ... of the step that selected the EOS ending the utterance (None: stopped at max_new_tokens)
+    eos_top_logprobs: Optional[List[Optional[List[Tuple[int, float]]]]] = None
 
 
 class AsrInference:
@@ -234,22 +248,58 @@ class AsrInference:
             rows.append([float(v) for v in r[: nan[0] if len(nan) else len(r)]])
         return rows, [None if np.isnan(e) else float(e) for e in eos[:B]]
 
-    def _finish(self, s, B: int, ids, n, max_new_tokens: int, logprobs: bool) -> TranscribeIds:
+    # ---- top-k alternatives (session option "top_logprobs") ------------------------------------
+    def _record_top_logprobs(self, s, k: int, on: bool) -> None:
+        """Record k >= 1 alternatives for one call (True) or go back to the engine's configured value (False).  Nothing
+        is set when the two agree (setting an option drops the captured per-phase step graph)."""
+        conf = self._options.get("top_logprobs", "0")
+        if conf != str(k):
+            _lib.check(self._lib.asrb_session_set_option(s, b"top_logprobs", (str(k) if on else conf).encode()))
+
+    def last_top_logprobs(self, max_new_tokens: int, k: int):
+        """asrb_last_top_logprobs: (per utterance, per id of the last run, the k best candidates of its step as
+        (id, log p) pairs, best first; per utterance the same for the step that selected the ending EOS, or None).
+        Raises AsrbError: ASRB_ERR_STATE when the last run did not record them, ASRB_ERR_INVALID when k is outside
+        [1, the recorded top_logprobs]."""
+        if self._session is None:
+            raise _lib.AsrbError(4, "no session: nothing has run yet")
+        cap = self._cap[0]
+        ids = np.full((cap, max_new_tokens, max(k, 1)), -1, dtype=np.int32)
+        lp = np.full(ids.shape, np.nan, dtype=np.float32)
+        eids = np.full((cap, max(k, 1)), -1, dtype=np.int32)
+        elp = np.full(eids.shape, np.nan, dtype=np.float32)
+        _lib.check(self._lib.asrb_last_top_logprobs(
+            self._session, int(max_new_tokens), int(k), ids.ctypes.data_as(C.POINTER(C.c_int32)),
+            lp.ctypes.data_as(C.POINTER(C.c_float)), eids.ctypes.data_as(C.POINTER(C.c_int32)),
+            elp.ctypes.data_as(C.POINTER(C.c_float))))
+        B = getattr(self, "_B", cap)
+        rows = []
+        for b in range(B):                                   # the rows before the utterance's length (-1 from there on)
+            n = int(np.count_nonzero(ids[b, :, 0] >= 0))
+            rows.append([[(int(i), float(v)) for i, v in zip(ids[b, t], lp[b, t])] for t in range(n)])
+        eos = [None if eids[b, 0] < 0 else [(int(i), float(v)) for i, v in zip(eids[b], elp[b])] for b in range(B)]
+        return rows, eos
+
+    def _finish(self, s, B: int, ids, n, max_new_tokens: int, logprobs: bool, top_logprobs: int = 0) -> TranscribeIds:
         ms = (C.c_float * 6)()
         k, st = C.c_int64(), C.c_int64()
         _lib.check(self._lib.asrb_last_timings(s, ms, C.byref(k), C.byref(st)))
         names = ("h2d", "mel", "encoder", "prefill", "decode", "total")
         r = TranscribeIds([ids[b, : n[b]].tolist() for b in range(B)], dict(zip(names, ms)), k.value, st.value)
         self._B = B
-        if logprobs:
+        if logprobs or top_logprobs:
             r.logprobs, r.eos_logprobs = self.last_logprobs(max_new_tokens)
+        if top_logprobs:
+            r.top_logprobs, r.eos_top_logprobs = self.last_top_logprobs(max_new_tokens, top_logprobs)
         return r
 
     # ---- the hot path ----------------------------------------------------------------
     def transcribe_ids(self, clips: Sequence[np.ndarray], language_ids: Optional[Sequence] = None,
-                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False) -> TranscribeIds:
+                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0) -> TranscribeIds:
         """transcribe() steps 2-8 for a batch: host f32 samples in, host token ids out (and, with `logprobs`, the
-        log-probability of every id and of the ending EOS, from the kernels that selected them)."""
+        log-probability of every id and of the ending EOS, from the kernels that selected them; with `top_logprobs` = k
+        in 1..8, also the k best candidates of each of those steps, and the log-probabilities as with `logprobs`)."""
+        top_logprobs = check_top_logprobs(top_logprobs)
         B = len(clips)
         arrs, ptrs, lens = self._pack_samples(clips)
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
@@ -258,14 +308,18 @@ class AsrInference:
         n = np.zeros(B, dtype=np.int32)
         if logprobs:
             self._record_logprobs(s, True)
+        if top_logprobs:
+            self._record_top_logprobs(s, top_logprobs, True)
         try:
             _lib.check(self._lib.asrb_transcribe_ids(
                 s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
                 ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
-            return self._finish(s, B, ids, n, max_new_tokens, logprobs)
+            return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs)
         finally:
             if logprobs:
                 self._record_logprobs(s, False)
+            if top_logprobs:
+                self._record_top_logprobs(s, top_logprobs, False)
 
     # ---- GPU-side audio ingest (step 1, src/audio.rs:162-245) -------------------------------------------
     _PCM_FMT = {"int16": 0, "float32": 1, "int32": 2}
@@ -298,9 +352,10 @@ class AsrInference:
         return out
 
     def transcribe_pcm(self, pcms: Sequence, rates: Sequence[int], language_ids: Optional[Sequence] = None,
-                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False) -> TranscribeIds:
-        """transcribe() steps 1-8 for a batch with step 1 on the GPU: raw PCM in, token ids out (`logprobs`: as in
-        transcribe_ids)."""
+                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0) -> TranscribeIds:
+        """transcribe() steps 1-8 for a batch with step 1 on the GPU: raw PCM in, token ids out (`logprobs`,
+        `top_logprobs`: as in transcribe_ids)."""
+        top_logprobs = check_top_logprobs(top_logprobs)
         B = len(pcms)
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
         s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens)
@@ -308,37 +363,46 @@ class AsrInference:
         n = np.zeros(B, dtype=np.int32)
         if logprobs:
             self._record_logprobs(s, True)
+        if top_logprobs:
+            self._record_top_logprobs(s, top_logprobs, True)
         try:
             _lib.check(self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens),
                                                           ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
-            return self._finish(s, B, ids, n, max_new_tokens, logprobs)
+            return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs)
         finally:
             if logprobs:
                 self._record_logprobs(s, False)
+            if top_logprobs:
+                self._record_top_logprobs(s, top_logprobs, False)
 
     def transcribe(self, audio_path: str, language: Optional[str] = None,
-                   max_new_tokens: int = MAX_NEW_TOKENS, gpu_ingest: bool = True, logprobs: bool = False) -> TranscribeResult:
+                   max_new_tokens: int = MAX_NEW_TOKENS, gpu_ingest: bool = True, logprobs: bool = False,
+                   top_logprobs: int = 0) -> TranscribeResult:
         """AsrInference::transcribe (inference.rs:89-213): step 1 (WAV payload -> mono 16 kHz; on the GPU by default,
         `gpu_ingest=False` = the host loader) -> steps 2-8 on the GPU -> step 9 (detokenise + parse, host; needs
-        tokenizer.json, else raw_output is the id list as text).  `logprobs`: also fill token_logprobs / avg_logprob."""
+        tokenizer.json, else raw_output is the id list as text).  `logprobs`: also fill token_logprobs / avg_logprob;
+        `top_logprobs` = k in 1..8: also fill top_logprobs (and token_logprobs / avg_logprob)."""
         from .audio import load_wav, read_wav_pcm
         from .text import language_prompt_ids, parse_asr_output
         lang_ids = language_prompt_ids(self.tokenizer, language)
         if gpu_ingest:
             pcm, rate = read_wav_pcm(audio_path)
             r = self.transcribe_pcm([pcm], [rate], language_ids=[lang_ids] if lang_ids is not None else None,
-                                    max_new_tokens=max_new_tokens, logprobs=logprobs)
+                                    max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs)
         else:
             samples = load_wav(audio_path, MEL_SAMPLE_RATE)
             r = self.transcribe_ids([samples], language_ids=[lang_ids] if lang_ids is not None else None,
-                                    max_new_tokens=max_new_tokens, logprobs=logprobs)
+                                    max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs)
         ids = r.ids[0]
         raw = self.tokenizer.decode(ids) if self.tokenizer is not None else " ".join(str(i) for i in ids)
         lang, text = parse_asr_output(raw, language is not None) if self.tokenizer is not None else ("unknown", raw)
         res = TranscribeResult(text=text, language=lang, raw_output=raw, ids=ids)
-        if logprobs:
+        if logprobs or top_logprobs:
             res.token_logprobs = r.logprobs[0]
             res.avg_logprob = avg_logprob(r.logprobs[0], r.eos_logprobs[0])
+        if top_logprobs:
+            res.top_logprobs = r.top_logprobs[0]
+            res.eos_top_logprobs = r.eos_top_logprobs[0]
         return res
 
     # ---- stage-level calls (the calls transcribe() makes; used by the parity tests) ----

@@ -106,4 +106,37 @@ impl B200Engine {
         check(unsafe { ffi::asrb_session_set_option(session, key.as_ptr(), off.as_ptr()) })?;
         run
     }
+
+    /// `transcribe_ids` that also returns, for every generated id, the `k` (1..=8) best candidates of the decode step
+    /// that selected it as `(id, natural-log probability)` pairs, best first (entry 0 is the id itself), and the same
+    /// for the step that selected the EOS ending the sequence (`None` when it stopped at `max_new_tokens`).  The
+    /// candidates come from the decode kernels, under the same fp32 logits that selected the ids
+    /// (`asrb_last_top_logprobs`).  The ids are those `transcribe_ids` returns.
+    pub fn transcribe_ids_with_top_logprobs(&self, samples: &[f32], lang_ids: Option<&[i64]>, k: usize)
+        -> Result<(Vec<i64>, Vec<Vec<(i64, f32)>>, Option<Vec<(i64, f32)>>)> {
+        if !(1..=8).contains(&k) { return Err(anyhow!("top_logprobs k must be in 1..=8, got {k}")); }
+        let session = self.session_for(samples.len())?;
+        let key = CString::new("top_logprobs")?;
+        let on = CString::new(k.to_string())?;
+        let off = CString::new("0")?;
+        check(unsafe { ffi::asrb_session_set_option(session, key.as_ptr(), on.as_ptr()) })?;
+        let run = (|| -> Result<(Vec<i64>, Vec<Vec<(i64, f32)>>, Option<Vec<(i64, f32)>>)> {
+            let ids = self.transcribe_ids(samples, lang_ids)?;
+            let mut cid = vec![-1i32; self.max_new_tokens * k];
+            let mut clp = vec![0f32; self.max_new_tokens * k];
+            let mut eid = vec![-1i32; k];
+            let mut elp = vec![0f32; k];
+            check(unsafe {
+                ffi::asrb_last_top_logprobs(session, self.max_new_tokens as i32, k as i32, cid.as_mut_ptr(), clp.as_mut_ptr(),
+                                            eid.as_mut_ptr(), elp.as_mut_ptr())
+            })?;
+            let rows = (0..ids.len())
+                .map(|t| (0..k).map(|j| (cid[t * k + j] as i64, clp[t * k + j])).collect())
+                .collect();
+            let eos = if eid[0] < 0 { None } else { Some((0..k).map(|j| (eid[j] as i64, elp[j])).collect()) };
+            Ok((ids, rows, eos))
+        })();
+        check(unsafe { ffi::asrb_session_set_option(session, key.as_ptr(), off.as_ptr()) })?;
+        run
+    }
 }
