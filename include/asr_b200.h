@@ -173,7 +173,18 @@ ASRB_API int asrb_session_stats(asrb_session* s, int64_t* out, int n);
  * asrb_last_logprobs; same ids, same decode paths; the value in effect at the prefill applies to the whole run),
  * "top_logprobs" = "0".."8" (k >= 1: every greedy step also records its k best candidates, read with
  * asrb_last_top_logprobs, and the log-probabilities asrb_last_logprobs reads; same ids, same decode paths; the value in
- * effect at the prefill applies to the whole run) */
+ * effect at the prefill applies to the whole run),
+ * "temperature" = a decimal string, "0" (default: greedy) or a finite value in [1e-6, 100]: every step samples its
+ * token by the Gumbel-max draw below instead of taking the argmax, on every decode path,
+ * "seed" = a decimal unsigned 64-bit integer (default "0") seeding that draw.
+ * Both are latched at the prefill and apply to the whole run.  The draw for sequence row r (0-based in the call's
+ * batch), step n (ids already generated for that sequence when the step selects; 0 after the prefill) and token id v:
+ * x0 = word 0 of Philox4x32-10 (Random123 constants) with key (seed & 0xffffffff, seed >> 32) and counter (v, n, r, 0),
+ * u = (float)((x0 >> 8) | 1) * 2^-24, g = -logf(-logf(u)), key = fmaf(logit, (float)(1.0 / T), g); the selected id is
+ * the argmax of the keys under (key descending, id ascending).  Ids are bitwise deterministic for a given (inputs, seed,
+ * temperature, batch order).  With "logprobs" the record holds the model's own log-probability of the sampled id.
+ * temperature > 0 with top_logprobs >= 1 is refused with ASRB_ERR_INVALID by asrb_prefill, asrb_transcribe_ids and
+ * asrb_transcribe_ingested, before any work. */
 ASRB_API int asrb_session_set_option(asrb_session* s, const char* key, const char* value);
 
 /* Per-token log-probabilities of the last run (asrb_generate / asrb_transcribe_ids / asrb_transcribe_ingested, or

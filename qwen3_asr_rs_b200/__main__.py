@@ -1,10 +1,13 @@
 """CLI mirroring the reference's `asr <model_dir> <audio_file> [language]` (/root/reference/src/main.rs:7-81).
 `--logprobs` (anywhere on the line) also prints the utterance's average token log-probability.
 `--top-logprobs N` (N in 1..8, anywhere on the line) also prints, for every generated token and the ending EOS, the N
-best candidates of the step that selected it with their log-probabilities."""
+best candidates of the step that selected it with their log-probabilities.
+`--temperature T[,T...]` samples with temperature T (a list is a fallback schedule), `--seed N` seeds the draw; both
+anywhere on the line, and `Temperature: x` reports the temperature of the kept attempt."""
 import sys
 
-USAGE = "Usage: python -m qwen3_asr_rs_b200 <model_dir> <audio_file> [language] [--logprobs] [--top-logprobs N]"
+USAGE = ("Usage: python -m qwen3_asr_rs_b200 <model_dir> <audio_file> [language] [--logprobs] [--top-logprobs N] "
+         "[--temperature T[,T...]] [--seed N]")
 
 
 def parse_args(argv):
@@ -39,6 +42,51 @@ def split_top_logprobs(argv):
     return rest, k
 
 
+def _take_flag(argv, name):
+    """Remove `name V` / `name=V` from argv -> (remaining argv, V or None when absent), or None when it has no value."""
+    rest, val, i = [], None, 0
+    while i < len(argv):
+        a = argv[i]
+        if a == name or a.startswith(name + "="):
+            if "=" in a:
+                val = a.split("=", 1)[1]
+            elif i + 1 < len(argv):
+                val = argv[i + 1]
+                i += 1
+            else:
+                return None
+        else:
+            rest.append(a)
+        i += 1
+    return rest, val
+
+
+def split_sampling(argv):
+    """Remove `--temperature T[,T...]` and `--seed N` from argv -> (remaining argv, temperature, seed), where temperature
+    is None when absent, a float, or a tuple for a comma-separated schedule, and seed is 0 when absent; None when a value
+    is missing or invalid."""
+    from .inference import check_seed, check_temperature
+    t = _take_flag(argv, "--temperature")
+    if t is None:
+        return None
+    sd = _take_flag(t[0], "--seed")
+    if sd is None:
+        return None
+    temperature, seed = None, 0
+    try:
+        if t[1] is not None:
+            parts = t[1].split(",")
+            vals = check_temperature(tuple(float(v) for v in parts))
+            temperature = vals if len(parts) > 1 else vals[0]
+        if sd[1] is not None:
+            if not sd[1].isdigit():
+                return None
+            seed = check_seed(int(sd[1]))
+    except ValueError:
+        return None
+    return sd[0], temperature, seed
+
+
 def format_candidates(cands, decode) -> str:
     """One line of candidates: `'text' -0.0123` pairs, best first; `decode([id])` gives each candidate's text."""
     return "  ".join(f"{decode([i])!r} {lp:.4f}" for i, lp in cands)
@@ -46,7 +94,8 @@ def format_candidates(cands, decode) -> str:
 
 def main(argv=None) -> int:
     argv = list(sys.argv[1:] if argv is None else argv)
-    split = split_top_logprobs(argv)
+    sampling = split_sampling(argv)
+    split = split_top_logprobs(sampling[0]) if sampling is not None else None
     args = parse_args(split[0]) if split is not None else None
     if args is None:
         print(USAGE, file=sys.stderr)   # main.rs:18-27
@@ -56,12 +105,16 @@ def main(argv=None) -> int:
     from . import AsrInference
     eng = AsrInference.load(model_dir, device=0)
     try:
-        r = eng.transcribe(audio, language, logprobs=logprobs, top_logprobs=top)
+        _, temperature, seed = sampling
+        kw = {} if temperature is None else dict(temperature=temperature, seed=seed)
+        r = eng.transcribe(audio, language, logprobs=logprobs, top_logprobs=top, **kw)
         decode = eng.tokenizer.decode if eng.tokenizer is not None else (lambda ids: " ".join(str(i) for i in ids))
     finally:
         eng.close()
     print(f"Language: {r.language}")                       # main.rs:77-78
     print(f"Text: {r.text}")
+    if r.temperature is not None:
+        print(f"Temperature: {r.temperature:g}")
     if logprobs:
         print(f"Avg logprob: {r.avg_logprob:.4f}" if r.avg_logprob is not None else "Avg logprob: n/a")
     if top:

@@ -170,6 +170,72 @@ __device__ __forceinline__ void tk_write(const TopK& t, float lp, int* ids, floa
     for (int j = 0; j < TK_MAX; ++j) { ids[j] = t.i[j]; lps[j] = j == 0 ? lp : (t.v[j] - t.v[0]) + lp; }
 }
 
+// ---- seeded temperature sampling by the Gumbel-max trick ------------------------------------------------
+// For sequence row r (0-based in the call's batch), step n (ids already generated for that sequence when the step
+// selects; 0 for the token selected after the prefill, the EOS-selecting step included) and token id v:
+//   x0    = word 0 of Philox4x32-10 (Random123 constants), key (seed & 0xffffffff, seed >> 32), counter (v, n, r, 0)
+//   u     = (float)((x0 >> 8) | 1) * 2^-24               exact, in [2^-24, 1 - 2^-24]: never 0 or 1
+//   g_v   = -logf(-logf(u))                              full-precision logf, g in about [-2.8, 16.6]
+//   key_v = fmaf(l_v, inv_t, g_v)                        inv_t = (float)(1.0 / T), computed on the host in double
+// and the selected id is the argmax of key_v under (key descending, id ascending), the greedy argmax's own order.  The
+// draw is a pure function of (seed, r, n, v): every decode path selects the same ids, whatever its merge order.
+// With LOGPROB the kernels also keep the raw (max, sum of exponentials) record of the logits and the raw logit of the
+// best-key row, so the recorded value is the model's own (temperature-1) log-probability (l_sel - M) - log S.
+struct SampleParams {       // device-resident, written at the prefill: a captured graph reads the values of its run
+    float inv_t;            // 1 / temperature
+    uint32_t k0, k1;        // seed & 0xffffffff, seed >> 32
+};
+__host__ __device__ __forceinline__ uint32_t philox4x32_10_x0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1) {
+#pragma unroll
+    for (int i = 0; i < 10; ++i) {
+        if (i > 0) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+        const uint64_t p0 = (uint64_t)0xD2511F53u * c0, p1 = (uint64_t)0xCD9E8D57u * c2;
+        const uint32_t n0 = (uint32_t)(p1 >> 32) ^ c1 ^ k0, n2 = (uint32_t)(p0 >> 32) ^ c3 ^ k1;
+        c0 = n0; c1 = (uint32_t)p1; c2 = n2; c3 = (uint32_t)p0;
+    }
+    return c0;
+}
+// one sequence's draw context: the run's parameters and the (step, row) of the counter
+struct Draw {
+    float inv_t; uint32_t k0, k1, n, r;
+};
+__device__ __forceinline__ Draw make_draw(const SampleParams* sp, int n, int r) {
+    Draw d; d.inv_t = __ldg(&sp->inv_t); d.k0 = __ldg(&sp->k0); d.k1 = __ldg(&sp->k1); d.n = (uint32_t)n; d.r = (uint32_t)r;
+    return d;
+}
+__device__ __forceinline__ float gumbel_noise(uint32_t x0) {
+    const float u = (float)((x0 >> 8) | 1u) * 0x1p-24f;
+    return -logf(-logf(u));
+}
+__device__ __forceinline__ float sample_key(const Draw& d, float l, int v) {
+    return fmaf(l, d.inv_t, gumbel_noise(philox4x32_10_x0((uint32_t)v, d.n, d.r, 0u, d.k0, d.k1)));
+}
+// fold logit l of `row` (rows ascend per thread: strict > keeps the first maximum): (best_v, best_i) = argmax of the
+// keys; LOGPROB: (m, best_s) = raw (max, sum of exp(l - m)) record, sel = raw logit of the best-key row
+template <bool LOGPROB>
+__device__ __forceinline__ void sample_fold(const Draw& d, float l, int row, float& best_v, int& best_i, float& best_s, float& m,
+                                            float& sel) {
+    const float k = sample_key(d, l, row);
+    if (k > best_v) { best_v = k; best_i = row; if constexpr (LOGPROB) sel = l; }
+    if constexpr (LOGPROB) {
+        if (l > m) { best_s = lse_rescale(best_s, m, l) + 1.f; m = l; }
+        else best_s += expf(l - m);
+    }
+}
+// merge with the records of lane ^ o (both lanes end with the same records)
+template <bool LOGPROB>
+__device__ __forceinline__ void sample_merge_xor(int o, float& best_v, int& best_i, float& best_s, float& m, float& sel) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best_v, o); const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
+    float osel = 0.f;
+    if constexpr (LOGPROB) {
+        osel = __shfl_xor_sync(0xffffffffu, sel, o);
+        const float om = __shfl_xor_sync(0xffffffffu, m, o);
+        best_s = lse_merge(m, best_s, om, __shfl_xor_sync(0xffffffffu, best_s, o));
+        m = fmaxf(m, om);
+    }
+    if (ov > best_v || (ov == best_v && oi < best_i)) { best_v = ov; best_i = oi; if constexpr (LOGPROB) sel = osel; }
+}
+
 // order-preserving float <-> int key (for atomicMax on floats of either sign)
 __device__ __host__ __forceinline__ int float_to_ordered(float f) {
 #ifdef __CUDA_ARCH__

@@ -20,7 +20,10 @@ namespace asrb {
 
 static constexpr int DG_THREADS = 256, DG_WARPS = 8;
 // DE_ARGMAX_LSE: DE_ARGMAX + per-CTA sum of exp(logit - max) (part_sum), the partial record of the token log-probability
-enum { DE_STORE = 0, DE_RESID = 1, DE_SWIGLU = 2, DE_ARGMAX = 3, DE_ARGMAX_LSE = 4 };
+// DE_ARGMAX_GUMBEL: argmax of the sampling keys fmaf(logit, inv_t, g) instead of the logits (common.cuh); part_val holds
+// the CTA's best key.  DE_ARGMAX_GUMBEL_LSE: + the raw (max, sum) record (part_max, part_sum) and the raw logit of the
+// best-key row (part_sel)
+enum { DE_STORE = 0, DE_RESID = 1, DE_SWIGLU = 2, DE_ARGMAX = 3, DE_ARGMAX_LSE = 4, DE_ARGMAX_GUMBEL = 5, DE_ARGMAX_GUMBEL_LSE = 6 };
 
 struct GemvParams {
     const bf16* W; int N, K;
@@ -32,14 +35,23 @@ struct GemvParams {
     int B;
     float* part_sum;                                // ARGMAX_LSE: [B][gridDim.x]
 };
+// ARGMAX_GUMBEL*: a second kernel argument (the `sample` pack), so the parameter block of the other epilogues stays as it is
+struct GemvSample {
+    const SampleParams* smp;                        // the run's 1 / temperature and seed
+    const int* n_out; int row0;                     // each sequence's step n (= ids generated so far), global row of sequence 0
+    float* part_max; float* part_sel;               // ARGMAX_GUMBEL_LSE: [B][gridDim.x]
+};
 
-template <int MAXB, bool PRE_NORM, int EPI>
-__global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p) {
+template <typename... S> __device__ __forceinline__ const GemvSample& gemv_sample(const S&... s) { return (s, ...); }
+
+template <int MAXB, bool PRE_NORM, int EPI, typename... Sample>
+__global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p, Sample... sample) {
     extern __shared__ float xs[];          // [MAXB][K]
     __shared__ float red[32];
     __shared__ float bestv[DG_WARPS][MAXB];
     __shared__ int besti[DG_WARPS][MAXB];
-    constexpr bool ARGMAX = EPI == DE_ARGMAX || EPI == DE_ARGMAX_LSE, LSE = EPI == DE_ARGMAX_LSE;
+    constexpr bool SMP = EPI == DE_ARGMAX_GUMBEL || EPI == DE_ARGMAX_GUMBEL_LSE, SLSE = EPI == DE_ARGMAX_GUMBEL_LSE;
+    constexpr bool ARGMAX = EPI == DE_ARGMAX || EPI == DE_ARGMAX_LSE || SMP, LSE = EPI == DE_ARGMAX_LSE;
     const int K = p.K, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     for (int b = 0; b < MAXB; ++b) {
         if (b < p.B) {
@@ -62,9 +74,19 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p) {
     const int per_cta = (units + gridDim.x - 1) / gridDim.x;
     const int u0 = blockIdx.x * per_cta, u1 = min(units, u0 + per_cta);
     float bv[MAXB]; int bi[MAXB];
-    float bs[LSE ? MAXB : 1];                     // LSE: sum of exp(logit - bv[b]) over this warp's rows
+    float bs[(LSE || SLSE) ? MAXB : 1];           // LSE: sum of exp(logit - bv[b]) over this warp's rows (SLSE: - bm[b])
+    float bm[SLSE ? MAXB : 1], bsel[SLSE ? MAXB : 1];   // SLSE: raw maximum logit, raw logit of the best-key row
 #pragma unroll
     for (int b = 0; b < MAXB; ++b) { bv[b] = -INFINITY; bi[b] = 0x7fffffff; if constexpr (LSE) bs[b] = 0.f; }
+    Draw dr[SMP ? MAXB : 1];                      // SMP: each sequence's draw (global row row0 + b, step n_out[b])
+    if constexpr (SMP) {
+#pragma unroll
+        for (int b = 0; b < MAXB; ++b) {
+            const GemvSample& ps = gemv_sample(sample...);
+            dr[b] = make_draw(ps.smp, b < p.B ? __ldg(ps.n_out + b) : 0, ps.row0 + b);
+            if constexpr (SLSE) { bs[b] = 0.f; bm[b] = -INFINITY; bsel[b] = 0.f; }
+        }
+    }
     for (int u = u0 + warp; u < u1; u += DG_WARPS) {
         float acc[RSTEP][MAXB];
 #pragma unroll
@@ -102,13 +124,18 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p) {
                 if (EPI == DE_SWIGLU) p.out[(size_t)b * p.ldo + u] = silu(acc[0][b]) * acc[RSTEP - 1][b];
                 if (ARGMAX) {
                     if (p.logits) p.logits[(size_t)b * p.ldl + u] = acc[0][b];
-                    if constexpr (LSE) lse_fold(acc[0][b], u, bv[b], bi[b], bs[b]);
+                    if constexpr (SMP) {
+                        float unused = 0.f;
+                        if constexpr (SLSE) sample_fold<true>(dr[b], acc[0][b], u, bv[b], bi[b], bs[b], bm[b], bsel[b]);
+                        else sample_fold<false>(dr[b], acc[0][b], u, bv[b], bi[b], unused, unused, unused);
+                    }
+                    else if constexpr (LSE) lse_fold(acc[0][b], u, bv[b], bi[b], bs[b]);
                     else if (acc[0][b] > bv[b]) { bv[b] = acc[0][b]; bi[b] = u; }   // rows ascend per warp: first max wins
                 }
             }
         }
     }
-    if (EPI == DE_ARGMAX) {
+    if (EPI == DE_ARGMAX || EPI == DE_ARGMAX_GUMBEL) {      // GUMBEL: the same merge over the keys
         if (lane == 0)
             for (int b = 0; b < MAXB; ++b) { bestv[warp][b] = bv[b]; besti[warp][b] = bi[b]; }
         __syncthreads();
@@ -136,19 +163,46 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p) {
             p.part_sum[(size_t)tid * gridDim.x + blockIdx.x] = sum;
         }
     }
+    if constexpr (SLSE) {
+        __shared__ float bests[DG_WARPS][MAXB], bestm[DG_WARPS][MAXB], bestsel[DG_WARPS][MAXB];
+        if (lane == 0)
+            for (int b = 0; b < MAXB; ++b) {
+                bestv[warp][b] = bv[b]; besti[warp][b] = bi[b]; bests[warp][b] = bs[b]; bestm[warp][b] = bm[b]; bestsel[warp][b] = bsel[b];
+            }
+        __syncthreads();
+        if (tid < p.B) {
+            float v = -INFINITY; int idx = 0x7fffffff, ws = 0; float M = -INFINITY;
+            for (int w = 0; w < DG_WARPS; ++w) {
+                if (bestv[w][tid] > v || (bestv[w][tid] == v && besti[w][tid] < idx)) { v = bestv[w][tid]; idx = besti[w][tid]; ws = w; }
+                M = fmaxf(M, bestm[w][tid]);
+            }
+            float sum = 0.f;                     // the warps' raw sums rescaled to the CTA's raw maximum, in warp order
+            for (int w = 0; w < DG_WARPS; ++w) sum += lse_rescale(bests[w][tid], bestm[w][tid], M);
+            const size_t o = (size_t)tid * gridDim.x + blockIdx.x;
+            const GemvSample& ps = gemv_sample(sample...);
+            p.part_val[o] = v; p.part_idx[o] = idx; p.part_sum[o] = sum; ps.part_max[o] = M; ps.part_sel[o] = bestsel[ws][tid];
+        }
+    }
 }
 
 template <bool PRE_NORM, int EPI>
-static void run_gemv(const GemvParams& p, int grid, cudaStream_t st) {
+static void run_gemv(const GemvParams& p, int grid, cudaStream_t st, const GemvSample* ps = nullptr) {
     size_t smem_of[4] = {(size_t)1 * p.K * 4, (size_t)2 * p.K * 4, (size_t)4 * p.K * 4, (size_t)8 * p.K * 4};
     ASRB_REQUIRE(p.K % 256 == 0, ASRB_ERR_INVALID, "decode GEMV needs K % 256 == 0");
     ASRB_REQUIRE(p.B >= 1 && p.B <= 8, ASRB_ERR_INVALID, "per-phase decode supports batch 1..8");
 #define ASRB_GEMV_CASE(MB, IDX)                                                                              \
     {                                                                                                        \
-        auto kern = dec_gemv_kernel<MB, PRE_NORM, EPI>;                                                      \
-        if (smem_of[IDX] > 48 * 1024)                                                                        \
-            ASRB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of[IDX])); \
-        kern<<<grid, DG_THREADS, smem_of[IDX], st>>>(p);                                                     \
+        if constexpr (EPI == DE_ARGMAX_GUMBEL || EPI == DE_ARGMAX_GUMBEL_LSE) {                              \
+            auto kern = dec_gemv_kernel<MB, PRE_NORM, EPI, GemvSample>;                                      \
+            if (smem_of[IDX] > 48 * 1024)                                                                    \
+                ASRB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of[IDX])); \
+            kern<<<grid, DG_THREADS, smem_of[IDX], st>>>(p, *ps);                                            \
+        } else {                                                                                             \
+            auto kern = dec_gemv_kernel<MB, PRE_NORM, EPI>;                                                  \
+            if (smem_of[IDX] > 48 * 1024)                                                                    \
+                ASRB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of[IDX])); \
+            kern<<<grid, DG_THREADS, smem_of[IDX], st>>>(p);                                                 \
+        }                                                                                                    \
     }
     if (p.B == 1) ASRB_GEMV_CASE(1, 0)
     else if (p.B == 2) ASRB_GEMV_CASE(2, 1)
@@ -237,44 +291,56 @@ __global__ void __launch_bounds__(128) dec_attn_kernel(const float* __restrict__
 // lp_out (appended token) or eos_lp (EOS).
 // TOPK (with LOGPROB): also select the TK_MAX best (logit, id) pairs of the step's logits [B][vocab] (written by the
 // lm_head GEMV) and store them in tk_ids / tk_lp [B][max_new][TK_MAX] or the EOS rows tk_eos_ids / tk_eos_lp [B][TK_MAX].
+// SAMPLE (with LOGPROB; without it the plain kernel merges the keys): part_val holds keys, the raw records are
+// (part_max, part_sum) and part_sel the raw logit of each record's best-key row; the value recorded is (l_sel - M) - log S.
 // grid = B blocks.
 // ---------------------------------------------------------------------------------------------
-template <bool LOGPROB, bool TOPK = false>
+template <bool LOGPROB, bool TOPK = false, bool SAMPLE = false>
 __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __restrict__ part_idx, int n_part,
                               int* __restrict__ done, int* __restrict__ pos, int* __restrict__ next_id,
                               int* __restrict__ ids_out, int* __restrict__ n_out, int max_new,
                               const bf16* __restrict__ embed, int hidden, float* __restrict__ x,
                               const float* __restrict__ part_sum, float* __restrict__ lp_out, float* __restrict__ eos_lp,
                               const float* __restrict__ logits, int vocab, int* __restrict__ tk_ids, float* __restrict__ tk_lp,
-                              int* __restrict__ tk_eos_ids, float* __restrict__ tk_eos_lp) {
+                              int* __restrict__ tk_eos_ids, float* __restrict__ tk_eos_lp,
+                              const float* __restrict__ part_max, const float* __restrict__ part_sel) {
     static_assert(!TOPK || LOGPROB, "the candidates' log-probabilities need the sum of exponentials");
+    static_assert(!SAMPLE || (LOGPROB && !TOPK), "SAMPLE: the logprob variant only, never with the candidates");
     __shared__ float sv[32];
     __shared__ int si[32];
     __shared__ int tok_s;
+    int* srec = nullptr; float* smax = nullptr;    // SAMPLE: per warp, the best key's record and the raw maximum
+    if constexpr (SAMPLE) { __shared__ int srec_[32]; __shared__ float smax_[32]; srec = srec_; smax = smax_; }
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (done[b]) { if (tid == 0) next_id[b] = -1; return; }
     float v = -INFINITY; int idx = 0x7fffffff;
+    int rec = 0; float mloc = -INFINITY;          // SAMPLE: the best key's record, the raw maximum of the records
     for (int i = tid; i < n_part; i += blockDim.x) {
         float pv = part_val[(size_t)b * n_part + i]; int pi = part_idx[(size_t)b * n_part + i];
-        if (pv > v || (pv == v && pi < idx)) { v = pv; idx = pi; }
+        if (pv > v || (pv == v && pi < idx)) { v = pv; idx = pi; if constexpr (SAMPLE) rec = i; }
+        if constexpr (SAMPLE) mloc = fmaxf(mloc, part_max[(size_t)b * n_part + i]);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         float ov = __shfl_xor_sync(0xffffffffu, v, o); int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-        if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
+        int orec = 0;
+        if constexpr (SAMPLE) orec = __shfl_xor_sync(0xffffffffu, rec, o);
+        if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; if constexpr (SAMPLE) rec = orec; }
     }
-    if (lane == 0) { sv[warp] = v; si[warp] = idx; }
+    if constexpr (SAMPLE) mloc = warp_max(mloc);
+    if (lane == 0) { sv[warp] = v; si[warp] = idx; if constexpr (SAMPLE) { srec[warp] = rec; smax[warp] = mloc; } }
     __syncthreads();
-    float lp = 0.f;
+    float lp = 0.f, M = 0.f;
     if constexpr (LOGPROB) {
         // S = sum_c s_c exp(m_c - M) over the n_part records, M = the maximum logit: each thread its records in index
         // order, then a fixed tree over lanes and warps; logprob = -log S
         __shared__ float ss[32];
         const int nw = (blockDim.x + 31) / 32;
-        float M = sv[0];
-        for (int w = 1; w < nw; ++w) M = fmaxf(M, sv[w]);
+        const float* rmax = SAMPLE ? part_max : part_val;      // SAMPLE: part_val holds keys
+        M = SAMPLE ? smax[0] : sv[0];
+        for (int w = 1; w < nw; ++w) M = fmaxf(M, SAMPLE ? smax[w] : sv[w]);
         float sum = 0.f;
-        for (int i = tid; i < n_part; i += blockDim.x) sum += lse_rescale(part_sum[(size_t)b * n_part + i], part_val[(size_t)b * n_part + i], M);
+        for (int i = tid; i < n_part; i += blockDim.x) sum += lse_rescale(part_sum[(size_t)b * n_part + i], rmax[(size_t)b * n_part + i], M);
         sum = warp_sum(sum);
         if (lane == 0) ss[warp] = sum;
         __syncthreads();
@@ -304,8 +370,9 @@ __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __r
     if (tid == 0) {
         int nw = (blockDim.x + 31) / 32;
         for (int w = 1; w < nw; ++w)
-            if (sv[w] > v || (sv[w] == v && si[w] < idx)) { v = sv[w]; idx = si[w]; }
+            if (sv[w] > v || (sv[w] == v && si[w] < idx)) { v = sv[w]; idx = si[w]; if constexpr (SAMPLE) rec = srec[w]; }
         int tok = idx;
+        if constexpr (SAMPLE) lp = (part_sel[(size_t)b * n_part + rec] - M) + lp;   // (l_sel - M) - log S
         if constexpr (LOGPROB) {
             if (tok == 151643 || tok == 151645) eos_lp[b] = lp;
             else if (n_out[b] < max_new) lp_out[(size_t)b * max_new + n_out[b]] = lp;
@@ -335,18 +402,23 @@ __global__ void greedy_kernel(const float* __restrict__ part_val, const int* __r
 }
 
 void launch_greedy(const Model& m, const DecodeBufs& b, int B, cudaStream_t st, int64_t* launches) {
-    if (b.topk)     // the lm_head wrote the logits (launch_lmhead_argmax): one CTA per sequence selects the candidates
+    if (b.sample && b.logprobs)     // sampling without logprobs: the plain kernel below merges the keys
+        greedy_kernel<true, false, true><<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
+                                                            b.max_new, m.embed, m.d.c.hidden_size, b.x, b.part_sum, b.lp_out, b.eos_lp,
+                                                            nullptr, 0, nullptr, nullptr, nullptr, nullptr, b.part_max, b.part_sel);
+    else if (b.topk && !b.sample)     // the lm_head wrote the logits (launch_lmhead_argmax): one CTA per sequence selects the candidates
         greedy_kernel<true, true><<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
                                                      b.max_new, m.embed, m.d.c.hidden_size, b.x, b.part_sum, b.lp_out, b.eos_lp,
-                                                     b.logits, m.d.c.vocab_size, b.tk_ids, b.tk_lp, b.tk_eos_ids, b.tk_eos_lp);
-    else if (b.logprobs)
+                                                     b.logits, m.d.c.vocab_size, b.tk_ids, b.tk_lp, b.tk_eos_ids, b.tk_eos_lp,
+                                                     nullptr, nullptr);
+    else if (b.logprobs && !b.sample)
         greedy_kernel<true><<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
                                                b.max_new, m.embed, m.d.c.hidden_size, b.x, b.part_sum, b.lp_out, b.eos_lp,
-                                               nullptr, 0, nullptr, nullptr, nullptr, nullptr);
+                                               nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
     else
         greedy_kernel<false><<<B, 256, 0, st>>>(b.part_val, b.part_idx, b.n_part, b.done, b.pos, b.next_id, b.ids_out, b.n_out,
                                                 b.max_new, m.embed, m.d.c.hidden_size, b.x, nullptr, nullptr, nullptr,
-                                                nullptr, 0, nullptr, nullptr, nullptr, nullptr);
+                                                nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
     ASRB_CUDA_CHECK(cudaGetLastError());
     if (launches) *launches += 1;
 }
@@ -358,6 +430,8 @@ static DecodeBufs offset_bufs(const DecodeBufs& b, int b0, const Model& m) {
     o.act = b.act + (size_t)b0 * c.intermediate_size; o.logits = b.logits ? b.logits + (size_t)b0 * c.vocab_size : nullptr;
     o.part_val = b.part_val + (size_t)b0 * b.n_part; o.part_idx = b.part_idx + (size_t)b0 * b.n_part;
     o.part_sum = b.part_sum ? b.part_sum + (size_t)b0 * b.n_part : nullptr;
+    o.part_max = b.part_max ? b.part_max + (size_t)b0 * b.n_part : nullptr;
+    o.part_sel = b.part_sel ? b.part_sel + (size_t)b0 * b.n_part : nullptr;
     o.pos = b.pos + b0; o.done = b.done + b0; o.next_id = b.next_id + b0; o.ids_out = b.ids_out + (size_t)b0 * b.max_new; o.n_out = b.n_out + b0;
     return o;
 }
@@ -372,9 +446,18 @@ void launch_lmhead_argmax(const Model& m, const float* x_rows, const int* d_row_
         p.W = m.lm_head; p.N = c.vocab_size; p.K = c.hidden_size;
         p.x = d_row_idx ? x_rows : x_rows + (size_t)b0 * c.hidden_size; p.ldx = c.hidden_size; p.row_idx = d_row_idx ? d_row_idx + b0 : nullptr;
         p.norm_w = m.final_norm; p.eps = (float)c.rms_norm_eps;
-        p.logits = (write_logits || b.topk) ? ob.logits : nullptr; p.ldl = c.vocab_size;   // TOPK: greedy_kernel reads them
+        p.logits = (write_logits || (b.topk && !b.sample)) ? ob.logits : nullptr; p.ldl = c.vocab_size;   // TOPK: greedy_kernel reads them
         p.part_val = ob.part_val; p.part_idx = ob.part_idx; p.B = nb;
-        if (b.logprobs) { p.part_sum = ob.part_sum; run_gemv<true, DE_ARGMAX_LSE>(p, b.n_part, st); }
+        if (b.sample) {                              // the draw's row is global: b0 + the sequence's index in the launch
+            GemvSample ps{};
+            ps.smp = b.smp; ps.n_out = ob.n_out; ps.row0 = b0;
+            if (b.logprobs) {
+                p.part_sum = ob.part_sum; ps.part_max = ob.part_max; ps.part_sel = ob.part_sel;
+                run_gemv<true, DE_ARGMAX_GUMBEL_LSE>(p, b.n_part, st, &ps);
+            }
+            else run_gemv<true, DE_ARGMAX_GUMBEL>(p, b.n_part, st, &ps);
+        }
+        else if (b.logprobs) { p.part_sum = ob.part_sum; run_gemv<true, DE_ARGMAX_LSE>(p, b.n_part, st); }
         else run_gemv<true, DE_ARGMAX>(p, b.n_part, st);
         if (launches) *launches += 1;
     }

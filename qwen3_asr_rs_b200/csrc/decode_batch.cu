@@ -65,6 +65,10 @@ struct Params {
     float* tk_part_val; int* tk_part_idx;   // [nb][n_part][TK_MAX] each CTA's best (logit, id) candidates per sequence
     int* tk_ids; float* tk_lp;              // [nb][max_new][TK_MAX] candidates of each appended token's step, best first
     int* tk_eos_ids; float* tk_eos_lp;      // [nb][TK_MAX] those of the step that selects EOS
+    // SAMPLE instantiations only (appended as well)
+    const SampleParams* smp;     // 1 / temperature and seed of the run
+    int row0;                    // row of sequence 0 of this launch in the call's batch (the draw's counter)
+    float* part_max; float* part_sel;       // LOGPROB: [nb][n_part] raw maximum logit, raw logit of the best-key row
 };
 
 __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
@@ -160,7 +164,10 @@ enum { BE_STORE = 0, BE_SWIGLU = 1, BE_ARGMAX = 2 };
 // TOPK (with LOGPROB): each (tile row, sequence) thread also keeps its best TK_MAX (logit, id) pairs; they are merged
 // per sequence across tile rows and CTAs, and the last CTA records each step's candidates (p.tk_ids / p.tk_lp, or the
 // EOS rows)
-template <int H, int QD, int I, int NB, int NS, int KVK, bool LOGPROB, bool TOPK = false>
+// SAMPLE: each (tile row, sequence) thread folds the sampling keys of draw (p.row0 + sequence, n = p.n_out[sequence])
+// instead of the logits (common.cuh); with LOGPROB the tile-row, CTA and last-CTA merges also carry the raw (max, sum)
+// record and the raw logit of the best-key row
+template <int H, int QD, int I, int NB, int NS, int KVK, bool LOGPROB, bool TOPK = false, bool SAMPLE = false>
 __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params p) {   // 9 warps are allocated as 12 (granularity 4): 168 registers
     static_assert(NB % 8 == 0 && NB <= 16, "NB must be 8 or 16");
     static_assert(H % 256 == 0 && QD % H == 0 && I % H == 0, "chunking needs QD, I multiples of H, H multiple of 256");
@@ -175,6 +182,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
     constexpr int XS_FLOATS = (3 * PSTR / 4 > ATT_SCRATCH) ? 3 * PSTR / 4 : ATT_SCRATCH;   // activation planes; attention scratch aliases them
     static_assert(!TOPK || LOGPROB, "the candidates' log-probabilities need the sum of exponentials");
     static_assert(16 * NB * (1 + 2 * TK_MAX) <= XS_FLOATS, "lm_head merge records must fit the activation planes");
+    static_assert(!(SAMPLE && TOPK), "sampling is never combined with the candidate lists");
+    constexpr bool SLP = SAMPLE && LOGPROB;
     extern __shared__ __align__(128) uint8_t smem[];
     Ring ring;
     ring.slots = smem; ring.nslot = NS;
@@ -308,6 +317,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
     float best_s = 0.f;                                      // LOGPROB: its sum of exp(logit - best_v)
     TopK tk;                                                 // TOPK: its best rows
     if constexpr (TOPK) tk_init(tk);
+    Draw dr{};                                               // SAMPLE: the draw of its sequence (n_out changes only after
+    float smx = -INFINITY, ssel = 0.f;                       // every CTA's ticket); SLP: raw maximum, raw logit of the best key
+    if constexpr (SAMPLE) if (tid < 16 * NB && tid % NB < nb) dr = make_draw(p.smp, __ldcg(p.n_out + tid % NB), p.row0 + tid % NB);
     // merging CTA: which (sequence, kv head), and which record slots will be written for it -- slot u holds a record iff a
     // run starts at split u, i.e. u == 0 or item base + u opens its owner's range.  Positions do not change within the
     // step, so this is computed once, not per layer (the owner search is a dozen integer divisions per slot).
@@ -500,6 +512,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
                     } else if (epi == BE_SWIGLU) {
                         const float up = __shfl_down_sync(0xffffffffu, v, NB);     // rows 2j (gate) and 2j + 1 (up): NB threads apart
                         if (valid && !(rr & 1)) sx_store(sxo + (size_t)sq * I + (row >> 1), silu(v) * up);
+                    } else if constexpr (SAMPLE) {
+                        if (valid) sample_fold<LOGPROB>(dr, v, row, best_v, best_i, best_s, smx, ssel);   // rows ascend per thread
                     } else if constexpr (LOGPROB) {
                         if (valid) {
                             lse_fold(v, row, best_v, best_i, best_s);     // rows ascend per thread: ties keep the first
@@ -818,18 +832,29 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
     float* bests = xs;                                       // [16 rows][NB]
     float* tkv = xs + 16 * NB;                               // TOPK: [16 rows][NB][TK_MAX] candidate values, then ids
     int* tki = reinterpret_cast<int*>(tkv + 16 * NB * TK_MAX);
+    float* smxs = xs + 16 * NB;                              // SLP: [16 rows][NB] raw maxima, then raw logits of the best keys
+    float* ssels = smxs + 16 * NB;
     if (tid < 16 * NB) { bestv[tid] = best_v; besti[tid] = best_i; if constexpr (LOGPROB) bests[tid] = best_s; }
+    if constexpr (SLP) if (tid < 16 * NB) { smxs[tid] = smx; ssels[tid] = ssel; }
     if constexpr (TOPK) if (tid < 16 * NB) tk_store(tk, tkv + tid * TK_MAX, tki + tid * TK_MAX);
     cons_sync();
     int& is_last = misc[0];
     if (tid < nb) {
-        float v = -INFINITY; int idx = 0x7fffffff;
+        float v = -INFINITY; int idx = 0x7fffffff; int ws = 0;
         for (int wq = 0; wq < 16; ++wq) {
             const float cv = bestv[wq * NB + tid]; const int ci = besti[wq * NB + tid];
-            if (cv > v || (cv == v && ci < idx)) { v = cv; idx = ci; }
+            if (cv > v || (cv == v && ci < idx)) { v = cv; idx = ci; if constexpr (SLP) ws = wq; }
         }
         p.part_val[(size_t)tid * p.n_part + blockIdx.x] = v; p.part_idx[(size_t)tid * p.n_part + blockIdx.x] = idx;
-        if constexpr (LOGPROB) {                             // the 16 tile rows' sums rescaled to the CTA maximum, in row order
+        if constexpr (SLP) {                                 // the 16 tile rows' raw sums rescaled to the CTA's raw maximum
+            float M = -INFINITY;
+            for (int wq = 0; wq < 16; ++wq) M = fmaxf(M, smxs[wq * NB + tid]);
+            float sum = 0.f;
+            for (int wq = 0; wq < 16; ++wq) sum += lse_rescale(bests[wq * NB + tid], smxs[wq * NB + tid], M);
+            const size_t o = (size_t)tid * p.n_part + blockIdx.x;
+            p.part_sum[o] = sum; p.part_max[o] = M; p.part_sel[o] = ssels[ws * NB + tid];
+        }
+        else if constexpr (LOGPROB) {                             // the 16 tile rows' sums rescaled to the CTA maximum, in row order
             float sum = 0.f;
             for (int wq = 0; wq < 16; ++wq) sum += lse_rescale(bests[wq * NB + tid], bestv[wq * NB + tid], v);
             p.part_sum[(size_t)tid * p.n_part + blockIdx.x] = sum;
@@ -855,24 +880,33 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
     for (int b = warp; b < nb; b += NCONS_WARPS) {
         if (__ldcg(p.done + b) != 0) { if (lane == 0) p.next_id[b] = -1; continue; }
         float v = -INFINITY; int idx = 0x7fffffff;
+        int rec = 0; float M = -INFINITY;                    // SLP: the best key's record, the raw maximum of the records
         for (int i = lane; i < (int)G; i += 32) {
             const float pv = __ldcg(p.part_val + (size_t)b * p.n_part + i); const int pi = __ldcg(p.part_idx + (size_t)b * p.n_part + i);
-            if (pv > v || (pv == v && pi < idx)) { v = pv; idx = pi; }
+            if (pv > v || (pv == v && pi < idx)) { v = pv; idx = pi; if constexpr (SLP) rec = i; }
+            if constexpr (SLP) M = fmaxf(M, __ldcg(p.part_max + (size_t)b * p.n_part + i));
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
             const float ov = __shfl_xor_sync(0xffffffffu, v, o); const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-            if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
+            int orec = 0;
+            if constexpr (SLP) orec = __shfl_xor_sync(0xffffffffu, rec, o);
+            if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; if constexpr (SLP) rec = orec; }
         }
+        if constexpr (SLP) M = warp_max(M);
         int tok = idx;
         const int n = p.n_out[b];
         if constexpr (LOGPROB) {
-            // S = sum_c s_c exp(m_c - M) over the G records (M = v, the maximum: every lane holds it after the butterfly),
-            // each lane its records in index order, then a fixed butterfly; logprob = -log S
+            // S = sum_c s_c exp(m_c - M) over the G records (M = v, the maximum: every lane holds it after the butterfly;
+            // SLP: the raw maximum), each lane its records in index order, then a fixed butterfly; logprob = -log S
+            // (SLP: (l_sel - M) - log S)
             float sum = 0.f;
-            for (int i = lane; i < (int)G; i += 32)
-                sum += lse_rescale(__ldcg(p.part_sum + (size_t)b * p.n_part + i), __ldcg(p.part_val + (size_t)b * p.n_part + i), v);
-            const float lp = -logf(warp_sum(sum));
+            for (int i = lane; i < (int)G; i += 32) {
+                if constexpr (SLP) sum += lse_rescale(__ldcg(p.part_sum + (size_t)b * p.n_part + i), __ldcg(p.part_max + (size_t)b * p.n_part + i), M);
+                else sum += lse_rescale(__ldcg(p.part_sum + (size_t)b * p.n_part + i), __ldcg(p.part_val + (size_t)b * p.n_part + i), v);
+            }
+            float lp = -logf(warp_sum(sum));
+            if constexpr (SLP) lp = (__ldcg(p.part_sel + (size_t)b * p.n_part + rec) - M) + lp;
             if (lane == 0) {
                 if (tok == 151643 || tok == 151645) p.eos_lp[b] = lp;
                 else if (n < p.max_new) p.lp_out[(size_t)b * p.max_new + n] = lp;
@@ -982,7 +1016,24 @@ void launch_decode_step_batch(const Model& m, const DecodeBufs& b, int B, float*
         const BatchCfg k = batch_cfg(nb);
         const size_t smem = batch_smem_bytes(c.hidden_size, k);
         const void* fn = nullptr;
-        if (b.topk) {
+        if (b.sample) {     // with or without the log-probability record; never with the candidate lists
+            if (b.logprobs) {
+                if (bdims_match<1024, 2048, 3072>(c))
+                    fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, true, false, true>
+                                   : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, true, false, true>;
+                else
+                    fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, true, false, true>
+                                   : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, true, false, true>;
+            } else {
+                if (bdims_match<1024, 2048, 3072>(c))
+                    fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, false, false, true>
+                                   : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, false, false, true>;
+                else
+                    fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, false, false, true>
+                                   : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, false, false, true>;
+            }
+        }
+        else if (b.topk) {
             if (bdims_match<1024, 2048, 3072>(c))
                 fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, true, true>
                                : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, true, true>;
@@ -1034,6 +1085,10 @@ void launch_decode_step_batch(const Model& m, const DecodeBufs& b, int B, float*
             p.tk_part_val = b.tk_part_val + (size_t)b0 * b.n_part * TK_MAX; p.tk_part_idx = b.tk_part_idx + (size_t)b0 * b.n_part * TK_MAX;
             p.tk_ids = b.tk_ids + (size_t)b0 * b.max_new * TK_MAX; p.tk_lp = b.tk_lp + (size_t)b0 * b.max_new * TK_MAX;
             p.tk_eos_ids = b.tk_eos_ids + (size_t)b0 * TK_MAX; p.tk_eos_lp = b.tk_eos_lp + (size_t)b0 * TK_MAX;
+        }
+        if (b.sample) {                              // passes of 16: the draw's row is global
+            p.smp = b.smp; p.row0 = b0;
+            if (b.logprobs) { p.part_max = b.part_max + (size_t)b0 * b.n_part; p.part_sel = b.part_sel + (size_t)b0 * b.n_part; }
         }
         { static const int fl = getenv("ASRB_BATCH_FLAGS") ? atoi(getenv("ASRB_BATCH_FLAGS")) : 0; p.flags = fl; }   // bit 0 (K/V L2 prefetch): measured slower, off
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {   // tags must stay monotonic: wipe long before the epoch wraps

@@ -59,6 +59,10 @@ struct Params {
     float* tk_part_val; int* tk_part_idx;   // [gridDim.x][TK_MAX] the CTA's best (logit, id) candidates
     int* tk_ids; float* tk_lp;              // [max_new][TK_MAX] candidates of each appended token's step, best first
     int* tk_eos_ids; float* tk_eos_lp;      // [TK_MAX] those of the step that selects EOS
+    // SAMPLE instantiations only (appended as well)
+    const SampleParams* smp;     // 1 / temperature and seed of the run
+    int row;                     // the sequence's row in the call's batch (the draw's counter)
+    float* part_max; float* part_sel;       // LOGPROB: [gridDim.x] raw maximum logit, raw logit of the best-key row
 };
 
 static_assert(KV_KEYS * HD * 4 == SLOT_BYTES, "K / V tiles travel through the weight ring: one tile per slot");
@@ -273,10 +277,11 @@ __device__ __forceinline__ void consume_ksplit(const Slice& s, const Ring& ring,
 }
 
 // K <= 1024 GEMVs (qkv, gate/up, lm_head of the 0.6B dims): four rows per warp and turn, two ring slots (32 rows) per turn.
-template <int K, int EPI, bool LOGPROB, bool TOPK>
+template <int K, int EPI, bool LOGPROB, bool TOPK, bool SAMPLE>
 __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
                                              uint32_t tag, uint32_t* sxo, float& best_v, int& best_i, float& best_s,
-                                             const float* norm_w, float norm_r, long long* fine, TopK* tk) {
+                                             const float* norm_w, float norm_r, long long* fine, TopK* tk,
+                                             const Draw* dr, float* smx, float* ssel) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int fi = 0;
 #define CF() do { if (fine && threadIdx.x == 0 && fi < 24) fine[fi++] = clock64(); } while (0)
@@ -315,6 +320,8 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
                 if ((lane & 15) == 0 && j < nv) sx_store(sxo + (row >> 1), silu(v) * up);
             } else if (EPI == ME_STORE) {
                 if ((lane & 7) == 0 && j < nv) ll_store(out + row, v, tag);
+            } else if constexpr (SAMPLE) {         // ME_ARGMAX over the sampling keys (+ the raw record with LOGPROB)
+                if ((lane & 7) == 0 && j < nv) sample_fold<LOGPROB>(*dr, v, row, best_v, best_i, best_s, *smx, *ssel);
             } else if constexpr (LOGPROB) {        // ME_ARGMAX + running sum of exponentials (the lanes that keep best_v)
                 if ((lane & 7) == 0 && j < nv) {
                     lse_fold(v, row, best_v, best_i, best_s);
@@ -336,13 +343,17 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
 // consumer: process all chunks of a slice.  `xs` holds the (already normalised) activation vector.
 // Results are published as tagged words to `out` (ME_STORE), as self-validating words to `sxo` (ME_SWIGLU), or folded
 // into the running argmax (ME_ARGMAX; with LOGPROB also into the running sum of exponentials `best_s`, with TOPK also
-// into the sorted candidate list `*tk`).
-template <int K, int EPI, bool LOGPROB = false, bool TOPK = false>
+// into the sorted candidate list `*tk`; with SAMPLE the argmax is over the sampling keys of the draw `*dr`, and LOGPROB
+// keeps the raw (max `*smx`, sum `best_s`) record and the raw logit `*ssel` of the best-key row).
+template <int K, int EPI, bool LOGPROB = false, bool TOPK = false, bool SAMPLE = false>
 __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
                                         uint32_t tag, uint32_t* sxo, float& best_v, int& best_i, float& best_s,
                                         const float* norm_w = nullptr, float norm_r = 1.f, long long* fine = nullptr,
-                                        TopK* tk = nullptr) {
-    if constexpr (K <= 1024) { consume_quad<K, EPI, LOGPROB, TOPK>(s, ring, q, xs, out, tag, sxo, best_v, best_i, best_s, norm_w, norm_r, fine, tk); return; }
+                                        TopK* tk = nullptr, const Draw* dr = nullptr, float* smx = nullptr, float* ssel = nullptr) {
+    if constexpr (K <= 1024) {
+        consume_quad<K, EPI, LOGPROB, TOPK, SAMPLE>(s, ring, q, xs, out, tag, sxo, best_v, best_i, best_s, norm_w, norm_r, fine, tk, dr, smx, ssel);
+        return;
+    }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int fi = 0;
 #define CF() do { if (fine && threadIdx.x == 0 && fi < 24) fine[fi++] = clock64(); } while (0)
@@ -401,6 +412,8 @@ __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32
                 }
                 if (EPI == ME_STORE) {
                     if (act) ll_store(out + row, v0, tag);
+                } else if constexpr (SAMPLE) {
+                    if (act) sample_fold<LOGPROB>(*dr, v0, row, best_v, best_i, best_s, *smx, *ssel);
                 } else if constexpr (LOGPROB) {
                     if (act) {
                         lse_fold(v0, row, best_v, best_i, best_s);
@@ -528,7 +541,9 @@ __device__ __forceinline__ void head_norm_rope(const uint2* __restrict__ src, ui
 // the selected token (p.lp_out / p.eos_lp)
 // TOPK (with LOGPROB): each folding lane also keeps its best TK_MAX (logit, id) pairs; they are merged across lanes,
 // warps and CTAs, and the last CTA records the step's candidates (p.tk_ids / p.tk_lp, or the EOS row)
-template <int H, int QD, int I, int NS, bool LOGPROB, bool TOPK = false>
+// SAMPLE: the lm_head folds the sampling keys of draw (p.row, n = *p.n_out) instead of the logits (common.cuh); with
+// LOGPROB the lanes, warps and CTAs also carry the raw (max, sum) record and the raw logit of the best-key row
+template <int H, int QD, int I, int NS, bool LOGPROB, bool TOPK = false, bool SAMPLE = false>
 __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p) {
     constexpr int XS_FLOATS = (I > XS_MIN ? I : XS_MIN) + 64;
     extern __shared__ __align__(128) uint8_t smem[];
@@ -961,31 +976,49 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
         mbar_wait(&p_full[p.L & 1], (p.L >> 1) & 1);
         nrf = norm_scale(ss, H, p.eps, red);
     }
-    consume<H, ME_ARGMAX, LOGPROB, TOPK>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i, best_s,
-                                         pbuf + (p.L & 1) * PARAM_FLOATS, nrf, nullptr, &tk);
+    static_assert(!(SAMPLE && TOPK), "sampling is never combined with the candidate lists");
+    static_assert(4 * NCONS_WARPS <= 62, "per-warp records must fit red / ired");
+    constexpr bool SLP = SAMPLE && LOGPROB;
+    Draw dr{};
+    float smx = -INFINITY, ssel = 0.f;                 // SLP: this lane's raw maximum logit, raw logit of its best-key row
+    if constexpr (SAMPLE) dr = make_draw(p.smp, __ldcg(p.n_out), p.row);   // n_out changes only after every CTA's ticket
+    consume<H, ME_ARGMAX, LOGPROB, TOPK, SAMPLE>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i,
+                                                 best_s, pbuf + (p.L & 1) * PARAM_FLOATS, nrf, nullptr, &tk, &dr, &smx, &ssel);
     MEGA_MARK();
     // candidates live in lanes 0, 8, 16, 24 of every warp (the four rows of a turn; lanes 0 / 16 in the two-row form):
     // merge them, lane 0 publishes the warp's best
 #pragma unroll
     for (int o = 8; o <= 16; o <<= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best_v, o); const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
-        if constexpr (LOGPROB) best_s = lse_merge(best_v, best_s, ov, __shfl_xor_sync(0xffffffffu, best_s, o));
-        if (ov > best_v || (ov == best_v && oi < best_i)) { best_v = ov; best_i = oi; }
-        if constexpr (TOPK) tk_merge_xor(tk, o);
+        if constexpr (SAMPLE) {
+            sample_merge_xor<LOGPROB>(o, best_v, best_i, best_s, smx, ssel);
+        } else {
+            const float ov = __shfl_xor_sync(0xffffffffu, best_v, o); const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
+            if constexpr (LOGPROB) best_s = lse_merge(best_v, best_s, ov, __shfl_xor_sync(0xffffffffu, best_s, o));
+            if (ov > best_v || (ov == best_v && oi < best_i)) { best_v = ov; best_i = oi; }
+            if constexpr (TOPK) tk_merge_xor(tk, o);
+        }
     }
     cons_sync();
     // TOPK: the warps' lists go to xs ([NCONS_WARPS][TK_MAX] values, then ids), free once the lm_head has read it
     float* tkv = xs; int* tki = reinterpret_cast<int*>(xs + NCONS_WARPS * TK_MAX);
     if (lane == 0) { red[warp] = best_v; ired[warp] = best_i; if constexpr (LOGPROB) red[NCONS_WARPS + warp] = best_s; }
+    if constexpr (SLP) if (lane == 0) { red[2 * NCONS_WARPS + warp] = smx; red[3 * NCONS_WARPS + warp] = ssel; }
     if constexpr (TOPK) if (lane == 0) tk_store(tk, tkv + warp * TK_MAX, tki + warp * TK_MAX);
     cons_sync();
     int& is_last = ired[63];
     if (tid == 0) {
-        float v = -INFINITY; int idx = 0x7fffffff;
+        float v = -INFINITY; int idx = 0x7fffffff; int ws = 0;
         for (int wq = 0; wq < NCONS_WARPS; ++wq)
-            if (red[wq] > v || (red[wq] == v && ired[wq] < idx)) { v = red[wq]; idx = ired[wq]; }
+            if (red[wq] > v || (red[wq] == v && ired[wq] < idx)) { v = red[wq]; idx = ired[wq]; if constexpr (SLP) ws = wq; }
         p.part_val[blockIdx.x] = v; p.part_idx[blockIdx.x] = idx;
-        if constexpr (LOGPROB) {             // the warps' sums rescaled to the CTA maximum, in warp order
+        if constexpr (SLP) {                 // the warps' raw sums rescaled to the CTA's raw maximum, in warp order
+            float M = -INFINITY;
+            for (int wq = 0; wq < NCONS_WARPS; ++wq) M = fmaxf(M, red[2 * NCONS_WARPS + wq]);
+            float sum = 0.f;
+            for (int wq = 0; wq < NCONS_WARPS; ++wq) sum += lse_rescale(red[NCONS_WARPS + wq], red[2 * NCONS_WARPS + wq], M);
+            p.part_sum[blockIdx.x] = sum; p.part_max[blockIdx.x] = M; p.part_sel[blockIdx.x] = red[3 * NCONS_WARPS + ws];
+        }
+        else if constexpr (LOGPROB) {        // the warps' sums rescaled to the CTA maximum, in warp order
             float sum = 0.f;
             for (int wq = 0; wq < NCONS_WARPS; ++wq) sum += lse_rescale(red[NCONS_WARPS + wq], red[wq], v);
             p.part_sum[blockIdx.x] = sum;
@@ -1004,25 +1037,32 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     __threadfence();
     {
         float v = -INFINITY; int idx = 0x7fffffff;
+        int rec = 0; float mloc = -INFINITY;         // SLP: the best key's record, the raw maximum of the records
         for (int i = tid; i < (int)G; i += NCONS) {
             float pv = __ldcg(p.part_val + i); int pi = __ldcg(p.part_idx + i);
-            if (pv > v || (pv == v && pi < idx)) { v = pv; idx = pi; }
+            if (pv > v || (pv == v && pi < idx)) { v = pv; idx = pi; if constexpr (SLP) rec = i; }
+            if constexpr (SLP) mloc = fmaxf(mloc, __ldcg(p.part_max + i));
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
             float ov = __shfl_xor_sync(0xffffffffu, v, o); int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-            if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
+            int orec = 0;
+            if constexpr (SLP) orec = __shfl_xor_sync(0xffffffffu, rec, o);
+            if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; if constexpr (SLP) rec = orec; }
         }
+        if constexpr (SLP) mloc = warp_max(mloc);
         if (lane == 0) { red[warp] = v; ired[warp] = idx; }
+        if constexpr (SLP) if (lane == 0) { ired[NCONS_WARPS + warp] = rec; red[2 * NCONS_WARPS + warp] = mloc; }
         cons_sync();
-        float lp = 0.f;
+        float lp = 0.f, M = 0.f;
         if constexpr (LOGPROB) {
-            // S = sum_c s_c exp(m_c - M) over the G records, M = the step's maximum logit (= that of the selected token):
-            // each thread its records in index order, then the warps in a fixed tree; logprob = -log S
-            float M = red[0];
-            for (int wq = 1; wq < NCONS_WARPS; ++wq) M = fmaxf(M, red[wq]);
+            // S = sum_c s_c exp(m_c - M) over the G records, M = the step's maximum logit (= that of the selected token
+            // when not sampling): each thread its records in index order, then the warps in a fixed tree; logprob = -log S
+            const float* rmax = SLP ? p.part_max : p.part_val;
+            M = red[SLP ? 2 * NCONS_WARPS : 0];
+            for (int wq = 1; wq < NCONS_WARPS; ++wq) M = fmaxf(M, red[(SLP ? 2 * NCONS_WARPS : 0) + wq]);
             float sum = 0.f;
-            for (int i = tid; i < (int)G; i += NCONS) sum += lse_rescale(__ldcg(p.part_sum + i), __ldcg(p.part_val + i), M);
+            for (int i = tid; i < (int)G; i += NCONS) sum += lse_rescale(__ldcg(p.part_sum + i), __ldcg(rmax + i), M);
             sum = warp_sum(sum);
             if (lane == 0) red[NCONS_WARPS + warp] = sum;
             cons_sync();
@@ -1047,8 +1087,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
         int& tok_s = ired[62];
         if (tid == 0) {
             for (int wq = 1; wq < NCONS_WARPS; ++wq)
-                if (red[wq] > v || (red[wq] == v && ired[wq] < idx)) { v = red[wq]; idx = ired[wq]; }
+                if (red[wq] > v || (red[wq] == v && ired[wq] < idx)) { v = red[wq]; idx = ired[wq]; if constexpr (SLP) rec = ired[NCONS_WARPS + wq]; }
             int tok = idx;
+            if constexpr (SLP) lp = (__ldcg(p.part_sel + rec) - M) + lp;      // (l_sel - M) - log S
             const int n = *p.n_out;
             if constexpr (LOGPROB) {
                 if (tok == 151643 || tok == 151645) *p.eos_lp = lp;
@@ -1133,7 +1174,18 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
     const int nsplit = std::min(mega::MAX_SPLITS, std::min(G / c.num_key_value_heads, (max_ctx + mega::KV_KEYS - 1) / mega::KV_KEYS));
     const size_t smem = mega_smem_bytes(c.hidden_size, c.intermediate_size, mega_nslot(c));
     const void* fn = nullptr;
-    if (b.topk) {
+    if (b.sample) {         // with or without the log-probability record; never with the candidate lists
+        if (b.logprobs) {
+            if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, true, false, true>;
+            else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, true, false, true>;
+            else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, true, false, true>;
+        } else {
+            if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, false, false, true>;
+            else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, false, false, true>;
+            else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, false, false, true>;
+        }
+    }
+    else if (b.topk) {
         if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, true, true>;
         else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, true, true>;
         else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, true, true>;
@@ -1175,6 +1227,10 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
             p.tk_part_val = b.tk_part_val; p.tk_part_idx = b.tk_part_idx;
             p.tk_ids = b.tk_ids + (size_t)sb * b.max_new * TK_MAX; p.tk_lp = b.tk_lp + (size_t)sb * b.max_new * TK_MAX;
             p.tk_eos_ids = b.tk_eos_ids + (size_t)sb * TK_MAX; p.tk_eos_lp = b.tk_eos_lp + (size_t)sb * TK_MAX;
+        }
+        if (b.sample) {                      // per-sequence launches: the draw's row is the sequence's index in the batch
+            p.smp = b.smp; p.row = sb;
+            if (b.logprobs) { p.part_max = b.part_max; p.part_sel = b.part_sel; }
         }
         // tags must stay monotonic for red.max publication: long before the 24-bit epoch wraps, wipe the tagged exchange
         // buffers (the self-validating words live elsewhere and are left alone: to them 0 would be a published 0.0)

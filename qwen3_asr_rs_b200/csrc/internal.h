@@ -195,6 +195,12 @@ struct DecodeBufs {
     float* tk_lp;       // [B][max_new][TK_MAX] their log-probabilities
     int* tk_eos_ids;    // [B][TK_MAX] candidates of the step that selected the EOS token ending the sequence
     float* tk_eos_lp;   // [B][TK_MAX]
+    // seeded temperature sampling (session options "temperature" / "seed", latched at the prefill): the kernels select
+    // the argmax of the Gumbel keys (common.cuh) instead of the logits
+    bool sample;              // launch the SAMPLE kernel variants
+    const SampleParams* smp;  // device: 1 / temperature and the seed of the current run
+    float* part_max;          // [B][n_part] sampling with logprobs: raw maximum logit per argmax partial (part_val holds keys)
+    float* part_sel;          // [B][n_part] raw logit of each partial's best-key row (allocated when first needed)
 };
 void launch_decode_step_phases(const Model& m, const DecodeBufs& b, int B, float* kcache, float* vcache,
                                size_t cache_layer_stride, size_t cache_seq_stride, int max_ctx,

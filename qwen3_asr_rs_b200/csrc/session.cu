@@ -4,6 +4,9 @@
 // is in the kernels.  Everything is varlen: rows of all utterances are concatenated and described
 // by small index arrays uploaded once per call.
 #include <algorithm>
+#include <cerrno>
+#include <cmath>
+#include <cstdlib>
 #include <cstring>
 #include <limits>
 #include "internal.h"
@@ -80,6 +83,10 @@ struct Session {
     // top-k alternatives: option "top_logprobs" (top_k >= 1 sets db.topk and db.logprobs); tk_valid = the k the prefill
     // and every step since ran with (0: none), i.e. db.tk_* describe the current run for k <= tk_valid
     bool opt_logprobs = false; int top_k = 0, tk_valid = 0;
+    // seeded temperature sampling: options "temperature" (0 = greedy) and "seed", latched at the prefill into db.sample
+    // and the device-resident db.smp, so they apply to the whole run
+    double temperature = 0.0; uint64_t seed = 0;
+    SampleParams* d_smp = nullptr;
     ~Session();
 };
 
@@ -178,6 +185,8 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
         b.pos = salloc<int>(s, Bm); b.done = salloc<int>(s, Bm); b.next_id = salloc<int>(s, Bm);
         b.ids_out = salloc<int>(s, Bm * max_new); b.n_out = salloc<int>(s, Bm);
         b.max_new = max_new;
+        s->d_smp = salloc<SampleParams>(s, 1, true);
+        b.smp = s->d_smp;
         s->d_lastrow = salloc<int>(s, Bm);
         s->mega.bar = salloc<unsigned>(s, 4, true);
         { const unsigned one = 1; ASRB_CUDA_CHECK(cudaMemcpy(s->mega.bar + 1, &one, sizeof(one), cudaMemcpyHostToDevice)); }   // epoch 1
@@ -408,9 +417,24 @@ void session_encode_read(Session* s, int b, float* out) {
 // -------------------------------------------------------------------------------------------------
 // steps 4-7: prompt, embed + inject, positions, prefill  (inference.rs:105-149)
 // -------------------------------------------------------------------------------------------------
+// sampling with the top-k candidate lists is not offered: refused by every call that runs a prefill, before any work
+static void check_sampling_options(const Session* s) {
+    ASRB_REQUIRE(!(s->temperature > 0.0 && s->top_k > 0), ASRB_ERR_INVALID, "temperature > 0 cannot be combined with top_logprobs");
+}
+
+static void ensure_sample_bufs(Session* s) {     // sampling with logprobs: the raw records beside the keys
+    DecodeBufs& b = s->db;
+    if (b.sample && b.logprobs && !b.part_max) {
+        ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+        b.part_max = salloc<float>(s, (size_t)s->max_batch * b.n_part);
+        b.part_sel = salloc<float>(s, (size_t)s->max_batch * b.n_part);
+    }
+}
+
 void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, int64_t* seq_lens_out,
                      float* last_logits) {
     ASRB_REQUIRE(s->stage >= 2, ASRB_ERR_STATE, "prefill called before encode");
+    check_sampling_options(s);
     Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
     const int B = s->B; cudaStream_t st = s->st; const int np = s->nplanes;
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
@@ -453,6 +477,12 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     if (s->db.logprobs) {                  // all NaN (0xFFFFFFFF): no EOS seen, nothing appended
         ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.eos_lp, 0xFF, B * sizeof(float), st));
         ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.lp_out, 0xFF, (size_t)B * s->max_new * sizeof(float), st));
+    }
+    s->db.sample = s->temperature > 0.0;   // latched: the whole run samples with this run's temperature and seed
+    if (s->db.sample) {
+        const SampleParams hp{(float)(1.0 / s->temperature), (uint32_t)(s->seed & 0xffffffffu), (uint32_t)(s->seed >> 32)};
+        ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_smp, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
+        ensure_sample_bufs(s);
     }
     s->tk_valid = s->top_k;
     if (s->db.topk) {                      // ids -1, values NaN (0xFFFFFFFF): nothing recorded yet
@@ -580,7 +610,7 @@ void session_generate(Session* s, int max_new_tokens, int32_t* ids_out, int32_t*
     // (inference.rs:160-200); that wasted forward is not issued here.
     const int steps = std::max(0, max_new_tokens - s->greedy_done);
     auto ensure_graph = [&]() {   // per-phase path: ~142 launches per step -> replay them as one CUDA graph
-        const int mode_key = (((int)s->db.topk * 2 + (int)s->db.logprobs) * 2 + s->decode_mode) * (s->max_batch + 1) + B;   // unique per (topk, logprobs, mode, batch)
+        const int mode_key = ((((int)s->db.sample * 2 + (int)s->db.topk) * 2 + (int)s->db.logprobs) * 2 + s->decode_mode) * (s->max_batch + 1) + B;   // unique per (sample, topk, logprobs, mode, batch)
         if (s->step_graph == nullptr || s->graph_mode != mode_key) {
             if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
             cudaGraph_t g = nullptr;
@@ -623,6 +653,7 @@ void session_transcribe_ids(Session* s, const float* const* samples, const int64
                             const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
                             int32_t* ids_out, int32_t* lens_out) {
     ASRB_REQUIRE(ids_out && lens_out, ASRB_ERR_INVALID, "null output");
+    check_sampling_options(s);
     if (samples == nullptr) batch = (int)s->ingested_n.size();      // asrb_transcribe_ingested
     ASRB_REQUIRE(max_new_tokens >= 1 && max_new_tokens <= s->max_new, ASRB_ERR_INVALID, "max_new_tokens exceeds session capacity");
     cudaStream_t st = s->st;
@@ -735,6 +766,29 @@ static void apply_record_options(Session* s) {
         b.tk_eos_ids = salloc<int>(s, (size_t)s->max_batch * TK_MAX);
         b.tk_eos_lp = salloc<float>(s, (size_t)s->max_batch * TK_MAX);
     }
+    ensure_sample_bufs(s);                           // logprobs switched on during a sampled run
+}
+
+// option values: a decimal temperature, 0 or a finite value in [1e-6, 100]; a decimal unsigned 64-bit seed.  The whole
+// string must be consumed, with no sign or leading space.
+static double parse_temperature(const std::string& v) {
+    ASRB_REQUIRE(!v.empty() && (isdigit((unsigned char)v[0]) || v[0] == '.') &&
+                 v.find_first_not_of("0123456789.eE+-") == std::string::npos,
+                 ASRB_ERR_INVALID, "temperature must be a decimal number");   // no sign, space, hex, inf or nan
+    errno = 0;
+    char* end = nullptr;
+    const double t = strtod(v.c_str(), &end);
+    ASRB_REQUIRE(end && *end == '\0' && errno == 0 && std::isfinite(t), ASRB_ERR_INVALID, "temperature must be a decimal number");
+    ASRB_REQUIRE(t == 0.0 || (t >= 1e-6 && t <= 100.0), ASRB_ERR_INVALID, "temperature must be 0 or in [1e-6, 100]");
+    return t;
+}
+static uint64_t parse_seed(const std::string& v) {
+    ASRB_REQUIRE(!v.empty() && isdigit((unsigned char)v[0]), ASRB_ERR_INVALID, "seed must be a decimal unsigned 64-bit integer");
+    errno = 0;
+    char* end = nullptr;
+    const unsigned long long x = strtoull(v.c_str(), &end, 10);
+    ASRB_REQUIRE(end && *end == '\0' && errno == 0, ASRB_ERR_INVALID, "seed must be a decimal unsigned 64-bit integer");
+    return (uint64_t)x;
 }
 
 void session_set_option(Session* s, const char* key, const char* value) {
@@ -762,6 +816,10 @@ void session_set_option(Session* s, const char* key, const char* value) {
         ASRB_REQUIRE(v.size() == 1 && v[0] >= '0' && v[0] < '0' + 1 + TK_MAX, ASRB_ERR_INVALID, "top_logprobs must be 0..8");
         s->top_k = v[0] - '0';
         apply_record_options(s);
+    } else if (k == "temperature") {
+        s->temperature = parse_temperature(v);
+    } else if (k == "seed") {
+        s->seed = parse_seed(v);
     } else throw Error(ASRB_ERR_INVALID, "unknown option: " + k);
 }
 

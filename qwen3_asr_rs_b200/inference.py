@@ -11,9 +11,10 @@ for host buffers.  No fallback exists: a missing library or GPU raises.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -56,6 +57,66 @@ def check_top_logprobs(top_logprobs) -> int:
     return int(top_logprobs)
 
 
+def check_temperature(temperature) -> Tuple[float, ...]:
+    """The `temperature` argument as a schedule: a float, or a non-empty sequence of floats (a fallback schedule), each
+    0 (greedy) or finite in [1e-6, 100], else ValueError."""
+    ts = tuple(temperature) if isinstance(temperature, (list, tuple)) else (temperature,)
+    if not ts:
+        raise ValueError("temperature schedule must not be empty")
+    for t in ts:
+        if isinstance(t, bool) or not isinstance(t, (int, float, np.integer, np.floating)) or not math.isfinite(float(t)) \
+                or not (float(t) == 0.0 or 1e-6 <= float(t) <= 100.0):
+            raise ValueError(f"temperature must be 0 or a finite value in [1e-6, 100], got {t!r}")
+    return tuple(float(t) for t in ts)
+
+
+def check_seed(seed) -> int:
+    """The `seed` argument as an int in [0, 2^64), else ValueError."""
+    if not isinstance(seed, (int, np.integer)) or isinstance(seed, bool) or not 0 <= int(seed) < 1 << 64:
+        raise ValueError(f"seed must be an int in [0, 2^64), got {seed!r}")
+    return int(seed)
+
+
+def temperature_option(t: float) -> str:
+    """The session option string of temperature t (a decimal the library parses exactly back to t)."""
+    return "0" if t == 0.0 else repr(float(t))
+
+
+def needs_fallback(token_logprobs: Sequence[float], eos_logprob: Optional[float],
+                   logprob_threshold: Optional[float]) -> bool:
+    """Whisper's fallback test without the compression-ratio criterion: the attempt stopped at max_new_tokens without EOS
+    (eos_logprob None: a repetition loop, typically), or its avg_logprob is below the threshold (None: no such test)."""
+    if eos_logprob is None:
+        return True
+    lp = avg_logprob(token_logprobs, eos_logprob)
+    return logprob_threshold is not None and lp is not None and lp < logprob_threshold
+
+
+def temperature_fallback(run: Callable[[List[int], float], "TranscribeIds"], n: int, temperatures: Sequence[float],
+                         logprob_threshold: Optional[float]):
+    """Temperature fallback over n utterances.  `run(indices, t)` decodes the utterances `indices` (ascending, one batch)
+    at temperature t with the log-probability record on, and returns their TranscribeIds in that order.  All utterances
+    run at temperatures[0]; those that need fallback (needs_fallback) run again, as one batch in their original order, at
+    the next temperature, and so on.  Each utterance keeps its first accepted attempt, else its last one.
+    Returns (per utterance (TranscribeIds, index in it), per utterance the temperature of the kept attempt, the runs)."""
+    kept: List[Optional[Tuple["TranscribeIds", int]]] = [None] * n
+    temps: List[Optional[float]] = [None] * n
+    runs = []
+    pending = list(range(n))
+    for t in temperatures:
+        if not pending:
+            break
+        r = run(pending, t)
+        runs.append(r)
+        retry = []
+        for j, b in enumerate(pending):
+            kept[b], temps[b] = (r, j), t
+            if needs_fallback(r.logprobs[j], r.eos_logprobs[j], logprob_threshold):
+                retry.append(b)
+        pending = retry
+    return kept, temps, runs
+
+
 @dataclass
 class TranscribeResult:           # inference.rs:270-274
     text: str
@@ -67,6 +128,7 @@ class TranscribeResult:           # inference.rs:270-274
     # transcribe(top_logprobs=k): per id, the k best candidates of its step as (id, log p), best first (entry 0 = the id)
     top_logprobs: Optional[List[List[Tuple[int, float]]]] = None
     eos_top_logprobs: Optional[List[Tuple[int, float]]] = None   # ... of the step that selected EOS (None: stopped by the cap)
+    temperature: Optional[float] = None             # transcribe(temperature=...): that of the kept attempt
 
 
 @dataclass
@@ -81,6 +143,8 @@ class TranscribeIds:
     top_logprobs: Optional[List[List[List[Tuple[int, float]]]]] = None
     # ... of the step that selected the EOS ending the utterance (None: stopped at max_new_tokens)
     eos_top_logprobs: Optional[List[Optional[List[Tuple[int, float]]]]] = None
+    # temperature=T or a schedule: per utterance, the temperature of the attempt kept (None for a plain greedy call)
+    temperatures: Optional[List[float]] = None
 
 
 class AsrInference:
@@ -293,13 +357,68 @@ class AsrInference:
             r.top_logprobs, r.eos_top_logprobs = self.last_top_logprobs(max_new_tokens, top_logprobs)
         return r
 
+    # ---- seeded temperature sampling (session options "temperature" / "seed") ---------------------------
+    def _set_sampling(self, s, t: Optional[float], seed: int) -> List[Tuple[str, str]]:
+        """Set temperature t and seed for one call; returns the (option, configured value) pairs to restore."""
+        undo = []
+        if t is None:
+            return undo
+        for key, val in (("temperature", temperature_option(t)), ("seed", str(seed))):
+            conf = self._options.get(key, "0")
+            if conf != val:
+                _lib.check(self._lib.asrb_session_set_option(s, key.encode(), val.encode()))
+                undo.append((key, conf))
+        return undo
+
+    def _restore(self, s, undo) -> None:
+        for key, conf in undo:
+            _lib.check(self._lib.asrb_session_set_option(s, key.encode(), conf.encode()))
+
+    def _sampled(self, B: int, once, temperature, seed, logprob_threshold, logprobs: bool, top_logprobs: int) -> TranscribeIds:
+        """One call of transcribe_ids / transcribe_pcm.  `once(indices, logprobs, top_logprobs, t)` runs the utterances
+        `indices` at temperature t (None: the session's configured options)."""
+        top_logprobs = check_top_logprobs(top_logprobs)
+        temps = check_temperature(temperature)
+        seed = check_seed(seed)
+        schedule = isinstance(temperature, (list, tuple))
+        if top_logprobs and any(t > 0.0 for t in temps):
+            raise ValueError("temperature > 0 cannot be combined with top_logprobs")
+        if not schedule and temps[0] == 0.0:                 # plain greedy call: the session's options as configured
+            return once(list(range(B)), logprobs, top_logprobs, None)
+        if not schedule:
+            r = once(list(range(B)), logprobs, 0, temps[0])
+            r.temperatures = [temps[0]] * B
+            return r
+        kept, used, runs = temperature_fallback(lambda idx, t: once(idx, True, 0, t), B, temps, logprob_threshold)
+        r = TranscribeIds([k[0].ids[k[1]] for k in kept], {}, sum(x.kernels_launched for x in runs),
+                          sum(x.decode_steps for x in runs))
+        for x in runs:
+            for name, ms in x.stage_ms.items():
+                r.stage_ms[name] = r.stage_ms.get(name, 0.0) + ms
+        r.logprobs = [k[0].logprobs[k[1]] for k in kept]
+        r.eos_logprobs = [k[0].eos_logprobs[k[1]] for k in kept]
+        r.temperatures = used
+        return r
+
     # ---- the hot path ----------------------------------------------------------------
     def transcribe_ids(self, clips: Sequence[np.ndarray], language_ids: Optional[Sequence] = None,
-                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0) -> TranscribeIds:
+                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0,
+                       temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
+                       logprob_threshold: Optional[float] = -1.0) -> TranscribeIds:
         """transcribe() steps 2-8 for a batch: host f32 samples in, host token ids out (and, with `logprobs`, the
         log-probability of every id and of the ending EOS, from the kernels that selected them; with `top_logprobs` = k
-        in 1..8, also the k best candidates of each of those steps, and the log-probabilities as with `logprobs`)."""
-        top_logprobs = check_top_logprobs(top_logprobs)
+        in 1..8, also the k best candidates of each of those steps, and the log-probabilities as with `logprobs`).
+        `temperature` T > 0 samples every id with the seeded Gumbel-max draw of the kernels (ids are a pure function of
+        the inputs, `seed`, T and the batch order); a sequence of temperatures is a fallback schedule
+        (temperature_fallback) with the log-probability record on and `logprob_threshold` (None: off)."""
+        def once(idx, lp, k, t):
+            sub = clips if len(idx) == len(clips) else [clips[i] for i in idx]
+            lang = None if language_ids is None else [language_ids[i] for i in idx]
+            return self._ids_once(sub, lang, max_new_tokens, lp, k, t, seed)
+        return self._sampled(len(clips), once, temperature, seed, logprob_threshold, logprobs, top_logprobs)
+
+    def _ids_once(self, clips, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
+                  temperature: Optional[float], seed: int) -> TranscribeIds:
         B = len(clips)
         arrs, ptrs, lens = self._pack_samples(clips)
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
@@ -310,12 +429,15 @@ class AsrInference:
             self._record_logprobs(s, True)
         if top_logprobs:
             self._record_top_logprobs(s, top_logprobs, True)
+        undo = []
         try:
+            undo = self._set_sampling(s, temperature, seed)
             _lib.check(self._lib.asrb_transcribe_ids(
                 s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
                 ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
             return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs)
         finally:
+            self._restore(s, undo)
             if logprobs:
                 self._record_logprobs(s, False)
             if top_logprobs:
@@ -352,10 +474,19 @@ class AsrInference:
         return out
 
     def transcribe_pcm(self, pcms: Sequence, rates: Sequence[int], language_ids: Optional[Sequence] = None,
-                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0) -> TranscribeIds:
+                       max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0,
+                       temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
+                       logprob_threshold: Optional[float] = -1.0) -> TranscribeIds:
         """transcribe() steps 1-8 for a batch with step 1 on the GPU: raw PCM in, token ids out (`logprobs`,
-        `top_logprobs`: as in transcribe_ids)."""
-        top_logprobs = check_top_logprobs(top_logprobs)
+        `top_logprobs`, `temperature`, `seed`, `logprob_threshold`: as in transcribe_ids)."""
+        def once(idx, lp, k, t):
+            sel = (lambda xs: xs if len(idx) == len(pcms) else [xs[i] for i in idx])
+            lang = None if language_ids is None else sel(language_ids)
+            return self._pcm_once(sel(pcms), sel(rates), lang, max_new_tokens, lp, k, t, seed)
+        return self._sampled(len(pcms), once, temperature, seed, logprob_threshold, logprobs, top_logprobs)
+
+    def _pcm_once(self, pcms, rates, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
+                  temperature: Optional[float], seed: int) -> TranscribeIds:
         B = len(pcms)
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
         s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens)
@@ -365,11 +496,14 @@ class AsrInference:
             self._record_logprobs(s, True)
         if top_logprobs:
             self._record_top_logprobs(s, top_logprobs, True)
+        undo = []
         try:
+            undo = self._set_sampling(s, temperature, seed)
             _lib.check(self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens),
                                                           ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
             return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs)
         finally:
+            self._restore(s, undo)
             if logprobs:
                 self._record_logprobs(s, False)
             if top_logprobs:
@@ -377,27 +511,32 @@ class AsrInference:
 
     def transcribe(self, audio_path: str, language: Optional[str] = None,
                    max_new_tokens: int = MAX_NEW_TOKENS, gpu_ingest: bool = True, logprobs: bool = False,
-                   top_logprobs: int = 0) -> TranscribeResult:
+                   top_logprobs: int = 0, temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
+                   logprob_threshold: Optional[float] = -1.0) -> TranscribeResult:
         """AsrInference::transcribe (inference.rs:89-213): step 1 (WAV payload -> mono 16 kHz; on the GPU by default,
         `gpu_ingest=False` = the host loader) -> steps 2-8 on the GPU -> step 9 (detokenise + parse, host; needs
         tokenizer.json, else raw_output is the id list as text).  `logprobs`: also fill token_logprobs / avg_logprob;
-        `top_logprobs` = k in 1..8: also fill top_logprobs (and token_logprobs / avg_logprob)."""
+        `top_logprobs` = k in 1..8: also fill top_logprobs (and token_logprobs / avg_logprob); `temperature`, `seed`,
+        `logprob_threshold`: as in transcribe_ids, and `temperature` of the result is that of the kept attempt."""
+        sampling = dict(temperature=temperature, seed=seed, logprob_threshold=logprob_threshold)
         from .audio import load_wav, read_wav_pcm
         from .text import language_prompt_ids, parse_asr_output
         lang_ids = language_prompt_ids(self.tokenizer, language)
         if gpu_ingest:
             pcm, rate = read_wav_pcm(audio_path)
             r = self.transcribe_pcm([pcm], [rate], language_ids=[lang_ids] if lang_ids is not None else None,
-                                    max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs)
+                                    max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs, **sampling)
         else:
             samples = load_wav(audio_path, MEL_SAMPLE_RATE)
             r = self.transcribe_ids([samples], language_ids=[lang_ids] if lang_ids is not None else None,
-                                    max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs)
+                                    max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs, **sampling)
         ids = r.ids[0]
         raw = self.tokenizer.decode(ids) if self.tokenizer is not None else " ".join(str(i) for i in ids)
         lang, text = parse_asr_output(raw, language is not None) if self.tokenizer is not None else ("unknown", raw)
         res = TranscribeResult(text=text, language=lang, raw_output=raw, ids=ids)
-        if logprobs or top_logprobs:
+        if r.temperatures is not None:
+            res.temperature = r.temperatures[0]
+        if (logprobs or top_logprobs or r.temperatures is not None) and r.logprobs is not None:
             res.token_logprobs = r.logprobs[0]
             res.avg_logprob = avg_logprob(r.logprobs[0], r.eos_logprobs[0])
         if top_logprobs:

@@ -139,4 +139,26 @@ impl B200Engine {
         check(unsafe { ffi::asrb_session_set_option(session, key.as_ptr(), off.as_ptr()) })?;
         run
     }
+
+    /// `transcribe_ids` with seeded temperature sampling: every id is drawn by the decode kernels from
+    /// softmax(logits / `temperature`) with the Gumbel-max draw of the options "temperature" / "seed"
+    /// (`include/asr_b200.h`).  `temperature` 0 is greedy, else finite in [1e-6, 100]; its shortest decimal form is what
+    /// the library parses.  The ids are a pure function of (samples, language prompt, seed, temperature).  The options
+    /// are set for this call and restored to greedy / seed 0 afterwards.
+    pub fn transcribe_ids_sampled(&self, samples: &[f32], lang_ids: Option<&[i64]>, temperature: f32, seed: u64) -> Result<Vec<i64>> {
+        let session = self.session_for(samples.len())?;
+        let tkey = CString::new("temperature")?;
+        let skey = CString::new("seed")?;
+        let tval = CString::new(format!("{temperature}"))?;
+        let sval = CString::new(seed.to_string())?;
+        let zero = CString::new("0")?;
+        let set = (|| -> Result<()> {
+            check(unsafe { ffi::asrb_session_set_option(session, tkey.as_ptr(), tval.as_ptr()) })?;
+            check(unsafe { ffi::asrb_session_set_option(session, skey.as_ptr(), sval.as_ptr()) })
+        })();
+        let run = set.and_then(|_| self.transcribe_ids(samples, lang_ids));
+        check(unsafe { ffi::asrb_session_set_option(session, tkey.as_ptr(), zero.as_ptr()) })?;
+        check(unsafe { ffi::asrb_session_set_option(session, skey.as_ptr(), zero.as_ptr()) })?;
+        run
+    }
 }
