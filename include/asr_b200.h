@@ -184,7 +184,30 @@ ASRB_API int asrb_session_stats(asrb_session* s, int64_t* out, int n);
  * the argmax of the keys under (key descending, id ascending).  Ids are bitwise deterministic for a given (inputs, seed,
  * temperature, batch order).  With "logprobs" the record holds the model's own log-probability of the sampled id.
  * temperature > 0 with top_logprobs >= 1 is refused with ASRB_ERR_INVALID by asrb_prefill, asrb_transcribe_ids and
- * asrb_transcribe_ingested, before any work. */
+ * asrb_transcribe_ingested, before any work.
+ * "beam_size" = "1".."6" (default "1": greedy, exactly the code above) and "length_penalty" = "none" (default) or a
+ * decimal in [0, 10]; both latched at the prefill.  With beam_size = K > 1 every utterance runs this beam search
+ * (Whisper's BeamSearchDecoder with patience 1, exact and deterministic):
+ *   1. candidates: each alive beam contributes the first K + 2 entries of its step's top-8 record (logit descending, id
+ *      ascending; two EOS ids exist, so at least K are not EOS), with sum = sum_parent + lp, one fp32 add;
+ *   2. walk: all candidates of the utterance in (sum descending, parent rank ascending, position in the record
+ *      ascending) order; an EOS candidate joins the newly finished, any other becomes the next alive beam (its rank is
+ *      the count so far); stop at K alive beams; then admit the newly finished in walk order while the utterance has
+ *      fewer than K finished hypotheses;
+ *   3. token 0: the walk runs on the prefill's single record;
+ *   4. slots: utterance b uses K slots, beam j in slot j * batch + b; a beam's best-ranked child keeps its parent's slot,
+ *      the other children take, in rank order, the slots of childless beams in ascending slot order;
+ *   5. a slot handed to a child of another slot gets only the KV cache positions after the last common ancestor of its
+ *      old and new lineage (the earlier ones are bitwise equal already);
+ *   6. an utterance is done at K finished hypotheses; at max_new_tokens its alive beams, in rank order, fill the list up
+ *      to K as "no EOS";
+ *   7. score = sum / P(n), n = ids (EOS excluded), the sum including the EOS log-probability; P(n) = max(n, 1) with
+ *      "none", else ((5 + n) / 6) ** length_penalty, in double; ranked by (score descending, admission order).
+ * Rank 0 of each utterance is the result: ids_out / lens_out, asrb_session_device_ids ([batch] rows) and, with
+ * "logprobs", asrb_last_logprobs (its per-token values and its EOS value).  Read all K with asrb_last_nbest.
+ * Refused with ASRB_ERR_INVALID before any work: beam_size > 1 with temperature > 0, with top_logprobs >= 1, or with
+ * batch * beam_size > max_batch; asrb_decode_step in a beam run.  A beam run takes one asrb_generate per prefill (its
+ * end writes the result rows, which are also beam 0's slots); a second one returns ASRB_ERR_STATE. */
 ASRB_API int asrb_session_set_option(asrb_session* s, const char* key, const char* value);
 
 /* Per-token log-probabilities of the last run (asrb_generate / asrb_transcribe_ids / asrb_transcribe_ingested, or
@@ -207,6 +230,19 @@ ASRB_API int asrb_last_logprobs(asrb_session* s, int max_new_tokens, float* logp
  * ASRB_ERR_STATE when the last run did not record them; ASRB_ERR_INVALID when k < 1 or k > k_rec. */
 ASRB_API int asrb_last_top_logprobs(asrb_session* s, int max_new_tokens, int k, int32_t* ids_out, float* logprobs_out,
                                     int32_t* eos_ids_out, float* eos_logprobs_out);
+
+/* The k (1..beam_size) best hypotheses of each utterance of the last beam run, ranked (entry 0 = the result):
+ *   ids_out          [batch][k][max_new_tokens], -1 at and beyond the length
+ *   lens_out         [batch][k] ids (EOS excluded)
+ *   sum_logprob_out  [batch][k] or NULL: the fp32 running sum of the ids' log-probabilities and the EOS one
+ *   score_out        [batch][k] or NULL: sum / P(n) (option "length_penalty")
+ *   eos_id_out       [batch][k] or NULL: the EOS id that ended it, -1 when stopped by max_new_tokens
+ * ASRB_ERR_STATE if the last run was not a beam run; ASRB_ERR_INVALID when k is outside [1, beam_size]. */
+ASRB_API int asrb_last_nbest(asrb_session* s, int max_new_tokens, int k, int32_t* ids_out, int32_t* lens_out,
+                             float* sum_logprob_out, float* score_out, int32_t* eos_id_out);
+/* Counters of the last beam run: [0] beam steps  [1] slots reassigned  [2] KV bytes copied by the prompt expansion
+ * [3] KV bytes copied by reorders; writes min(n, 4) values.  ASRB_ERR_STATE if the last run was not a beam run. */
+ASRB_API int asrb_last_beam_stats(asrb_session* s, int64_t* out, int n);
 
 /* debug (ASRB_MEGA_DEBUG=1): clock64 timeline of the last fused decode step, CTA 0 then CTA G-1;
  * returns the number of slots per CTA (0 if disabled) */

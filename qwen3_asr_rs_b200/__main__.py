@@ -3,11 +3,13 @@
 `--top-logprobs N` (N in 1..8, anywhere on the line) also prints, for every generated token and the ending EOS, the N
 best candidates of the step that selected it with their log-probabilities.
 `--temperature T[,T...]` samples with temperature T (a list is a fallback schedule), `--seed N` seeds the draw; both
-anywhere on the line, and `Temperature: x` reports the temperature of the kept attempt."""
+anywhere on the line, and `Temperature: x` reports the temperature of the kept attempt.
+`--beam-size N` (N in 1..6) decodes with beam search and prints an `N-best:` block of the ranked hypotheses with their
+scores; `--length-penalty A` (A in [0, 10]) scores them with ((5 + n) / 6) ** A instead of the length."""
 import sys
 
 USAGE = ("Usage: python -m qwen3_asr_rs_b200 <model_dir> <audio_file> [language] [--logprobs] [--top-logprobs N] "
-         "[--temperature T[,T...]] [--seed N]")
+         "[--temperature T[,T...]] [--seed N] [--beam-size N] [--length-penalty A]")
 
 
 def parse_args(argv):
@@ -87,6 +89,25 @@ def split_sampling(argv):
     return sd[0], temperature, seed
 
 
+def split_beam(argv):
+    """Remove `--beam-size N` and `--length-penalty A` from argv -> (remaining argv, N; 1 when absent, A; None when
+    absent), or None when a value is missing or invalid."""
+    from .inference import check_beam
+    k = _take_flag(argv, "--beam-size")
+    if k is None:
+        return None
+    a = _take_flag(k[0], "--length-penalty")
+    if a is None:
+        return None
+    try:
+        if k[1] is not None and not k[1].isdigit():
+            return None
+        size, alpha = check_beam(int(k[1]) if k[1] is not None else 1, float(a[1]) if a[1] is not None else None)
+    except ValueError:
+        return None
+    return a[0], size, alpha
+
+
 def format_candidates(cands, decode) -> str:
     """One line of candidates: `'text' -0.0123` pairs, best first; `decode([id])` gives each candidate's text."""
     return "  ".join(f"{decode([i])!r} {lp:.4f}" for i, lp in cands)
@@ -94,7 +115,8 @@ def format_candidates(cands, decode) -> str:
 
 def main(argv=None) -> int:
     argv = list(sys.argv[1:] if argv is None else argv)
-    sampling = split_sampling(argv)
+    beam = split_beam(argv)
+    sampling = split_sampling(beam[0]) if beam is not None else None
     split = split_top_logprobs(sampling[0]) if sampling is not None else None
     args = parse_args(split[0]) if split is not None else None
     if args is None:
@@ -102,11 +124,19 @@ def main(argv=None) -> int:
         return 1
     model_dir, audio, language, logprobs = args
     top = split[1]
+    _, beam_size, length_penalty = beam
+    temperature = sampling[1]
+    if beam_size > 1 and (top or (temperature is not None and not isinstance(temperature, tuple) and temperature > 0)):
+        print("--beam-size > 1 cannot be combined with --top-logprobs or a temperature > 0", file=sys.stderr)
+        print(USAGE, file=sys.stderr)
+        return 1
     from . import AsrInference
     eng = AsrInference.load(model_dir, device=0)
     try:
         _, temperature, seed = sampling
         kw = {} if temperature is None else dict(temperature=temperature, seed=seed)
+        if beam_size > 1:
+            kw.update(beam_size=beam_size, length_penalty=length_penalty)
         r = eng.transcribe(audio, language, logprobs=logprobs, top_logprobs=top, **kw)
         decode = eng.tokenizer.decode if eng.tokenizer is not None else (lambda ids: " ".join(str(i) for i in ids))
     finally:
@@ -123,6 +153,10 @@ def main(argv=None) -> int:
             print(f"  [{t}] {format_candidates(cands, decode)}")
         if r.eos_top_logprobs is not None:
             print(f"  [eos] {format_candidates(r.eos_top_logprobs, decode)}")
+    if r.nbest is not None:
+        print("N-best:")
+        for j, (text, score) in enumerate(r.nbest):
+            print(f"  [{j}] {score:.4f} {text}")
     return 0
 
 

@@ -16,7 +16,7 @@ SYMBOLS = [
     "asrb_transcribe_ids", "asrb_mel", "asrb_mel_read", "asrb_encode", "asrb_encode_read",
     "asrb_prefill", "asrb_decode_step", "asrb_generate", "asrb_last_timings", "asrb_session_set_option",
     "asrb_debug_mega_timeline", "asrb_session_stats", "asrb_session_device_ids", "asrb_model_lossy_tensors", "asrb_ingest_pcm", "asrb_ingested_read", "asrb_transcribe_ingested",
-    "asrb_last_logprobs", "asrb_last_top_logprobs",
+    "asrb_last_logprobs", "asrb_last_top_logprobs", "asrb_last_nbest", "asrb_last_beam_stats",
 ]
 
 
@@ -82,6 +82,8 @@ def load_library() -> C.CDLL:
         "asrb_transcribe_ingested": [vp, P(P(i64)), P(i32), C.c_int, P(i32), P(i32)],
         "asrb_last_logprobs": [vp, C.c_int, P(C.c_float), P(C.c_float)],
         "asrb_last_top_logprobs": [vp, C.c_int, C.c_int, P(i32), P(C.c_float), P(i32), P(C.c_float)],
+        "asrb_last_nbest": [vp, C.c_int, C.c_int, P(i32), P(i32), P(C.c_float), P(C.c_float), P(i32)],
+        "asrb_last_beam_stats": [vp, P(i64), C.c_int],
     }
     for name, args in sig.items():
         fn = getattr(lib, name)

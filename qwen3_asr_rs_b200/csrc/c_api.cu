@@ -31,6 +31,9 @@ void session_ingest_pcm(Session* s, const void* const* pcm, const int64_t* n_fra
                         const int32_t* format, int batch, int64_t* n_samples_out);
 void session_ingested_read(Session* s, int b, float* out);
 void session_device_ids(Session* s, const int32_t** ids, const int32_t** lens, int* stride, int* batch);
+void session_last_nbest(Session* s, int max_new_tokens, int k, int32_t* ids_out, int32_t* lens_out, float* sum_out,
+                        float* score_out, int32_t* eos_out);
+void session_last_beam_stats(Session* s, int64_t* out, int n);
 int decode_mega_debug_timeline(long long* out, int cap);
 int decode_batch_debug_timeline(long long* out, int cap);
 }  // namespace asrb
@@ -200,6 +203,16 @@ int asrb_last_top_logprobs(asrb_session* s, int max_new_tokens, int k, int32_t* 
         NONNULL(s); NONNULL(ids_out); NONNULL(logprobs_out);
         session_last_top_logprobs(s->s, max_new_tokens, k, ids_out, logprobs_out, eos_ids_out, eos_logprobs_out);
     });
+}
+int asrb_last_nbest(asrb_session* s, int max_new_tokens, int k, int32_t* ids_out, int32_t* lens_out, float* sum_logprob_out,
+                    float* score_out, int32_t* eos_id_out) {
+    return guarded([&] {
+        NONNULL(s); NONNULL(ids_out); NONNULL(lens_out);
+        session_last_nbest(s->s, max_new_tokens, k, ids_out, lens_out, sum_logprob_out, score_out, eos_id_out);
+    });
+}
+int asrb_last_beam_stats(asrb_session* s, int64_t* out, int n) {
+    return guarded([&] { NONNULL(s); NONNULL(out); session_last_beam_stats(s->s, out, n); });
 }
 
 int asrb_debug_mega_timeline(long long* out, int cap) {

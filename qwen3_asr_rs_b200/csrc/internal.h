@@ -220,4 +220,36 @@ void launch_greedy(const Model& m, const DecodeBufs& b, int B, cudaStream_t st, 
 void launch_lmhead_argmax(const Model& m, const float* x_rows, const int* d_row_idx, int B,
                           const DecodeBufs& b, bool write_logits, cudaStream_t st, int64_t* launches);
 
+// beam.cu -- beam search over the TOPK records (session option "beam_size"); the spec is in include/asr_b200.h
+constexpr int BEAM_MAX = 6;
+struct BeamUtt {                   // device state of one utterance's search
+    int t;                         // records consumed = ids in every alive beam
+    int done;                      // K finished hypotheses
+    int S;                         // prompt length
+    int nfin;                      // finished hypotheses so far, in admission order:
+    int fin_depth[BEAM_MAX];       //   last id's depth in the history (-1: no id), = n - 1
+    int fin_slot[BEAM_MAX];        //   its slot at that depth
+    int fin_eos[BEAM_MAX];         //   the EOS id
+    float fin_eos_lp[BEAM_MAX], fin_sum[BEAM_MAX];
+    int slot_of_rank[BEAM_MAX];    // alive beams, best first
+    float sum_of_rank[BEAM_MAX];
+    int cp[BEAM_MAX][BEAM_MAX];    // by beam index: depth of the deepest common node of two beams (-1: the prompt only)
+    long long reassigned, reorder_bytes, expand_bytes;
+};
+struct BeamArgs {
+    int B, K, max_new, hidden, ldh;          // utterances, beams, id capacity, hidden size, history row stride (max_batch)
+    long long bytes_per_pos;                 // K and V bytes of one cache position over all layers and kv heads
+    BeamUtt* u;
+    const int* tk_ids; const float* tk_lp; const int* tk_eos_ids; const float* tk_eos_lp;
+    int *done, *pos, *next_id, *n_out, *ids_out;
+    float* x; const bf16* embed;
+    int *hist_tok, *hist_par; float* hist_lp;   // [max_new][max_batch]: id, parent slot (-1: the prompt), log p
+    int *cp_src, *cp_p0, *cp_n;                 // [max_batch] KV copy plan of the step, by destination slot
+    int* nb_ids; float* nb_lp;                  // [B][K][max_new] ranked hypotheses
+    float *lp_out, *eos_lp;
+    float *kcache, *vcache; int layers, nkv, head_dim, max_ctx; size_t layer_stride, seq_stride;
+};
+void launch_beam_step(const BeamArgs& a, bool first, const int* pos0, cudaStream_t st, int64_t* launches);
+void launch_beam_finalize(const BeamArgs& a, const int* hyp, const float* best_eos_lp, cudaStream_t st, int64_t* launches);
+
 }  // namespace asrb

@@ -87,6 +87,15 @@ struct Session {
     // and the device-resident db.smp, so they apply to the whole run
     double temperature = 0.0; uint64_t seed = 0;
     SampleParams* d_smp = nullptr;
+    // beam search: options "beam_size" (1 = greedy) and "length_penalty" (< 0: none), latched at the prefill into run_k /
+    // run_alpha.  A beam run decodes nslots = B * run_k slots; B stays the number of utterances.
+    int beam_k = 1, run_k = 1, nslots = 0;
+    double length_penalty = -1.0, run_alpha = -1.0;
+    BeamArgs beam{};                    // device buffers (allocated on the first beam run) and the run's geometry
+    int* d_hyp = nullptr; float* d_best_eos = nullptr;   // finalize input: ranked (depth, slot) per hypothesis, rank 0's EOS lp
+    bool nbest_valid = false;           // the last run was a beam run and has been finalized
+    std::vector<float> nb_sum; std::vector<double> nb_score; std::vector<int> nb_eos, nb_n;   // [B][run_k], ranked
+    int64_t beam_steps = 0, beam_reassigned = 0, beam_expand_bytes = 0, beam_reorder_bytes = 0;
     ~Session();
 };
 
@@ -417,9 +426,43 @@ void session_encode_read(Session* s, int b, float* out) {
 // -------------------------------------------------------------------------------------------------
 // steps 4-7: prompt, embed + inject, positions, prefill  (inference.rs:105-149)
 // -------------------------------------------------------------------------------------------------
-// sampling with the top-k candidate lists is not offered: refused by every call that runs a prefill, before any work
-static void check_sampling_options(const Session* s) {
+// sampling with the top-k candidate lists is not offered, nor beam search with either; a beam run needs batch * K slots.
+// Refused by every call that runs a prefill, before any work.
+static void check_sampling_options(const Session* s, int batch) {
     ASRB_REQUIRE(!(s->temperature > 0.0 && s->top_k > 0), ASRB_ERR_INVALID, "temperature > 0 cannot be combined with top_logprobs");
+    if (s->beam_k > 1) {
+        ASRB_REQUIRE(s->temperature == 0.0, ASRB_ERR_INVALID, "beam_size > 1 cannot be combined with temperature > 0");
+        ASRB_REQUIRE(s->top_k == 0, ASRB_ERR_INVALID, "beam_size > 1 cannot be combined with top_logprobs");
+        ASRB_REQUIRE((int64_t)batch * s->beam_k <= s->max_batch, ASRB_ERR_INVALID,
+                     "beam search needs batch * beam_size <= the session's max_batch");
+    }
+}
+
+static void ensure_beam_bufs(Session* s) {
+    BeamArgs& a = s->beam;
+    if (a.u) return;
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    const size_t Bm = s->max_batch, hist = (size_t)s->max_new * Bm, nb = Bm * BEAM_MAX * s->max_new;
+    a.u = salloc<BeamUtt>(s, Bm, true);
+    a.hist_tok = salloc<int>(s, hist); a.hist_par = salloc<int>(s, hist); a.hist_lp = salloc<float>(s, hist);
+    a.cp_src = salloc<int>(s, Bm); a.cp_p0 = salloc<int>(s, Bm); a.cp_n = salloc<int>(s, Bm, true);
+    a.nb_ids = salloc<int>(s, nb); a.nb_lp = salloc<float>(s, nb);
+    s->d_hyp = salloc<int>(s, Bm * BEAM_MAX * 2);
+    s->d_best_eos = salloc<float>(s, Bm);
+}
+
+// the run's geometry and the current decode buffers (the record buffers may have been allocated since the last call)
+static const BeamArgs& beam_args(Session* s) {
+    const Dims& d = s->m->d; const asrb_dims& c = d.c; const DecodeBufs& db = s->db;
+    BeamArgs& a = s->beam;
+    a.B = s->B; a.K = s->run_k; a.max_new = s->max_new; a.hidden = c.hidden_size; a.ldh = s->max_batch;
+    a.bytes_per_pos = 2LL * c.num_hidden_layers * c.num_key_value_heads * c.head_dim * (long long)sizeof(float);
+    a.tk_ids = db.tk_ids; a.tk_lp = db.tk_lp; a.tk_eos_ids = db.tk_eos_ids; a.tk_eos_lp = db.tk_eos_lp;
+    a.done = db.done; a.pos = db.pos; a.next_id = db.next_id; a.n_out = db.n_out; a.ids_out = db.ids_out;
+    a.x = db.x; a.embed = s->m->embed; a.lp_out = db.lp_out; a.eos_lp = db.eos_lp;
+    a.kcache = s->kcache; a.vcache = s->vcache; a.layers = c.num_hidden_layers; a.nkv = c.num_key_value_heads;
+    a.head_dim = c.head_dim; a.max_ctx = s->max_ctx; a.layer_stride = s->cache_layer_stride; a.seq_stride = s->cache_seq_stride;
+    return a;
 }
 
 static void ensure_sample_bufs(Session* s) {     // sampling with logprobs: the raw records beside the keys
@@ -434,10 +477,12 @@ static void ensure_sample_bufs(Session* s) {     // sampling with logprobs: the 
 void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, int64_t* seq_lens_out,
                      float* last_logits) {
     ASRB_REQUIRE(s->stage >= 2, ASRB_ERR_STATE, "prefill called before encode");
-    check_sampling_options(s);
+    check_sampling_options(s, s->B);
     Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
     const int B = s->B; cudaStream_t st = s->st; const int np = s->nplanes;
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
+    s->run_k = s->beam_k; s->run_alpha = s->length_penalty; s->nslots = B * s->run_k; s->nbest_valid = false;
+    if (s->run_k > 1) { ensure_beam_bufs(s); s->beam_steps = 0; }
     s->S.assign(B, 0); s->srow0.assign(B, 0);
     int totS = 0, maxlen = 0;
     for (int b = 0; b < B; ++b) {
@@ -473,7 +518,7 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.pos, di + (pos0 - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
     ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.done, 0, B * sizeof(int), st));
     ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.n_out, 0, B * sizeof(int), st));
-    s->lp_valid = s->db.logprobs;          // latched here: a run records log-probabilities only if it starts with the option on
+    s->lp_valid = s->opt_logprobs || s->top_k > 0;   // latched here: a run records log-probabilities only if it starts with the option on
     if (s->db.logprobs) {                  // all NaN (0xFFFFFFFF): no EOS seen, nothing appended
         ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.eos_lp, 0xFF, B * sizeof(float), st));
         ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.lp_out, 0xFF, (size_t)B * s->max_new * sizeof(float), st));
@@ -530,6 +575,8 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     launch_lmhead_argmax(m, s->hid, s->d_lastrow, B, s->db, last_logits != nullptr, st, &s->launches);
     // greedy bookkeeping for token 0 (inference.rs:161-170): argmax, EOS check, append, embed
     launch_greedy(m, s->db, B, st, &s->launches);
+    // beam search: the token-0 walk on each utterance's record, then its prompt KV copied into its other K - 1 slots
+    if (s->run_k > 1) launch_beam_step(beam_args(s), true, di + (pos0 - hi), st, &s->launches);
     s->greedy_done = 1;
     if (seq_lens_out) for (int b = 0; b < B; ++b) seq_lens_out[b] = s->S[b];
     if (last_logits) {
@@ -553,38 +600,83 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
                              cudaStream_t st, int64_t* launches);
 size_t decode_mega_part_floats(const Model& m);
 int decode_mega_dbg_slots();
+static void apply_record_options(Session* s);
 
 // one iteration of the loop body: decoder forward on the pending token, then the greedy bookkeeping
 // that selects / appends / embeds the next one.  (The fused kernel does both.)
 // upper bound of (position + 1) for the next forward: prompt length + tokens appended so far
 static int ctx_bound(const Session* s) { return std::min(s->max_ctx, s->maxlenS + s->greedy_done); }
+// the decode rows are the nslots sequences of the run: the utterances, or their beam slots
 static bool use_batch(Session* s, bool write_logits) {     // batch >= 2: weights streamed once for all sequences
-    return s->decode_mode == 1 && s->batch_step && !write_logits && s->B >= 2 && decode_batch_supported(*s->m, s->B, ctx_bound(s));
+    return s->decode_mode == 1 && s->batch_step && !write_logits && s->nslots >= 2 && decode_batch_supported(*s->m, s->nslots, ctx_bound(s));
 }
 static bool use_mega(Session* s, bool write_logits) {
     return use_batch(s, write_logits) ||
-           (s->decode_mode == 1 && !write_logits && decode_mega_supported(*s->m, s->B, ctx_bound(s)));
+           (s->decode_mode == 1 && !write_logits && decode_mega_supported(*s->m, s->nslots, ctx_bound(s)));
 }
 static void forward_step(Session* s, bool write_logits) {
     Model& m = *s->m;
+    const int R = s->nslots;
     if (use_batch(s, write_logits)) {
-        launch_decode_step_batch(m, s->db, s->B, s->kcache, s->vcache, s->cache_layer_stride, s->cache_seq_stride, s->max_ctx,
+        launch_decode_step_batch(m, s->db, R, s->kcache, s->vcache, s->cache_layer_stride, s->cache_seq_stride, s->max_ctx,
                                  ctx_bound(s), s->mega, s->st, &s->launches);
         s->n_batch_steps += 1;
     } else if (use_mega(s, write_logits)) {
-        launch_decode_step_mega(m, s->db, s->B, s->kcache, s->vcache, s->cache_layer_stride, s->cache_seq_stride, s->max_ctx,
+        launch_decode_step_mega(m, s->db, R, s->kcache, s->vcache, s->cache_layer_stride, s->cache_seq_stride, s->max_ctx,
                                 ctx_bound(s), s->mega, s->st, &s->launches);
         s->n_mega_steps += 1;
     } else {
         s->n_phase_steps += 1;
-        launch_decode_step_phases(m, s->db, s->B, s->kcache, s->vcache, s->cache_layer_stride, s->cache_seq_stride, s->max_ctx,
+        launch_decode_step_phases(m, s->db, R, s->kcache, s->vcache, s->cache_layer_stride, s->cache_seq_stride, s->max_ctx,
                                   write_logits, s->st, &s->launches);
-        launch_greedy(m, s->db, s->B, s->st, &s->launches);
+        launch_greedy(m, s->db, R, s->st, &s->launches);
     }
+}
+
+// end of a beam run: the finished hypotheses (filled up to K with the alive beams, "no EOS", at the cap) ranked by
+// (sum / P(n) descending, admission order) with P(n) = max(n, 1), or ((5 + n) / 6) ** alpha with a length penalty, in
+// double; then the kernel backtracks them and writes rank 0 into the result rows 0..B-1
+static void beam_finalize(Session* s) {
+    const int B = s->B, K = s->run_k;
+    std::vector<BeamUtt> u((size_t)B);
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(u.data(), s->beam.u, B * sizeof(BeamUtt), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    std::vector<int> hyp((size_t)B * K * 2);
+    std::vector<float> best_eos((size_t)B);
+    s->nb_sum.assign((size_t)B * K, 0.f); s->nb_score.assign((size_t)B * K, 0.0);
+    s->nb_eos.assign((size_t)B * K, -1); s->nb_n.assign((size_t)B * K, 0);
+    s->beam_reassigned = s->beam_expand_bytes = s->beam_reorder_bytes = 0;
+    const float nan = std::numeric_limits<float>::quiet_NaN();
+    for (int b = 0; b < B; ++b) {
+        const BeamUtt& x = u[b];
+        struct H { int depth, slot, eos; float eos_lp, sum; double score; };
+        std::vector<H> h;
+        for (int f = 0; f < x.nfin && f < K; ++f) h.push_back({x.fin_depth[f], x.fin_slot[f], x.fin_eos[f], x.fin_eos_lp[f], x.fin_sum[f], 0.0});
+        for (int r = 0; (int)h.size() < K; ++r) h.push_back({x.t - 1, x.slot_of_rank[r], -1, nan, x.sum_of_rank[r], 0.0});
+        for (H& e : h) {
+            const int n = e.depth + 1;
+            const double p = s->run_alpha < 0.0 ? (double)std::max(n, 1) : std::pow((5.0 + n) / 6.0, s->run_alpha);
+            e.score = (double)e.sum / p;
+        }
+        std::stable_sort(h.begin(), h.end(), [](const H& p, const H& q) { return p.score > q.score; });
+        for (int k = 0; k < K; ++k) {
+            const size_t o = (size_t)b * K + k;
+            hyp[o * 2] = h[k].depth; hyp[o * 2 + 1] = h[k].slot;
+            s->nb_sum[o] = h[k].sum; s->nb_score[o] = h[k].score; s->nb_eos[o] = h[k].eos; s->nb_n[o] = h[k].depth + 1;
+        }
+        best_eos[b] = h[0].eos_lp;
+        s->beam_reassigned += x.reassigned; s->beam_expand_bytes += x.expand_bytes; s->beam_reorder_bytes += x.reorder_bytes;
+    }
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_hyp, hyp.data(), hyp.size() * sizeof(int), cudaMemcpyHostToDevice, s->st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_best_eos, best_eos.data(), best_eos.size() * sizeof(float), cudaMemcpyHostToDevice, s->st));
+    launch_beam_finalize(beam_args(s), s->d_hyp, s->d_best_eos, s->st, &s->launches);
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));     // the host vectors above are pageable
+    s->nbest_valid = true;
 }
 
 void session_decode_step(Session* s, int64_t* next_ids_out, float* logits) {
     ASRB_REQUIRE(s->stage >= 3, ASRB_ERR_STATE, "decode_step called before prefill");
+    ASRB_REQUIRE(s->run_k == 1, ASRB_ERR_INVALID, "decode_step is not available in a beam run (beam_size > 1): use generate");
     Model& m = *s->m; const int B = s->B;
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
     s->lp_valid = s->lp_valid && s->db.logprobs;
@@ -601,16 +693,21 @@ void session_decode_step(Session* s, int64_t* next_ids_out, float* logits) {
 void session_generate(Session* s, int max_new_tokens, int32_t* ids_out, int32_t* lens_out) {
     ASRB_REQUIRE(s->stage >= 3, ASRB_ERR_STATE, "generate called before prefill");
     ASRB_REQUIRE(max_new_tokens >= 1 && max_new_tokens <= s->max_new, ASRB_ERR_INVALID, "max_new_tokens exceeds session capacity");
-    Model& m = *s->m; const int B = s->B; cudaStream_t st = s->st;
+    Model& m = *s->m; const int B = s->B, R = s->nslots; cudaStream_t st = s->st;
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
-    s->lp_valid = s->lp_valid && s->db.logprobs;     // switched off after the prefill: this run's record is incomplete
+    s->lp_valid = s->lp_valid && (s->opt_logprobs || s->top_k > 0);   // switched off after the prefill: this run's record is incomplete
     if (s->tk_valid != s->top_k) s->tk_valid = 0;    // top_logprobs changed after the prefill: likewise
+    const bool beam = s->run_k > 1;
+    // finalize wrote the result rows, which are also the beam-0 slots: the search cannot resume after it
+    ASRB_REQUIRE(!(beam && s->nbest_valid), ASRB_ERR_STATE, "generate: a beam run takes one generate per prefill");
+    struct Restore { Session* s; bool on; ~Restore() { if (on) try { apply_record_options(s); } catch (...) {} } } restore{s, beam};
+    if (beam) { s->db.topk = true; s->db.logprobs = true; }   // the search reads the records, whatever the options now say
     // Token 0 was selected at the end of prefill; each further token costs one forward + greedy.  The
     // reference also runs `forward` after the last appended token and discards its logits
     // (inference.rs:160-200); that wasted forward is not issued here.
     const int steps = std::max(0, max_new_tokens - s->greedy_done);
     auto ensure_graph = [&]() {   // per-phase path: ~142 launches per step -> replay them as one CUDA graph
-        const int mode_key = ((((int)s->db.sample * 2 + (int)s->db.topk) * 2 + (int)s->db.logprobs) * 2 + s->decode_mode) * (s->max_batch + 1) + B;   // unique per (sample, topk, logprobs, mode, batch)
+        const int mode_key = ((((int)s->db.sample * 2 + (int)s->db.topk) * 2 + (int)s->db.logprobs) * 2 + s->decode_mode) * (s->max_batch + 1) + R;   // unique per (sample, topk, logprobs, mode, decode rows)
         if (s->step_graph == nullptr || s->graph_mode != mode_key) {
             if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
             cudaGraph_t g = nullptr;
@@ -631,14 +728,16 @@ void session_generate(Session* s, int max_new_tokens, int32_t* ids_out, int32_t*
         // the fused step covers contexts up to 1152 keys; beyond that (long generations) the per-phase path takes over
         if (use_mega(s, false)) forward_step(s, false);
         else { ensure_graph(); ASRB_CUDA_CHECK(cudaGraphLaunch(s->step_graph, st)); s->launches += s->graph_B; }
+        if (beam) { launch_beam_step(beam_args(s), false, nullptr, st, &s->launches); s->beam_steps += 1; }   // select, reorder
         s->decode_steps += 1; s->greedy_done += 1;
         if ((it + 1) % check_every == 0 && it + 1 < steps) {
-            ASRB_CUDA_CHECK(cudaMemcpyAsync(s->h_done, s->db.done, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+            ASRB_CUDA_CHECK(cudaMemcpyAsync(s->h_done, s->db.done, R * sizeof(int), cudaMemcpyDeviceToHost, st));
             ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
             all_done = true;
-            for (int b = 0; b < B; ++b) all_done = all_done && s->h_done[b];
+            for (int b = 0; b < R; ++b) all_done = all_done && s->h_done[b];
         }
     }
+    if (beam) beam_finalize(s);     // result rows 0..B-1: the best hypothesis of each utterance
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->h_nout, s->db.n_out, B * sizeof(int), cudaMemcpyDeviceToHost, st));
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->h_ids, s->db.ids_out, (size_t)B * s->max_new * sizeof(int), cudaMemcpyDeviceToHost, st));
     ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -653,8 +752,8 @@ void session_transcribe_ids(Session* s, const float* const* samples, const int64
                             const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
                             int32_t* ids_out, int32_t* lens_out) {
     ASRB_REQUIRE(ids_out && lens_out, ASRB_ERR_INVALID, "null output");
-    check_sampling_options(s);
     if (samples == nullptr) batch = (int)s->ingested_n.size();      // asrb_transcribe_ingested
+    check_sampling_options(s, batch);
     ASRB_REQUIRE(max_new_tokens >= 1 && max_new_tokens <= s->max_new, ASRB_ERR_INVALID, "max_new_tokens exceeds session capacity");
     cudaStream_t st = s->st;
     s->launches = 0; s->decode_steps = 0;
@@ -745,12 +844,44 @@ void session_stats(Session* s, int64_t* out, int n) {
     for (int i = 0; i < n && i < 5; ++i) out[i] = v[i];
 }
 
-// options "logprobs" / "top_logprobs" -> kernel variants; buffers are allocated when first needed, so a session that
-// never records keeps its allocations unchanged
+// ranked hypotheses of the last beam run: ids [batch][k][max_new_tokens] (-1 beyond the length), lens / sums / scores /
+// EOS ids (-1: stopped by the cap) [batch][k]
+void session_last_nbest(Session* s, int max_new_tokens, int k, int32_t* ids_out, int32_t* lens_out, float* sum_out,
+                        float* score_out, int32_t* eos_out) {
+    ASRB_REQUIRE(s->stage >= 3 && s->nbest_valid, ASRB_ERR_STATE, "last_nbest: the last run was not a beam run");
+    ASRB_REQUIRE(max_new_tokens >= 1, ASRB_ERR_INVALID, "max_new_tokens must be >= 1");
+    ASRB_REQUIRE(k >= 1 && k <= s->run_k, ASRB_ERR_INVALID, "k must be in [1, beam_size of the last run]");
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    const int B = s->B, K = s->run_k;
+    std::vector<int32_t> ids((size_t)B * K * s->max_new);
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(ids.data(), s->beam.nb_ids, ids.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    for (int b = 0; b < B; ++b)
+        for (int j = 0; j < k; ++j) {
+            const size_t o = (size_t)b * K + j, d = (size_t)b * k + j;
+            const int n = std::min(s->nb_n[o], max_new_tokens);
+            if (ids_out)
+                for (int i = 0; i < max_new_tokens; ++i) ids_out[d * max_new_tokens + i] = i < n ? ids[o * s->max_new + i] : -1;
+            if (lens_out) lens_out[d] = n;
+            if (sum_out) sum_out[d] = s->nb_sum[o];
+            if (score_out) score_out[d] = (float)s->nb_score[o];
+            if (eos_out) eos_out[d] = s->nb_eos[o];
+        }
+}
+
+// [0] beam steps  [1] slots reassigned  [2] KV bytes copied by the expansion  [3] KV bytes copied by reorders
+void session_last_beam_stats(Session* s, int64_t* out, int n) {
+    ASRB_REQUIRE(s->nbest_valid, ASRB_ERR_STATE, "last_beam_stats: the last run was not a beam run");
+    const int64_t v[4] = {s->beam_steps, s->beam_reassigned, s->beam_expand_bytes, s->beam_reorder_bytes};
+    for (int i = 0; i < n && i < 4; ++i) out[i] = v[i];
+}
+
+// options "logprobs" / "top_logprobs" / "beam_size" -> kernel variants; buffers are allocated when first needed, so a
+// session that never records keeps its allocations unchanged.  Beam search reads the TOPK records.
 static void apply_record_options(Session* s) {
     DecodeBufs& b = s->db;
-    b.logprobs = s->opt_logprobs || s->top_k > 0;    // the candidates' values need the selected token's log-probability
-    b.topk = s->top_k > 0;
+    b.logprobs = s->opt_logprobs || s->top_k > 0 || s->beam_k > 1;   // the candidates' values need the selected token's log-probability
+    b.topk = s->top_k > 0 || s->beam_k > 1;
     if (b.logprobs && !b.lp_out) {
         ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
         b.part_sum = salloc<float>(s, (size_t)s->max_batch * b.n_part);
@@ -781,6 +912,17 @@ static double parse_temperature(const std::string& v) {
     ASRB_REQUIRE(end && *end == '\0' && errno == 0 && std::isfinite(t), ASRB_ERR_INVALID, "temperature must be a decimal number");
     ASRB_REQUIRE(t == 0.0 || (t >= 1e-6 && t <= 100.0), ASRB_ERR_INVALID, "temperature must be 0 or in [1e-6, 100]");
     return t;
+}
+static double parse_length_penalty(const std::string& v) {     // "none" is handled by the caller
+    ASRB_REQUIRE(!v.empty() && (isdigit((unsigned char)v[0]) || v[0] == '.') &&
+                 v.find_first_not_of("0123456789.eE+-") == std::string::npos,
+                 ASRB_ERR_INVALID, "length_penalty must be none or a decimal number");
+    errno = 0;
+    char* end = nullptr;
+    const double a = strtod(v.c_str(), &end);
+    ASRB_REQUIRE(end && *end == '\0' && errno == 0 && std::isfinite(a) && a >= 0.0 && a <= 10.0, ASRB_ERR_INVALID,
+                 "length_penalty must be none or a decimal in [0, 10]");
+    return a;
 }
 static uint64_t parse_seed(const std::string& v) {
     ASRB_REQUIRE(!v.empty() && isdigit((unsigned char)v[0]), ASRB_ERR_INVALID, "seed must be a decimal unsigned 64-bit integer");
@@ -820,6 +962,12 @@ void session_set_option(Session* s, const char* key, const char* value) {
         s->temperature = parse_temperature(v);
     } else if (k == "seed") {
         s->seed = parse_seed(v);
+    } else if (k == "beam_size") {
+        ASRB_REQUIRE(v.size() == 1 && v[0] >= '1' && v[0] <= '0' + BEAM_MAX, ASRB_ERR_INVALID, "beam_size must be 1..6");
+        s->beam_k = v[0] - '0';
+        apply_record_options(s);
+    } else if (k == "length_penalty") {
+        s->length_penalty = v == "none" ? -1.0 : parse_length_penalty(v);
     } else throw Error(ASRB_ERR_INVALID, "unknown option: " + k);
 }
 

@@ -77,6 +77,40 @@ def check_seed(seed) -> int:
     return int(seed)
 
 
+BEAM_MAX = 6
+
+
+def check_beam(beam_size, length_penalty) -> Tuple[int, Optional[float]]:
+    """The `beam_size` (an int in 1..6; 1: greedy) and `length_penalty` (None, or a finite value in [0, 10]) arguments,
+    else ValueError."""
+    if not isinstance(beam_size, (int, np.integer)) or isinstance(beam_size, bool) or not 1 <= beam_size <= BEAM_MAX:
+        raise ValueError(f"beam_size must be an int in 1..{BEAM_MAX}, got {beam_size!r}")
+    if length_penalty is not None:
+        if isinstance(length_penalty, bool) or not isinstance(length_penalty, (int, float, np.integer, np.floating)) \
+                or not math.isfinite(float(length_penalty)) or not 0.0 <= float(length_penalty) <= 10.0:
+            raise ValueError(f"length_penalty must be None or a finite value in [0, 10], got {length_penalty!r}")
+        length_penalty = float(length_penalty)
+    return int(beam_size), length_penalty
+
+
+def length_penalty_option(a: Optional[float]) -> str:
+    """The session option string of length penalty a (None: "none")."""
+    return "none" if a is None else repr(float(a))
+
+
+def beam_score(sum_logprob: float, n: int, length_penalty: Optional[float]) -> float:
+    """A hypothesis's score: sum / P(n), P(n) = max(n, 1) without a length penalty, else ((5 + n) / 6) ** alpha (the
+    library computes it in double from the fp32 sum)."""
+    p = float(max(n, 1)) if length_penalty is None else ((5.0 + n) / 6.0) ** length_penalty
+    return float(sum_logprob) / p
+
+
+def rank_hypotheses(hyps: Sequence[Tuple[int, float]], length_penalty: Optional[float]) -> List[int]:
+    """Indices of hypotheses (n ids, sum) given in admission order, ranked by (score descending, admission order)."""
+    scores = [beam_score(sm, n, length_penalty) for n, sm in hyps]
+    return sorted(range(len(hyps)), key=lambda i: (-scores[i], i))
+
+
 def temperature_option(t: float) -> str:
     """The session option string of temperature t (a decimal the library parses exactly back to t)."""
     return "0" if t == 0.0 else repr(float(t))
@@ -129,6 +163,7 @@ class TranscribeResult:           # inference.rs:270-274
     top_logprobs: Optional[List[List[Tuple[int, float]]]] = None
     eos_top_logprobs: Optional[List[Tuple[int, float]]] = None   # ... of the step that selected EOS (None: stopped by the cap)
     temperature: Optional[float] = None             # transcribe(temperature=...): that of the kept attempt
+    nbest: Optional[List[Tuple[str, float]]] = None   # transcribe(beam_size=K > 1): the K hypotheses as (text, score), ranked
 
 
 @dataclass
@@ -145,6 +180,9 @@ class TranscribeIds:
     eos_top_logprobs: Optional[List[Optional[List[Tuple[int, float]]]]] = None
     # temperature=T or a schedule: per utterance, the temperature of the attempt kept (None for a plain greedy call)
     temperatures: Optional[List[float]] = None
+    # beam_size=K > 1: per utterance, its K hypotheses ranked as (ids, sum_logprob, score, eos_id; -1 = stopped by the
+    # cap); entry 0 is `ids` (None for an attempt that sampled)
+    nbest: Optional[List[Optional[List[Tuple[List[int], float, float, int]]]]] = None
 
 
 class AsrInference:
@@ -344,7 +382,47 @@ class AsrInference:
         eos = [None if eids[b, 0] < 0 else [(int(i), float(v)) for i, v in zip(eids[b], elp[b])] for b in range(B)]
         return rows, eos
 
-    def _finish(self, s, B: int, ids, n, max_new_tokens: int, logprobs: bool, top_logprobs: int = 0) -> TranscribeIds:
+    # ---- beam search (session options "beam_size" / "length_penalty") ------------------------------------------
+    def last_nbest(self, max_new_tokens: int, k: int):
+        """asrb_last_nbest: per utterance of the last beam run, its k best hypotheses ranked as (ids, sum_logprob,
+        score, eos_id; -1 = stopped by the cap).  Raises AsrbError: ASRB_ERR_STATE when the last run was not a beam
+        run, ASRB_ERR_INVALID when k is outside [1, beam_size]."""
+        if self._session is None:
+            raise _lib.AsrbError(4, "no session: nothing has run yet")
+        B = getattr(self, "_B", self._cap[0])
+        kk = max(int(k), 1)
+        ids = np.full((B, kk, max_new_tokens), -1, dtype=np.int32)
+        lens = np.zeros((B, kk), dtype=np.int32)
+        sums = np.zeros((B, kk), dtype=np.float32)
+        scores = np.zeros((B, kk), dtype=np.float32)
+        eos = np.zeros((B, kk), dtype=np.int32)
+        P = C.POINTER
+        _lib.check(self._lib.asrb_last_nbest(self._session, int(max_new_tokens), int(k), ids.ctypes.data_as(P(C.c_int32)),
+                                             lens.ctypes.data_as(P(C.c_int32)), sums.ctypes.data_as(P(C.c_float)),
+                                             scores.ctypes.data_as(P(C.c_float)), eos.ctypes.data_as(P(C.c_int32))))
+        return [[(ids[b, j, : lens[b, j]].tolist(), float(sums[b, j]), float(scores[b, j]), int(eos[b, j])) for j in range(kk)]
+                for b in range(B)]
+
+    def last_beam_stats(self) -> Dict[str, int]:
+        """asrb_last_beam_stats: counters of the last beam run."""
+        out = (C.c_int64 * 4)()
+        _lib.check(self._lib.asrb_last_beam_stats(self._session, out, 4))
+        return dict(zip(("beam_steps", "slots_reassigned", "expand_kv_bytes", "reorder_kv_bytes"), [int(v) for v in out]))
+
+    def _set_beam(self, s, k: int, length_penalty: Optional[float]) -> List[Tuple[str, str]]:
+        """Set beam_size k and the length penalty for one call; returns the (option, configured value) pairs to
+        restore.  Nothing is set when they agree (setting an option drops the captured per-phase step graph)."""
+        undo = []
+        vals = (("beam_size", str(k)), ("length_penalty", length_penalty_option(length_penalty))) if k > 1 else (("beam_size", "1"),)
+        for key, val in vals:
+            conf = self._options.get(key, {"beam_size": "1", "length_penalty": "none"}[key])
+            if conf != val:
+                _lib.check(self._lib.asrb_session_set_option(s, key.encode(), val.encode()))
+                undo.append((key, conf))
+        return undo
+
+    def _finish(self, s, B: int, ids, n, max_new_tokens: int, logprobs: bool, top_logprobs: int = 0,
+                beam_size: int = 1) -> TranscribeIds:
         ms = (C.c_float * 6)()
         k, st = C.c_int64(), C.c_int64()
         _lib.check(self._lib.asrb_last_timings(s, ms, C.byref(k), C.byref(st)))
@@ -355,6 +433,8 @@ class AsrInference:
             r.logprobs, r.eos_logprobs = self.last_logprobs(max_new_tokens)
         if top_logprobs:
             r.top_logprobs, r.eos_top_logprobs = self.last_top_logprobs(max_new_tokens, top_logprobs)
+        if beam_size > 1:
+            r.nbest = self.last_nbest(max_new_tokens, beam_size)
         return r
 
     # ---- seeded temperature sampling (session options "temperature" / "seed") ---------------------------
@@ -374,22 +454,32 @@ class AsrInference:
         for key, conf in undo:
             _lib.check(self._lib.asrb_session_set_option(s, key.encode(), conf.encode()))
 
-    def _sampled(self, B: int, once, temperature, seed, logprob_threshold, logprobs: bool, top_logprobs: int) -> TranscribeIds:
-        """One call of transcribe_ids / transcribe_pcm.  `once(indices, logprobs, top_logprobs, t)` runs the utterances
-        `indices` at temperature t (None: the session's configured options)."""
+    def _sampled(self, B: int, once, temperature, seed, logprob_threshold, logprobs: bool, top_logprobs: int,
+                 beam_size: int = 1, length_penalty: Optional[float] = None) -> TranscribeIds:
+        """One call of transcribe_ids / transcribe_pcm.  `once(indices, logprobs, top_logprobs, t, beam)` runs the
+        utterances `indices` at temperature t (None: the session's configured options) with beam = (K, length penalty)
+        (None: greedy or sampling).  With a schedule, attempts at t = 0 run the beam search and attempts at t > 0
+        sample, as in Whisper."""
         top_logprobs = check_top_logprobs(top_logprobs)
         temps = check_temperature(temperature)
         seed = check_seed(seed)
+        beam_size, length_penalty = check_beam(beam_size, length_penalty)
         schedule = isinstance(temperature, (list, tuple))
         if top_logprobs and any(t > 0.0 for t in temps):
             raise ValueError("temperature > 0 cannot be combined with top_logprobs")
-        if not schedule and temps[0] == 0.0:                 # plain greedy call: the session's options as configured
-            return once(list(range(B)), logprobs, top_logprobs, None)
+        if beam_size > 1 and top_logprobs:
+            raise ValueError("beam_size > 1 cannot be combined with top_logprobs")
+        if beam_size > 1 and not schedule and temps[0] > 0.0:
+            raise ValueError("beam_size > 1 cannot be combined with temperature > 0 (a schedule runs the beam at t = 0)")
+        beam = (beam_size, length_penalty) if beam_size > 1 else None
+        if not schedule and temps[0] == 0.0:                 # plain greedy / beam call: the session's options as configured
+            return once(list(range(B)), logprobs, top_logprobs, None, beam)
         if not schedule:
-            r = once(list(range(B)), logprobs, 0, temps[0])
+            r = once(list(range(B)), logprobs, 0, temps[0], None)
             r.temperatures = [temps[0]] * B
             return r
-        kept, used, runs = temperature_fallback(lambda idx, t: once(idx, True, 0, t), B, temps, logprob_threshold)
+        kept, used, runs = temperature_fallback(lambda idx, t: once(idx, True, 0, t, beam if t == 0.0 else None), B, temps,
+                                                logprob_threshold)
         r = TranscribeIds([k[0].ids[k[1]] for k in kept], {}, sum(x.kernels_launched for x in runs),
                           sum(x.decode_steps for x in runs))
         for x in runs:
@@ -398,31 +488,39 @@ class AsrInference:
         r.logprobs = [k[0].logprobs[k[1]] for k in kept]
         r.eos_logprobs = [k[0].eos_logprobs[k[1]] for k in kept]
         r.temperatures = used
+        if beam is not None:
+            r.nbest = [k[0].nbest[k[1]] if k[0].nbest is not None else None for k in kept]
         return r
 
     # ---- the hot path ----------------------------------------------------------------
     def transcribe_ids(self, clips: Sequence[np.ndarray], language_ids: Optional[Sequence] = None,
                        max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0,
                        temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
-                       logprob_threshold: Optional[float] = -1.0) -> TranscribeIds:
+                       logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
+                       length_penalty: Optional[float] = None) -> TranscribeIds:
         """transcribe() steps 2-8 for a batch: host f32 samples in, host token ids out (and, with `logprobs`, the
         log-probability of every id and of the ending EOS, from the kernels that selected them; with `top_logprobs` = k
         in 1..8, also the k best candidates of each of those steps, and the log-probabilities as with `logprobs`).
         `temperature` T > 0 samples every id with the seeded Gumbel-max draw of the kernels (ids are a pure function of
         the inputs, `seed`, T and the batch order); a sequence of temperatures is a fallback schedule
-        (temperature_fallback) with the log-probability record on and `logprob_threshold` (None: off)."""
-        def once(idx, lp, k, t):
+        (temperature_fallback) with the log-probability record on and `logprob_threshold` (None: off).
+        `beam_size` K in 2..6 decodes every utterance with beam search (the session holds batch x K slots; `nbest`
+        holds the K ranked hypotheses, `ids` the best) scored with `length_penalty` (None: sum / length); with a
+        schedule, only the attempts at t = 0 use it."""
+        def once(idx, lp, k, t, beam):
             sub = clips if len(idx) == len(clips) else [clips[i] for i in idx]
             lang = None if language_ids is None else [language_ids[i] for i in idx]
-            return self._ids_once(sub, lang, max_new_tokens, lp, k, t, seed)
-        return self._sampled(len(clips), once, temperature, seed, logprob_threshold, logprobs, top_logprobs)
+            return self._ids_once(sub, lang, max_new_tokens, lp, k, t, seed, beam)
+        return self._sampled(len(clips), once, temperature, seed, logprob_threshold, logprobs, top_logprobs,
+                             beam_size, length_penalty)
 
     def _ids_once(self, clips, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
-                  temperature: Optional[float], seed: int) -> TranscribeIds:
+                  temperature: Optional[float], seed: int, beam=None) -> TranscribeIds:
         B = len(clips)
+        K = beam[0] if beam else 1
         arrs, ptrs, lens = self._pack_samples(clips)
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
-        s = self._ensure_session(B, max(a.shape[0] for a in arrs), mx, max_new_tokens)
+        s = self._ensure_session(B * K, max(a.shape[0] for a in arrs), mx, max_new_tokens)
         ids = np.zeros((B, max_new_tokens), dtype=np.int32)
         n = np.zeros(B, dtype=np.int32)
         if logprobs:
@@ -432,10 +530,11 @@ class AsrInference:
         undo = []
         try:
             undo = self._set_sampling(s, temperature, seed)
+            undo += self._set_beam(s, K, beam[1] if beam else None)
             _lib.check(self._lib.asrb_transcribe_ids(
                 s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
                 ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
-            return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs)
+            return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs, K)
         finally:
             self._restore(s, undo)
             if logprobs:
@@ -446,14 +545,14 @@ class AsrInference:
     # ---- GPU-side audio ingest (step 1, src/audio.rs:162-245) -------------------------------------------
     _PCM_FMT = {"int16": 0, "float32": 1, "int32": 2}
 
-    def _ingest(self, pcms: Sequence, rates: Sequence[int], max_lang: int, max_new: int):
+    def _ingest(self, pcms: Sequence, rates: Sequence[int], max_lang: int, max_new: int, slots: int = 0):
         B = len(pcms)
         arrs = [np.ascontiguousarray(a if a.ndim == 2 else a.reshape(-1, 1)) for a in pcms]
         for a in arrs:
             if a.dtype.name not in self._PCM_FMT:
                 raise ValueError(f"PCM dtype must be int16 / int32 / float32, got {a.dtype}")
         n_out = [-(-a.shape[0] * MEL_SAMPLE_RATE // int(r)) for a, r in zip(arrs, rates)]
-        s = self._ensure_session(B, max(n_out), max_lang, max_new)
+        s = self._ensure_session(max(B, slots), max(n_out), max_lang, max_new)
         ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in arrs])
         frames = (C.c_int64 * B)(*[a.shape[0] for a in arrs])
         chans = (C.c_int32 * B)(*[a.shape[1] for a in arrs])
@@ -476,20 +575,24 @@ class AsrInference:
     def transcribe_pcm(self, pcms: Sequence, rates: Sequence[int], language_ids: Optional[Sequence] = None,
                        max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0,
                        temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
-                       logprob_threshold: Optional[float] = -1.0) -> TranscribeIds:
+                       logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
+                       length_penalty: Optional[float] = None) -> TranscribeIds:
         """transcribe() steps 1-8 for a batch with step 1 on the GPU: raw PCM in, token ids out (`logprobs`,
-        `top_logprobs`, `temperature`, `seed`, `logprob_threshold`: as in transcribe_ids)."""
-        def once(idx, lp, k, t):
+        `top_logprobs`, `temperature`, `seed`, `logprob_threshold`, `beam_size`, `length_penalty`: as in
+        transcribe_ids)."""
+        def once(idx, lp, k, t, beam):
             sel = (lambda xs: xs if len(idx) == len(pcms) else [xs[i] for i in idx])
             lang = None if language_ids is None else sel(language_ids)
-            return self._pcm_once(sel(pcms), sel(rates), lang, max_new_tokens, lp, k, t, seed)
-        return self._sampled(len(pcms), once, temperature, seed, logprob_threshold, logprobs, top_logprobs)
+            return self._pcm_once(sel(pcms), sel(rates), lang, max_new_tokens, lp, k, t, seed, beam)
+        return self._sampled(len(pcms), once, temperature, seed, logprob_threshold, logprobs, top_logprobs,
+                             beam_size, length_penalty)
 
     def _pcm_once(self, pcms, rates, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
-                  temperature: Optional[float], seed: int) -> TranscribeIds:
+                  temperature: Optional[float], seed: int, beam=None) -> TranscribeIds:
         B = len(pcms)
+        K = beam[0] if beam else 1
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
-        s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens)
+        s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens, slots=B * K)
         ids = np.zeros((B, max_new_tokens), dtype=np.int32)
         n = np.zeros(B, dtype=np.int32)
         if logprobs:
@@ -499,9 +602,10 @@ class AsrInference:
         undo = []
         try:
             undo = self._set_sampling(s, temperature, seed)
+            undo += self._set_beam(s, K, beam[1] if beam else None)
             _lib.check(self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens),
                                                           ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
-            return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs)
+            return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs, K)
         finally:
             self._restore(s, undo)
             if logprobs:
@@ -512,13 +616,16 @@ class AsrInference:
     def transcribe(self, audio_path: str, language: Optional[str] = None,
                    max_new_tokens: int = MAX_NEW_TOKENS, gpu_ingest: bool = True, logprobs: bool = False,
                    top_logprobs: int = 0, temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
-                   logprob_threshold: Optional[float] = -1.0) -> TranscribeResult:
+                   logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
+                   length_penalty: Optional[float] = None) -> TranscribeResult:
         """AsrInference::transcribe (inference.rs:89-213): step 1 (WAV payload -> mono 16 kHz; on the GPU by default,
         `gpu_ingest=False` = the host loader) -> steps 2-8 on the GPU -> step 9 (detokenise + parse, host; needs
         tokenizer.json, else raw_output is the id list as text).  `logprobs`: also fill token_logprobs / avg_logprob;
         `top_logprobs` = k in 1..8: also fill top_logprobs (and token_logprobs / avg_logprob); `temperature`, `seed`,
-        `logprob_threshold`: as in transcribe_ids, and `temperature` of the result is that of the kept attempt."""
-        sampling = dict(temperature=temperature, seed=seed, logprob_threshold=logprob_threshold)
+        `logprob_threshold`, `beam_size`, `length_penalty`: as in transcribe_ids, and `temperature` of the result is that
+        of the kept attempt; `nbest` holds the beam's hypotheses as (text, score)."""
+        sampling = dict(temperature=temperature, seed=seed, logprob_threshold=logprob_threshold, beam_size=beam_size,
+                        length_penalty=length_penalty)
         from .audio import load_wav, read_wav_pcm
         from .text import language_prompt_ids, parse_asr_output
         lang_ids = language_prompt_ids(self.tokenizer, language)
@@ -531,9 +638,14 @@ class AsrInference:
             r = self.transcribe_ids([samples], language_ids=[lang_ids] if lang_ids is not None else None,
                                     max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs, **sampling)
         ids = r.ids[0]
-        raw = self.tokenizer.decode(ids) if self.tokenizer is not None else " ".join(str(i) for i in ids)
-        lang, text = parse_asr_output(raw, language is not None) if self.tokenizer is not None else ("unknown", raw)
+
+        def parse(ids):
+            raw = self.tokenizer.decode(ids) if self.tokenizer is not None else " ".join(str(i) for i in ids)
+            return raw, (parse_asr_output(raw, language is not None) if self.tokenizer is not None else ("unknown", raw))
+        raw, (lang, text) = parse(ids)
         res = TranscribeResult(text=text, language=lang, raw_output=raw, ids=ids)
+        if r.nbest is not None and r.nbest[0] is not None:
+            res.nbest = [(parse(h[0])[1][1], h[2]) for h in r.nbest[0]]
         if r.temperatures is not None:
             res.temperature = r.temperatures[0]
         if (logprobs or top_logprobs or r.temperatures is not None) and r.logprobs is not None:

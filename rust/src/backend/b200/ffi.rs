@@ -68,5 +68,8 @@ extern "C" {
     pub fn asrb_last_logprobs(s: *mut asrb_session, max_new_tokens: c_int, logprobs_out: *mut f32, eos_logprob_out: *mut f32) -> c_int;
     pub fn asrb_last_top_logprobs(s: *mut asrb_session, max_new_tokens: c_int, k: c_int, ids_out: *mut i32, logprobs_out: *mut f32,
                                   eos_ids_out: *mut i32, eos_logprobs_out: *mut f32) -> c_int;
+    pub fn asrb_last_nbest(s: *mut asrb_session, max_new_tokens: c_int, k: c_int, ids_out: *mut i32, lens_out: *mut i32,
+                           sum_logprob_out: *mut f32, score_out: *mut f32, eos_id_out: *mut i32) -> c_int;
+    pub fn asrb_last_beam_stats(s: *mut asrb_session, out: *mut i64, n: c_int) -> c_int;
     pub fn asrb_debug_mega_timeline(out: *mut c_longlong, cap: c_int) -> c_int;
 }

@@ -25,7 +25,7 @@ impl Drop for Session { fn drop(&mut self) { unsafe { ffi::asrb_session_free(sel
 /// arbitrary-length audio; a session sized for the worst case up front would pin ~1 GB of scratch per minute of audio).
 /// Field order = drop order: session before model before context.
 pub struct B200Engine {
-    session: std::cell::RefCell<Option<(Session, usize)>>,   // (handle, capacity in samples)
+    session: std::cell::RefCell<Option<(Session, usize, usize)>>,   // (handle, capacity in samples, slots)
     model: Model,
     _ctx: Ctx,
     max_new_tokens: usize,
@@ -50,16 +50,21 @@ impl B200Engine {
     }
 
     /// Session with room for `n_samples`: capacity grows in 30 s steps, the old session is dropped first.
-    fn session_for(&self, n_samples: usize) -> Result<*mut ffi::asrb_session> {
+    fn session_for(&self, n_samples: usize) -> Result<*mut ffi::asrb_session> { self.session_for_slots(n_samples, 1) }
+
+    /// Session with room for `n_samples` and `slots` decode rows (a beam search of K needs K); neither shrinks.
+    fn session_for_slots(&self, n_samples: usize, slots: usize) -> Result<*mut ffi::asrb_session> {
         let mut slot = self.session.borrow_mut();
-        if let Some((s, cap)) = slot.as_ref() {
-            if *cap >= n_samples { return Ok(s.0); }
+        let mut rows = slots;
+        if let Some((s, cap, have)) = slot.as_ref() {
+            if *cap >= n_samples && *have >= slots { return Ok(s.0); }
+            rows = rows.max(*have);
         }
         *slot = None;
         let cap = ((n_samples + 479_999) / 480_000).max(1) * 480_000;
         let mut session = ptr::null_mut();
-        check(unsafe { ffi::asrb_session_create(self.model.0, 1, cap as i64, 16, self.max_new_tokens as i32, &mut session) })?;
-        *slot = Some((Session(session), cap));
+        check(unsafe { ffi::asrb_session_create(self.model.0, rows as i32, cap as i64, 16, self.max_new_tokens as i32, &mut session) })?;
+        *slot = Some((Session(session), cap, rows));
         Ok(session)
     }
 
@@ -159,6 +164,42 @@ impl B200Engine {
         let run = set.and_then(|_| self.transcribe_ids(samples, lang_ids));
         check(unsafe { ffi::asrb_session_set_option(session, tkey.as_ptr(), zero.as_ptr()) })?;
         check(unsafe { ffi::asrb_session_set_option(session, skey.as_ptr(), zero.as_ptr()) })?;
+        run
+    }
+
+    /// `transcribe_ids` with beam search of `beam_size` (2..=6) beams, the options "beam_size" / "length_penalty"
+    /// (`include/asr_b200.h`; `length_penalty` None scores by sum / length).  Returns the `beam_size` hypotheses
+    /// ranked best first as (ids, sum of log-probabilities, score, EOS id or -1 when stopped by `max_new_tokens`);
+    /// entry 0 is what `transcribe_ids` would return under these options.  The options are restored afterwards.
+    pub fn transcribe_ids_beam(&self, samples: &[f32], lang_ids: Option<&[i64]>, beam_size: usize, length_penalty: Option<f32>)
+        -> Result<Vec<(Vec<i64>, f32, f32, i64)>> {
+        if !(2..=6).contains(&beam_size) { return Err(anyhow!("beam_size must be in 2..=6, got {beam_size}")); }
+        let session = self.session_for_slots(samples.len(), beam_size)?;
+        let bkey = CString::new("beam_size")?;
+        let lkey = CString::new("length_penalty")?;
+        let bval = CString::new(beam_size.to_string())?;
+        let lval = CString::new(length_penalty.map_or("none".to_string(), |a| format!("{a}")))?;
+        let (one, none) = (CString::new("1")?, CString::new("none")?);
+        let set = (|| -> Result<()> {
+            check(unsafe { ffi::asrb_session_set_option(session, bkey.as_ptr(), bval.as_ptr()) })?;
+            check(unsafe { ffi::asrb_session_set_option(session, lkey.as_ptr(), lval.as_ptr()) })
+        })();
+        let run = set.and_then(|_| self.transcribe_ids(samples, lang_ids)).and_then(|_| {
+            let (k, m) = (beam_size, self.max_new_tokens);
+            let mut ids = vec![-1i32; k * m];
+            let mut lens = vec![0i32; k];
+            let mut sums = vec![0f32; k];
+            let mut scores = vec![0f32; k];
+            let mut eos = vec![-1i32; k];
+            check(unsafe {
+                ffi::asrb_last_nbest(session, m as i32, k as i32, ids.as_mut_ptr(), lens.as_mut_ptr(), sums.as_mut_ptr(),
+                                     scores.as_mut_ptr(), eos.as_mut_ptr())
+            })?;
+            Ok((0..k).map(|j| (ids[j * m..j * m + lens[j] as usize].iter().map(|&t| t as i64).collect(), sums[j], scores[j],
+                               eos[j] as i64)).collect())
+        });
+        check(unsafe { ffi::asrb_session_set_option(session, bkey.as_ptr(), one.as_ptr()) })?;
+        check(unsafe { ffi::asrb_session_set_option(session, lkey.as_ptr(), none.as_ptr()) })?;
         run
     }
 }
