@@ -96,6 +96,11 @@ ASRB_API int asrb_model_free(asrb_model* m);
  * ids (the reference caps at 4096, src/inference.rs:153). */
 ASRB_API int asrb_session_create(asrb_model* m, int max_batch, int64_t max_samples,
                         int max_lang_ids, int max_new_tokens, asrb_session** out);
+/* asrb_session_create with room for up to max_context_ids context ids per utterance (asrb_session_set_context);
+ * asrb_session_create is this call with max_context_ids = 0.  Every prompt, the KV cache and the RoPE-table check
+ * (prompt + max_new_tokens positions) include them. */
+ASRB_API int asrb_session_create_ex(asrb_model* m, int max_batch, int64_t max_samples, int max_lang_ids,
+                                    int max_context_ids, int max_new_tokens, asrb_session** out);
 ASRB_API int asrb_session_free(asrb_session* s);
 
 /* Whole hot path, the call `transcribe()` makes once per file (src/inference.rs:94-200)
@@ -243,6 +248,29 @@ ASRB_API int asrb_last_nbest(asrb_session* s, int max_new_tokens, int k, int32_t
 /* Counters of the last beam run: [0] beam steps  [1] slots reassigned  [2] KV bytes copied by the prompt expansion
  * [3] KV bytes copied by reorders; writes min(n, 4) values.  ASRB_ERR_STATE if the last run was not a beam run. */
 ASRB_API int asrb_last_beam_stats(asrb_session* s, int64_t* out, int n);
+
+/* Context biasing: ids placed as the content of the prompt's system turn (a keyword list, names, related text; the
+ * model's own `context`).  Utterance b with context ids c_b (length L_b >= 0) gets the prompt
+ *   [151644, 8948, 198] + c_b + [151645, 198, 151644, 872, 198, 151669] + audio pads + tail + language ids
+ * at positions 0..S_b-1, S_b = 15 + L_b + audio tokens + language ids; with L_b = 0 it is the prompt without context.
+ *   n_rows = 0          clears the contexts
+ *   n_rows = 1          ids[0] (n_ids[0] of them) applies to every utterance of later runs
+ *   any other n_rows    one context per utterance; a NULL row or n_ids[b] = 0 means no context for utterance b
+ * The ids are copied and kept until the next call; like the options, they are latched at the prefill.
+ * ASRB_ERR_INVALID here, with the previous contexts kept: an id outside [0, vocab), or a row longer than the session's
+ * max_context_ids (so any context on a session made by asrb_session_create).  ASRB_ERR_INVALID from asrb_prefill,
+ * asrb_transcribe_ids and asrb_transcribe_ingested, before any work or state change: a batch that is neither n_rows
+ * nor covered by n_rows = 1.
+ * Shared contexts: utterances of one call whose contexts are identical and non-empty have the same first P = L + 9
+ * prompt ids at the same positions, hence the same K/V.  The lowest-indexed one (the leader) computes those rows and
+ * writes their K/V into the others' caches; the others compute their rows from position P on.  Utterances without a
+ * context never share.  asrb_prefill's seq_lens_out stays S_b, context included.  A context lengthens every
+ * sequence's KV: a run that crosses the fused decode step's key limit continues on the per-phase kernels, counted in
+ * asrb_session_stats [2]. */
+ASRB_API int asrb_session_set_context(asrb_session* s, int n_rows, const int64_t* const* ids, const int32_t* n_ids);
+/* Counters of the last prefill: [0] prompt rows computed  [1] prompt rows taken from a leader instead of computed
+ * [2] KV bytes fanned out to followers; writes min(n, 3) values. */
+ASRB_API int asrb_last_prefill_stats(asrb_session* s, int64_t* out, int n);
 
 /* debug (ASRB_MEGA_DEBUG=1): clock64 timeline of the last fused decode step, CTA 0 then CTA G-1;
  * returns the number of slots per CTA (0 if disabled) */

@@ -5,11 +5,13 @@ best candidates of the step that selected it with their log-probabilities.
 `--temperature T[,T...]` samples with temperature T (a list is a fallback schedule), `--seed N` seeds the draw; both
 anywhere on the line, and `Temperature: x` reports the temperature of the kept attempt.
 `--beam-size N` (N in 1..6) decodes with beam search and prints an `N-best:` block of the ranked hypotheses with their
-scores; `--length-penalty A` (A in [0, 10]) scores them with ((5 + n) / 6) ** A instead of the length."""
+scores; `--length-penalty A` (A in [0, 10]) scores them with ((5 + n) / 6) ** A instead of the length.
+`--context TEXT` or `--context-file PATH` (UTF-8), anywhere on the line, places TEXT in the prompt's system turn to bias
+recognition towards its words (names, jargon, a keyword list)."""
 import sys
 
 USAGE = ("Usage: python -m qwen3_asr_rs_b200 <model_dir> <audio_file> [language] [--logprobs] [--top-logprobs N] "
-         "[--temperature T[,T...]] [--seed N] [--beam-size N] [--length-penalty A]")
+         "[--temperature T[,T...]] [--seed N] [--beam-size N] [--length-penalty A] [--context TEXT | --context-file PATH]")
 
 
 def parse_args(argv):
@@ -108,6 +110,25 @@ def split_beam(argv):
     return a[0], size, alpha
 
 
+def split_context(argv):
+    """Remove `--context TEXT` and `--context-file PATH` from argv -> (remaining argv, context text; None when absent),
+    or None when a value is missing, both are given, or the file cannot be read as UTF-8."""
+    c = _take_flag(argv, "--context")
+    if c is None:
+        return None
+    f = _take_flag(c[0], "--context-file")
+    if f is None or (c[1] is not None and f[1] is not None):
+        return None
+    text = c[1]
+    if f[1] is not None:
+        try:
+            with open(f[1], encoding="utf-8") as fh:
+                text = fh.read()
+        except (OSError, UnicodeDecodeError):
+            return None
+    return f[0], text
+
+
 def format_candidates(cands, decode) -> str:
     """One line of candidates: `'text' -0.0123` pairs, best first; `decode([id])` gives each candidate's text."""
     return "  ".join(f"{decode([i])!r} {lp:.4f}" for i, lp in cands)
@@ -115,7 +136,8 @@ def format_candidates(cands, decode) -> str:
 
 def main(argv=None) -> int:
     argv = list(sys.argv[1:] if argv is None else argv)
-    beam = split_beam(argv)
+    ctx = split_context(argv)
+    beam = split_beam(ctx[0]) if ctx is not None else None
     sampling = split_sampling(beam[0]) if beam is not None else None
     split = split_top_logprobs(sampling[0]) if sampling is not None else None
     args = parse_args(split[0]) if split is not None else None
@@ -137,6 +159,8 @@ def main(argv=None) -> int:
         kw = {} if temperature is None else dict(temperature=temperature, seed=seed)
         if beam_size > 1:
             kw.update(beam_size=beam_size, length_penalty=length_penalty)
+        if ctx[1]:
+            kw.update(context=ctx[1])
         r = eng.transcribe(audio, language, logprobs=logprobs, top_logprobs=top, **kw)
         decode = eng.tokenizer.decode if eng.tokenizer is not None else (lambda ids: " ".join(str(i) for i in ids))
     finally:

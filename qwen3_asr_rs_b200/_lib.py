@@ -17,6 +17,7 @@ SYMBOLS = [
     "asrb_prefill", "asrb_decode_step", "asrb_generate", "asrb_last_timings", "asrb_session_set_option",
     "asrb_debug_mega_timeline", "asrb_session_stats", "asrb_session_device_ids", "asrb_model_lossy_tensors", "asrb_ingest_pcm", "asrb_ingested_read", "asrb_transcribe_ingested",
     "asrb_last_logprobs", "asrb_last_top_logprobs", "asrb_last_nbest", "asrb_last_beam_stats",
+    "asrb_session_create_ex", "asrb_session_set_context", "asrb_last_prefill_stats",
 ]
 
 
@@ -84,6 +85,9 @@ def load_library() -> C.CDLL:
         "asrb_last_top_logprobs": [vp, C.c_int, C.c_int, P(i32), P(C.c_float), P(i32), P(C.c_float)],
         "asrb_last_nbest": [vp, C.c_int, C.c_int, P(i32), P(i32), P(C.c_float), P(C.c_float), P(i32)],
         "asrb_last_beam_stats": [vp, P(i64), C.c_int],
+        "asrb_session_create_ex": [vp, C.c_int, i64, C.c_int, C.c_int, C.c_int, P(vp)],
+        "asrb_session_set_context": [vp, C.c_int, P(P(i64)), P(i32)],
+        "asrb_last_prefill_stats": [vp, P(i64), C.c_int],
     }
     for name, args in sig.items():
         fn = getattr(lib, name)

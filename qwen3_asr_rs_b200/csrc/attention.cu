@@ -14,7 +14,9 @@ namespace asrb {
 
 static constexpr int QT = 16, KT = 64, ATT_THREADS = 128;
 
-template <int HD>
+// OFF: causal segments with a query position offset (p.seg_pos0): query row q is at position pos0 + q and sees keys
+// 0..pos0 + q of its slot
+template <int HD, bool OFF>
 __global__ void __launch_bounds__(ATT_THREADS) attn_kernel(AttnParams p) {
     extern __shared__ float sm[];
     float* Qs = sm;                          // [QT][HD+1]
@@ -23,6 +25,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_kernel(AttnParams p) {
     float* Ps = Vs + KT * HD;                // [QT][KT]
     const int seg = blockIdx.z, h = blockIdx.y;
     const int q0 = p.seg_q0[seg], len = p.seg_len[seg];
+    const int pos0 = OFF ? p.seg_pos0[seg] : 0;
     const int qt0 = blockIdx.x * QT;
     if (qt0 >= len) return;
     const int g = h / p.group;
@@ -51,7 +54,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_kernel(AttnParams p) {
 #pragma unroll
     for (int i = 0; i < HD / 8; ++i) acc[i] = 0.f;
     const int my_q = qt0 + qi;
-    const int kend = p.causal ? min(len, qt0 + QT) : len;
+    const int kend = p.causal ? pos0 + min(len, qt0 + QT) : len;
 
     for (int kt0 = 0; kt0 < kend; kt0 += KT) {
         __syncthreads();
@@ -73,7 +76,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_kernel(AttnParams p) {
 #pragma unroll 8
             for (int d = 0; d < HD; ++d) dot = fmaf(Qs[qi * (HD + 1) + d], Ks[kj * (HD + 1) + d], dot);
             int kidx = kt0 + kj;
-            bool valid = (my_q < len) && (kidx < len) && (!p.causal || kidx <= my_q);
+            bool valid = (my_q < len) && (kidx < pos0 + len) && (!p.causal || kidx <= pos0 + my_q);
             s[jj] = valid ? dot / inv_div : -INFINITY;
             tmax = fmaxf(tmax, s[jj]);
         }
@@ -123,16 +126,18 @@ void launch_attention(const AttnParams& p, int hd, cudaStream_t st) {
     // 0 = register-tiled fp32 (default), 1 = 3xTF32 tensor-core variant, 2 = the simple kernel below
     static const int which = [] { const char* e = getenv("ASRB_ATTN"); return !e ? 0 : std::string(e) == "tc" ? 1 : std::string(e) == "simt" ? 2 : 0; }();
     if (which == 0 && launch_attention_f32(p, hd, st)) return;
-    if (which == 1 && launch_attention_tc(p, hd, st)) return;
+    if (which == 1 && launch_attention_tc(p, hd, st)) return;     // declines a query position offset
+    ASRB_REQUIRE(!p.seg_pos0 || p.causal, ASRB_ERR_INVALID, "attention: a query position offset needs a causal segment");
     dim3 grid((p.max_len + QT - 1) / QT, p.nheads, p.nseg);
+    auto run = [&](auto kern, size_t smem) {
+        ASRB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   // per device: set on every launch
+        kern<<<grid, ATT_THREADS, smem, st>>>(p);
+    };
+    const bool off = p.seg_pos0 != nullptr;
     if (hd == 64) {
-        size_t smem = (QT * 65 + KT * 65 + KT * 64 + QT * KT) * sizeof(float);
-        ASRB_CUDA_CHECK(cudaFuncSetAttribute(attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   // per device: set on every launch
-        attn_kernel<64><<<grid, ATT_THREADS, smem, st>>>(p);
+        run(off ? attn_kernel<64, true> : attn_kernel<64, false>, (QT * 65 + KT * 65 + KT * 64 + QT * KT) * sizeof(float));
     } else if (hd == 128) {
-        size_t smem = (QT * 129 + KT * 129 + KT * 128 + QT * KT) * sizeof(float);
-        ASRB_CUDA_CHECK(cudaFuncSetAttribute(attn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   // per device: set on every launch
-        attn_kernel<128><<<grid, ATT_THREADS, smem, st>>>(p);
+        run(off ? attn_kernel<128, true> : attn_kernel<128, false>, (QT * 129 + KT * 129 + KT * 128 + QT * KT) * sizeof(float));
     } else {
         throw Error(ASRB_ERR_INVALID, "attention head_dim must be 64 or 128");
     }

@@ -22,7 +22,9 @@ namespace af32 {
 
 static constexpr int QT = 32, KT = 64, THREADS = 128, PS = KT + 4;
 
-template <int HD>
+// OFF: causal segments with a query position offset (p.seg_pos0): query row r is at position pos0 + r and sees keys
+// 0..pos0 + r.  A tile's key count still grows with its index, so the tile pairing below stays balanced.
+template <int HD, bool OFF>
 __global__ void __launch_bounds__(THREADS, 2) attn_f32_kernel(AttnParams p) {
     constexpr int NG = HD / 64;                 // column groups of 64 owned 4 columns at a time by the 16 tx lanes
     extern __shared__ __align__(16) float sm[];
@@ -32,6 +34,7 @@ __global__ void __launch_bounds__(THREADS, 2) attn_f32_kernel(AttnParams p) {
     float* Ps = Vs + KT * HD;                   // [QT][PS]
     const int seg = blockIdx.z, h = blockIdx.y;
     const int q0 = p.seg_q0[seg], len = p.seg_len[seg];
+    const int pos0 = OFF ? p.seg_pos0[seg] : 0;
     const int nqt = (len + QT - 1) / QT;
     const int gkv = h / p.group;
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -78,7 +81,7 @@ __global__ void __launch_bounds__(THREADS, 2) attn_f32_kernel(AttnParams p) {
     float m_run[4], l_run[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) { m_run[i] = -INFINITY; l_run[i] = 0.f; }
-    const int kend = p.causal ? min(len, qt0 + QT) : len;
+    const int kend = p.causal ? pos0 + min(len, qt0 + QT) : len;
     const float div = sqrtf((float)HD);
 
     for (int kt0 = 0; kt0 < kend; kt0 += KT) {
@@ -140,7 +143,7 @@ __global__ void __launch_bounds__(THREADS, 2) attn_f32_kernel(AttnParams p) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const int col = kt0 + tx * 4 + j;
-                const bool valid = (r < len) && (col < len) && (!p.causal || col <= r);
+                const bool valid = (r < len) && (col < pos0 + len) && (!p.causal || col <= pos0 + r);
                 const float v = valid ? s[i][j] / div : -INFINITY;
                 s[i][j] = v;
                 tmax = fmaxf(tmax, v);
@@ -207,13 +210,15 @@ bool launch_attention_f32(const AttnParams& p, int hd, cudaStream_t st) {
     if ((p.ldq % 4) || (p.ldk % 4) || (p.head_stride % 4) || (p.seg_stride % 4)) return false;
     const int nqt_max = (p.max_len + QT - 1) / QT;
     dim3 grid(p.causal ? (nqt_max + 1) / 2 : nqt_max, p.nheads, p.nseg);
-    if (hd == 64) {
-        ASRB_CUDA_CHECK(cudaFuncSetAttribute(attn_f32_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<64>()));   // per device: set on every launch
-        attn_f32_kernel<64><<<grid, THREADS, smem_bytes<64>(), st>>>(p);
-    } else if (hd == 128) {
-        ASRB_CUDA_CHECK(cudaFuncSetAttribute(attn_f32_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<128>()));   // per device: set on every launch
-        attn_f32_kernel<128><<<grid, THREADS, smem_bytes<128>(), st>>>(p);
-    } else return false;
+    auto run = [&](auto kern, size_t smem) {
+        ASRB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   // per device: set on every launch
+        kern<<<grid, THREADS, smem, st>>>(p);
+    };
+    const bool off = p.seg_pos0 != nullptr;
+    if (off && !p.causal) return false;
+    if (hd == 64) run(off ? attn_f32_kernel<64, true> : attn_f32_kernel<64, false>, smem_bytes<64>());
+    else if (hd == 128) run(off ? attn_f32_kernel<128, true> : attn_f32_kernel<128, false>, smem_bytes<128>());
+    else return false;
     ASRB_CUDA_CHECK(cudaGetLastError());
     return true;
 }

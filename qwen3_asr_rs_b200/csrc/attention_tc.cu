@@ -191,6 +191,7 @@ bool launch_attention_tc(const AttnParams& p, int hd, cudaStream_t st) {
     using namespace atc;
     if (p.nseg <= 0 || p.max_len <= 0) return true;
     if ((p.ldq % 4) || (p.ldk % 4) || (p.head_stride % 4) || (p.seg_stride % 4)) return false;
+    if (p.seg_pos0) return false;                // no query position offset here: the simple kernel takes it
     dim3 grid((p.max_len + QT - 1) / QT, p.nheads, p.nseg);
     if (hd == 64) {
         ASRB_CUDA_CHECK(cudaFuncSetAttribute(attn_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<64>()));   // per device: set on every launch

@@ -9,7 +9,7 @@ struct Session;
 void model_set_tensor(Model* m, const char* name, int dtype, const int64_t* shape, int ndim, const void* host);
 void model_finalize(Model* m);
 void model_load_dir(Ctx* ctx, const char* dir, Model** out);
-Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_lang, int max_new);
+Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_lang, int max_context, int max_new);
 void session_free(Session* s);
 void session_mel(Session* s, const float* const* samples, const int64_t* n_samples, int batch, int64_t* n_frames_out);
 void session_mel_read(Session* s, int b, float* out);
@@ -34,6 +34,8 @@ void session_device_ids(Session* s, const int32_t** ids, const int32_t** lens, i
 void session_last_nbest(Session* s, int max_new_tokens, int k, int32_t* ids_out, int32_t* lens_out, float* sum_out,
                         float* score_out, int32_t* eos_out);
 void session_last_beam_stats(Session* s, int64_t* out, int n);
+void session_set_context(Session* s, int n_rows, const int64_t* const* ids, const int32_t* n_ids);
+void session_last_prefill_stats(Session* s, int64_t* out, int n);
 int decode_mega_debug_timeline(long long* out, int cap);
 int decode_batch_debug_timeline(long long* out, int cap);
 }  // namespace asrb
@@ -140,13 +142,24 @@ int asrb_model_dims(const asrb_model* m, asrb_dims* out) { return guarded([&] { 
 int asrb_model_lossy_tensors(const asrb_model* m, int* count) { return guarded([&] { NONNULL(m); NONNULL(count); *count = m->m.lossy_count; }); }
 int asrb_model_free(asrb_model* m) { return guarded([&] { if (m) { cudaSetDevice(m->m.ctx->device); delete m; } }); }
 
-int asrb_session_create(asrb_model* m, int max_batch, int64_t max_samples, int max_lang_ids, int max_new_tokens, asrb_session** out) {
+int asrb_session_create_ex(asrb_model* m, int max_batch, int64_t max_samples, int max_lang_ids, int max_context_ids,
+                           int max_new_tokens, asrb_session** out) {
     return guarded([&] {
         NONNULL(m); NONNULL(out);
         asrb_session* s = new asrb_session();
-        try { s->s = session_create(&m->m, max_batch, max_samples, max_lang_ids, max_new_tokens); } catch (...) { delete s; throw; }
+        try { s->s = session_create(&m->m, max_batch, max_samples, max_lang_ids, max_context_ids, max_new_tokens); }
+        catch (...) { delete s; throw; }
         *out = s;
     });
+}
+int asrb_session_create(asrb_model* m, int max_batch, int64_t max_samples, int max_lang_ids, int max_new_tokens, asrb_session** out) {
+    return asrb_session_create_ex(m, max_batch, max_samples, max_lang_ids, 0, max_new_tokens, out);
+}
+int asrb_session_set_context(asrb_session* s, int n_rows, const int64_t* const* ids, const int32_t* n_ids) {
+    return guarded([&] { NONNULL(s); session_set_context(s->s, n_rows, ids, n_ids); });
+}
+int asrb_last_prefill_stats(asrb_session* s, int64_t* out, int n) {
+    return guarded([&] { NONNULL(s); NONNULL(out); session_last_prefill_stats(s->s, out, n); });
 }
 int asrb_session_free(asrb_session* s) { return guarded([&] { if (s) { session_free(s->s); delete s; } }); }
 

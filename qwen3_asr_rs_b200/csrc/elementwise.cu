@@ -136,15 +136,18 @@ void launch_embed_inject(const bf16* embed, int hidden, const int* d_ids, const 
 // Prefill: per-head RMSNorm on q,k (layers.rs:303-304) -> NeoX rotate-half RoPE (layers.rs:307-308,
 // 361-375; the three MRoPE streams are equal, inference.rs:259-266, so it is plain RoPE) -> K,V
 // written straight into the static KV cache (replaces the growing Tensor::cat of layers.rs:311-317).
+// FAN: a leader row at position pos < fan.P[seq] also writes its K,V into every follower slot of its shared context
+// (DESIGN.md 4.5), so a follower holds the prefix before this layer's attention reads it.
 // grid (rows, nq + 2*nkv); block = head_dim threads.
 // ---------------------------------------------------------------------------------------------
+template <bool FAN>
 __global__ void qk_norm_rope_kernel(const float* __restrict__ qkv, const int* __restrict__ row_seq,
                                     const int* __restrict__ row_pos, const float* __restrict__ qnorm,
                                     const float* __restrict__ knorm, float eps,
                                     const float* __restrict__ rope_cos, const float* __restrict__ rope_sin,
                                     int nq, int nkv, int hd, float* __restrict__ q_out,
                                     float* __restrict__ kcache, float* __restrict__ vcache,
-                                    size_t cache_seq_stride, int max_ctx) {
+                                    size_t cache_seq_stride, int max_ctx, FanOut fan) {
     extern __shared__ float sh[];     // [hd] + 32
     float* ys = sh;
     float* red = sh + hd;
@@ -153,9 +156,12 @@ __global__ void qk_norm_rope_kernel(const float* __restrict__ qkv, const int* __
     const int qkv_dim = (nq + 2 * nkv) * hd;
     const float x = qkv[row * qkv_dim + (size_t)head * hd + d];
     const int seq = row_seq[row], pos = row_pos[row];
+    const int nfan = FAN && pos < fan.P[seq] ? fan.n[seq] : 0;
+    const int* fslots = FAN ? fan.slots + fan.off[seq] : nullptr;
     if (head >= nq + nkv) {           // V: plain copy into the cache
-        int g = head - nq - nkv;
-        vcache[seq * cache_seq_stride + ((size_t)g * max_ctx + pos) * hd + d] = x;
+        const size_t o = ((size_t)(head - nq - nkv) * max_ctx + pos) * hd + d;
+        vcache[seq * cache_seq_stride + o] = x;
+        for (int j = 0; j < nfan; ++j) vcache[(size_t)fslots[j] * cache_seq_stride + o] = x;
         return;
     }
     const float* nw = head < nq ? qnorm : knorm;
@@ -168,17 +174,23 @@ __global__ void qk_norm_rope_kernel(const float* __restrict__ qkv, const int* __
     const float c = rope_cos[(size_t)pos * half + (d % half)], s = rope_sin[(size_t)pos * half + (d % half)];
     const float o = y * c + rot * s;
     if (head < nq) q_out[row * ((size_t)nq * hd) + (size_t)head * hd + d] = o;
-    else kcache[seq * cache_seq_stride + ((size_t)(head - nq) * max_ctx + pos) * hd + d] = o;
+    else {
+        const size_t ko = ((size_t)(head - nq) * max_ctx + pos) * hd + d;
+        kcache[seq * cache_seq_stride + ko] = o;
+        for (int j = 0; j < nfan; ++j) kcache[(size_t)fslots[j] * cache_seq_stride + ko] = o;
+    }
 }
 void launch_qk_norm_rope(const float* qkv, int rows, const int* d_row_seq, const int* d_row_pos,
                          const float* qnorm, const float* knorm, float eps, const float* rope_cos,
                          const float* rope_sin, int nq, int nkv, int hd, float* q_out, float* kcache,
-                         float* vcache, size_t cache_seq_stride, int max_ctx, cudaStream_t st) {
+                         float* vcache, size_t cache_seq_stride, int max_ctx, cudaStream_t st, const FanOut* fan) {
     if (rows <= 0) return;
     dim3 grid(rows, nq + 2 * nkv);
-    qk_norm_rope_kernel<<<grid, hd, (hd + 32) * sizeof(float), st>>>(qkv, d_row_seq, d_row_pos, qnorm, knorm, eps,
-                                                                     rope_cos, rope_sin, nq, nkv, hd, q_out,
-                                                                     kcache, vcache, cache_seq_stride, max_ctx);
+    const size_t smem = (hd + 32) * sizeof(float);
+    if (fan) qk_norm_rope_kernel<true><<<grid, hd, smem, st>>>(qkv, d_row_seq, d_row_pos, qnorm, knorm, eps, rope_cos, rope_sin,
+                                                               nq, nkv, hd, q_out, kcache, vcache, cache_seq_stride, max_ctx, *fan);
+    else qk_norm_rope_kernel<false><<<grid, hd, smem, st>>>(qkv, d_row_seq, d_row_pos, qnorm, knorm, eps, rope_cos, rope_sin,
+                                                            nq, nkv, hd, q_out, kcache, vcache, cache_seq_stride, max_ctx, FanOut{});
     ASRB_CUDA_CHECK(cudaGetLastError());
 }
 

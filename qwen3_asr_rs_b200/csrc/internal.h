@@ -149,11 +149,18 @@ void launch_rmsnorm_s3(const float* x, const float* w, int rows, int dim, float 
                        bf16* out_s3, size_t plane_stride, cudaStream_t st);
 void launch_embed_inject(const bf16* embed, int hidden, const int* d_ids, const int* d_audio_row,
                          const float* audio, int rows, float* out, cudaStream_t st);
+// prefill K/V fan-out of shared context prefixes (DESIGN.md 4.5), device arrays indexed by sequence
+struct FanOut {
+    const int* n;       // [nseq] follower slots of a leader (0: not a leader)
+    const int* off;     // [nseq] index of its first follower slot in `slots`
+    const int* P;       // [nseq] shared prefix length of a leader's group: positions 0..P-1 are fanned out
+    const int* slots;   // follower slots, grouped by leader
+};
 void launch_qk_norm_rope(const float* qkv, int rows, const int* d_row_seq, const int* d_row_pos,
                          const float* qnorm, const float* knorm, float eps,
                          const float* rope_cos, const float* rope_sin,
                          int nq, int nkv, int hd, float* q_out, float* kcache, float* vcache,
-                         size_t cache_seq_stride, int max_ctx, cudaStream_t st);
+                         size_t cache_seq_stride, int max_ctx, cudaStream_t st, const FanOut* fan = nullptr);
 // attention.cu
 struct AttnParams {
     const float* q; int ldq;            // q row r, head h at q + r*ldq + h*hd
@@ -165,6 +172,8 @@ struct AttnParams {
     int nseg, nheads, group;            // q head h uses kv head h / group
     int causal; int max_len;
     bf16* out_s3; size_t plane_stride; int ldo;
+    const int* seg_pos0;                // [nseg] or null (causal cache keys only): query row i of segment s is at position
+                                        // seg_pos0[s] + i and attends to keys 0..seg_pos0[s] + i of its slot (DESIGN.md 4.5)
 };
 void launch_attention(const AttnParams& p, int hd, cudaStream_t st);
 // decode.cu  (per-phase kernels, any batch <= 8) -- see decode_mega.cu for the fused step

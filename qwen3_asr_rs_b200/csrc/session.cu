@@ -30,7 +30,7 @@ static const int kAudioPad = 151676;
 struct Session {
     Model* m = nullptr;
     cudaStream_t st = nullptr;
-    int max_batch = 0, max_lang = 0, max_new = 0;
+    int max_batch = 0, max_lang = 0, max_new = 0, max_context = 0;
     int64_t max_samples = 0, max_npad = 0;
     int maxF = 0, maxC = 0, maxT = 0, maxS = 0, max_ctx = 0;
     int gemm_impl = GEMM_TC;
@@ -96,6 +96,11 @@ struct Session {
     bool nbest_valid = false;           // the last run was a beam run and has been finalized
     std::vector<float> nb_sum; std::vector<double> nb_score; std::vector<int> nb_eos, nb_n;   // [B][run_k], ranked
     int64_t beam_steps = 0, beam_reassigned = 0, beam_expand_bytes = 0, beam_reorder_bytes = 0;
+    // context biasing (asrb_session_set_context): ids placed in the system turn, latched at the prefill.  ctx_rows = 0:
+    // none; 1: ctx[0] for every utterance; else one row per utterance (empty: no context)
+    int ctx_rows = 0;
+    std::vector<std::vector<int>> ctx;
+    int64_t pf_rows = 0, pf_shared_rows = 0, pf_fan_bytes = 0;   // last prefill: rows computed / taken from a leader, KV bytes fanned out
     ~Session();
 };
 
@@ -122,9 +127,10 @@ template <typename T> static T* salloc(Session* s, size_t n, bool zero = false) 
     return p;
 }
 
-Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_lang, int max_new) {
+Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_lang, int max_context, int max_new) {
     ASRB_REQUIRE(m && m->finalized, ASRB_ERR_STATE, "model not finalized");
-    ASRB_REQUIRE(max_batch >= 1 && max_samples > 200 && max_new >= 1 && max_lang >= 0, ASRB_ERR_INVALID, "bad session capacity");
+    ASRB_REQUIRE(max_batch >= 1 && max_samples > 200 && max_new >= 1 && max_lang >= 0 && max_context >= 0, ASRB_ERR_INVALID,
+                 "bad session capacity");
     ASRB_CUDA_CHECK(cudaSetDevice(m->ctx->device));
     Session* s = new Session();
     try {
@@ -133,11 +139,12 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
         if (const char* e = getenv("ASRB_DECODE")) s->decode_mode = (std::string(e) == "phases") ? 0 : 1;
         if (const char* e = getenv("ASRB_PLANES")) s->nplanes = std::min(3, std::max(1, atoi(e)));
         s->m = m; s->max_batch = max_batch; s->max_samples = max_samples; s->max_lang = max_lang; s->max_new = max_new;
+        s->max_context = max_context;
         s->max_npad = ((max_samples + 159) / 160) * 160;
         s->maxF = (int)(s->max_npad / 160);
         s->maxC = (s->maxF + d.chunk_frames - 1) / d.chunk_frames;
         s->maxT = s->maxC * d.tok_per_chunk;
-        s->maxS = s->maxT + 15 + max_lang;
+        s->maxS = s->maxT + 15 + max_lang + max_context;
         s->max_ctx = s->maxS + max_new;
         ASRB_REQUIRE(s->max_ctx <= m->rope_max_pos, ASRB_ERR_INVALID, "context exceeds RoPE table");
         ASRB_CUDA_CHECK(cudaStreamCreateWithFlags(&s->st, cudaStreamNonBlocking));
@@ -151,7 +158,7 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
         s->d_maxkey = salloc<int>(s, Bm);
         const size_t totC = Bm * s->maxC, totT = Bm * s->maxT, totS = Bm * s->maxS;
         s->enc_int_cap = 2 * totC + totC * d.tok_per_chunk + 2 * (totC + Bm) + 16;
-        s->int_cap = s->enc_int_cap + 4 * totS + 8 * Bm + 16;
+        s->int_cap = s->enc_int_cap + 4 * totS + 16 * Bm + 16;   // rows, then per-utterance plan and fan-out arrays
         ASRB_CUDA_CHECK(cudaMallocHost(&s->h_int, s->int_cap * sizeof(int)));
         s->d_int = salloc<int>(s, s->int_cap);
         // encoder activations
@@ -474,46 +481,112 @@ static void ensure_sample_bufs(Session* s) {     // sampling with logprobs: the 
     }
 }
 
+// contexts: set by asrb_session_set_context, checked against the run's batch by every call that runs a prefill, before
+// any work
+static void check_context(const Session* s, int batch) {
+    ASRB_REQUIRE(s->ctx_rows <= 1 || s->ctx_rows == batch, ASRB_ERR_INVALID,
+                 "the contexts set with asrb_session_set_context have neither 1 row nor one row per utterance of this batch");
+}
+static const std::vector<int>& context_of(const Session* s, int b) {
+    static const std::vector<int> none;
+    return s->ctx_rows == 0 ? none : s->ctx[s->ctx_rows == 1 ? 0 : b];
+}
+
+void session_set_context(Session* s, int n_rows, const int64_t* const* ids, const int32_t* n_ids) {
+    ASRB_REQUIRE(n_rows >= 0, ASRB_ERR_INVALID, "n_rows must be >= 0");
+    ASRB_REQUIRE(n_rows == 0 || n_ids, ASRB_ERR_INVALID, "null pointer: n_ids");
+    std::vector<std::vector<int>> rows((size_t)n_rows);
+    for (int b = 0; b < n_rows; ++b) {
+        const int n = (ids && ids[b]) ? n_ids[b] : 0;
+        ASRB_REQUIRE(n >= 0 && n <= s->max_context, ASRB_ERR_INVALID, "context exceeds the session's max_context_ids");
+        rows[b].resize(n);
+        for (int i = 0; i < n; ++i) {
+            const int64_t id = ids[b][i];
+            ASRB_REQUIRE(id >= 0 && id < s->m->d.c.vocab_size, ASRB_ERR_INVALID, "context id out of vocabulary");
+            rows[b][i] = (int)id;
+        }
+    }
+    s->ctx = std::move(rows); s->ctx_rows = n_rows;
+}
+
+// [0] prompt rows computed  [1] prompt rows taken from a leader  [2] KV bytes fanned out to followers
+void session_last_prefill_stats(Session* s, int64_t* out, int n) {
+    const int64_t v[3] = {s->pf_rows, s->pf_shared_rows, s->pf_fan_bytes};
+    for (int i = 0; i < n && i < 3; ++i) out[i] = v[i];
+}
+
 void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, int64_t* seq_lens_out,
                      float* last_logits) {
     ASRB_REQUIRE(s->stage >= 2, ASRB_ERR_STATE, "prefill called before encode");
     check_sampling_options(s, s->B);
+    check_context(s, s->B);
     Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
     const int B = s->B; cudaStream_t st = s->st; const int np = s->nplanes;
-    ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
-    s->run_k = s->beam_k; s->run_alpha = s->length_penalty; s->nslots = B * s->run_k; s->nbest_valid = false;
-    if (s->run_k > 1) { ensure_beam_bufs(s); s->beam_steps = 0; }
-    s->S.assign(B, 0); s->srow0.assign(B, 0);
-    int totS = 0, maxlen = 0;
     for (int b = 0; b < B; ++b) {
         int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
         ASRB_REQUIRE(nl >= 0 && nl <= s->max_lang, ASRB_ERR_INVALID, "language prompt exceeds session capacity");
-        s->srow0[b] = totS; s->S[b] = 9 + s->T[b] + 6 + nl; totS += s->S[b]; maxlen = std::max(maxlen, s->S[b]);
+        for (int i = 0; i < nl; ++i)
+            ASRB_REQUIRE(lang_ids[b][i] >= 0 && lang_ids[b][i] < c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
+    }
+    ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
+    s->run_k = s->beam_k; s->run_alpha = s->length_penalty; s->nslots = B * s->run_k; s->nbest_valid = false;
+    if (s->run_k > 1) { ensure_beam_bufs(s); s->beam_steps = 0; }
+    // shared contexts: an utterance whose non-empty context equals that of an earlier leader follows it; its first
+    // P = L + 9 positions (head, context, end of the system turn, user turn up to the audio start) are the leader's
+    std::vector<int> lead((size_t)B, -1), skip((size_t)B, 0);
+    bool fan = false;
+    for (int b = 0; b < B; ++b) {
+        const std::vector<int>& cb = context_of(s, b);
+        if (cb.empty()) continue;
+        for (int a = 0; a < b; ++a)
+            if (lead[a] < 0 && context_of(s, a) == cb) { lead[b] = a; skip[b] = (int)cb.size() + 9; fan = true; break; }
+    }
+    s->S.assign(B, 0); s->srow0.assign(B, 0);
+    int totS = 0, maxlen = 0, maxrows = 0;     // totS: rows computed; maxlen: longest prompt; maxrows: most rows of one utterance
+    for (int b = 0; b < B; ++b) {
+        int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
+        const int L = (int)context_of(s, b).size();
+        s->srow0[b] = totS; s->S[b] = 9 + L + s->T[b] + 6 + nl; totS += s->S[b] - skip[b];
+        maxlen = std::max(maxlen, s->S[b]); maxrows = std::max(maxrows, s->S[b] - skip[b]);
     }
     s->totS = totS; s->maxlenS = maxlen;
     int* hi = s->h_int + s->enc_int_cap;      // separate region: the encoder plan upload may still be in flight
     int* di = s->d_int + s->enc_int_cap;
     int* ids = hi; int* arow = ids + totS; int* rseq = arow + totS; int* rpos = rseq + totS;
     int* sq0 = rpos + totS; int* slen = sq0 + B; int* lastrow = slen + B; int* pos0 = lastrow + B;
+    int* qpos0 = pos0 + B; int* fan_n = qpos0 + B; int* fan_off = fan_n + B; int* fan_P = fan_off + B; int* fan_slots = fan_P + B;
+    int64_t shared = 0;
+    std::vector<int> pid, parow;
     for (int b = 0; b < B; ++b) {
-        int r = s->srow0[b];
-        for (int i = 0; i < 9; ++i, ++r) { ids[r] = kPromptHead[i]; arow[r] = -1; }
-        for (int t = 0; t < s->T[b]; ++t, ++r) { ids[r] = kAudioPad; arow[r] = s->toff[b] + t; }
-        for (int i = 0; i < 6; ++i, ++r) { ids[r] = kPromptTail[i]; arow[r] = -1; }
-        int nl = s->S[b] - (9 + s->T[b] + 6);
-        for (int i = 0; i < nl; ++i, ++r) {
-            int64_t id = lang_ids[b][i];
-            ASRB_REQUIRE(id >= 0 && id < c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
-            ids[r] = (int)id; arow[r] = -1;
-        }
-        for (int i = 0; i < s->S[b]; ++i) { rseq[s->srow0[b] + i] = b; rpos[s->srow0[b] + i] = i; }   // build_position_ids :259-266
-        sq0[b] = s->srow0[b]; slen[b] = s->S[b]; lastrow[b] = s->srow0[b] + s->S[b] - 1; pos0[b] = s->S[b] - 1;
+        const std::vector<int>& cb = context_of(s, b);
+        pid.clear(); parow.clear();                                    // the whole prompt, position by position
+        for (int i = 0; i < 3; ++i) { pid.push_back(kPromptHead[i]); parow.push_back(-1); }
+        for (int id : cb) { pid.push_back(id); parow.push_back(-1); }
+        for (int i = 3; i < 9; ++i) { pid.push_back(kPromptHead[i]); parow.push_back(-1); }
+        for (int t = 0; t < s->T[b]; ++t) { pid.push_back(kAudioPad); parow.push_back(s->toff[b] + t); }
+        for (int i = 0; i < 6; ++i) { pid.push_back(kPromptTail[i]); parow.push_back(-1); }
+        for (int i = 0, nl = s->S[b] - (int)pid.size(); i < nl; ++i) { pid.push_back((int)lang_ids[b][i]); parow.push_back(-1); }
+        // rows from position skip[b] on (build_position_ids :259-266: position = index in the prompt)
+        for (int i = skip[b], r = s->srow0[b]; i < s->S[b]; ++i, ++r) { ids[r] = pid[i]; arow[r] = parow[i]; rseq[r] = b; rpos[r] = i; }
+        const int rows = s->S[b] - skip[b];
+        sq0[b] = s->srow0[b]; slen[b] = rows; lastrow[b] = s->srow0[b] + rows - 1; pos0[b] = s->S[b] - 1; qpos0[b] = skip[b];
+        shared += skip[b];
     }
-    const size_t nint = (size_t)(pos0 + B - hi);
+    int nf = 0;                                // followers grouped by leader, ascending
+    for (int a = 0; a < B; ++a) {
+        fan_off[a] = nf; fan_n[a] = 0; fan_P[a] = 0;
+        for (int b = a + 1; b < B; ++b)
+            if (lead[b] == a) { fan_slots[nf++] = b; ++fan_n[a]; fan_P[a] = skip[b]; }
+    }
+    const size_t nint = (size_t)(fan_slots + std::max(nf, 1) - hi);
     ASRB_REQUIRE(s->enc_int_cap + nint <= s->int_cap, ASRB_ERR_INVALID, "plan exceeds session capacity");
+    s->pf_rows = totS; s->pf_shared_rows = shared;
+    s->pf_fan_bytes = shared * 2LL * c.num_hidden_layers * c.num_key_value_heads * c.head_dim * (int64_t)sizeof(float);
     ASRB_CUDA_CHECK(cudaMemcpyAsync(di, hi, nint * sizeof(int), cudaMemcpyHostToDevice, st));
     s->d_ids = di; s->d_audio_row = di + (arow - hi); s->d_row_seq = di + (rseq - hi);
     s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
+    const FanOut fan_plan{di + (fan_n - hi), di + (fan_off - hi), di + (fan_P - hi), di + (fan_slots - hi)};
+    const int* d_qpos0 = fan ? di + (qpos0 - hi) : nullptr;   // no follower: the plan and kernels of a call without contexts
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_lastrow, di + (lastrow - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.pos, di + (pos0 - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
     ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.done, 0, B * sizeof(int), st));
@@ -551,11 +624,11 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
           launch_gemm(A, w.wqkv, d.qkv_dim, E, s->gemm_impl, st); }
         launch_qk_norm_rope(s->dqkv, totS, s->d_row_seq, s->d_row_pos, w.qnorm, w.knorm, eps, m.rope_cos, m.rope_sin,
                             c.num_attention_heads, c.num_key_value_heads, c.head_dim, s->qrot, kc, vc, s->cache_seq_stride,
-                            s->max_ctx, st);
+                            s->max_ctx, st, fan ? &fan_plan : nullptr);
         { AttnParams p{}; p.q = s->qrot; p.ldq = d.q_dim; p.k = kc; p.v = vc; p.seg_stride = s->cache_seq_stride;
           p.head_stride = (size_t)s->max_ctx * c.head_dim; p.ldk = c.head_dim; p.keys_in_rows = 0;
           p.seg_q0 = s->d_seq_q0; p.seg_len = s->d_seq_len; p.nseg = B; p.nheads = c.num_attention_heads;
-          p.group = c.num_attention_heads / c.num_key_value_heads; p.causal = 1; p.max_len = maxlen;
+          p.group = c.num_attention_heads / c.num_key_value_heads; p.causal = 1; p.max_len = maxrows; p.seg_pos0 = d_qpos0;
           p.out_s3 = s->dattn; p.plane_stride = s->dattn_ps; p.ldo = d.q_dim;
           launch_attention(p, c.head_dim, st); }
         { GemmA A = plainA(s->dattn, s->dattn_ps, totS, d.q_dim, np);
@@ -754,6 +827,7 @@ void session_transcribe_ids(Session* s, const float* const* samples, const int64
     ASRB_REQUIRE(ids_out && lens_out, ASRB_ERR_INVALID, "null output");
     if (samples == nullptr) batch = (int)s->ingested_n.size();      // asrb_transcribe_ingested
     check_sampling_options(s, batch);
+    check_context(s, batch);
     ASRB_REQUIRE(max_new_tokens >= 1 && max_new_tokens <= s->max_new, ASRB_ERR_INVALID, "max_new_tokens exceeds session capacity");
     cudaStream_t st = s->st;
     s->launches = 0; s->decode_steps = 0;

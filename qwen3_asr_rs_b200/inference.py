@@ -111,6 +111,29 @@ def rank_hypotheses(hyps: Sequence[Tuple[int, float]], length_penalty: Optional[
     return sorted(range(len(hyps)), key=lambda i: (-scores[i], i))
 
 
+def check_context_ids(context_ids, batch: int, vocab: int) -> Optional[List[Optional[List[int]]]]:
+    """The `context_ids` argument: None, or one entry per utterance, each None or a sequence of ints in [0, vocab) (an
+    empty one: no context), else ValueError.  Returns None or the entries as lists (None for no context)."""
+    if context_ids is None:
+        return None
+    if isinstance(context_ids, (str, bytes)) or not isinstance(context_ids, Sequence) or len(context_ids) != batch:
+        raise ValueError(f"context_ids must be None or one entry per utterance ({batch}), got {context_ids!r}")
+    out: List[Optional[List[int]]] = []
+    for c in context_ids:
+        if c is None:
+            out.append(None)
+            continue
+        if isinstance(c, (str, bytes)) or not isinstance(c, (Sequence, np.ndarray)):
+            raise ValueError(f"a context must be None or a sequence of token ids, got {c!r}")
+        ids = []
+        for i in c:
+            if isinstance(i, bool) or not isinstance(i, (int, np.integer)) or not 0 <= int(i) < vocab:
+                raise ValueError(f"context ids must be ints in [0, {vocab}), got {i!r}")
+            ids.append(int(i))
+        out.append(ids or None)
+    return out
+
+
 def temperature_option(t: float) -> str:
     """The session option string of temperature t (a decimal the library parses exactly back to t)."""
     return "0" if t == 0.0 else repr(float(t))
@@ -149,6 +172,11 @@ def temperature_fallback(run: Callable[[List[int], float], "TranscribeIds"], n: 
                 retry.append(b)
         pending = retry
     return kept, temps, runs
+
+
+def _max_len(rows) -> int:
+    """Length of the longest of `rows` (None entries count 0; None: 0)."""
+    return max((len(r) for r in rows if r is not None), default=0) if rows is not None else 0
 
 
 @dataclass
@@ -287,17 +315,19 @@ class AsrInference:
         return dict(zip(("decode_batch_steps", "decode_fused_steps", "decode_phase_steps", "gemm_simt_fallbacks",
                          "gemm_tc_launches"), [int(v) for v in out]))
 
-    def _ensure_session(self, batch: int, max_samples: int, max_lang: int, max_new: int):
+    def _ensure_session(self, batch: int, max_samples: int, max_lang: int, max_new: int, max_context: int = 0):
         cap = self._cap
-        if cap is None or batch > cap[0] or max_samples > cap[1] or max_lang > cap[2] or max_new > cap[3]:
+        if cap is None or batch > cap[0] or max_samples > cap[1] or max_lang > cap[2] or max_new > cap[3] \
+                or max_context > cap[4]:
             if self._session is not None:
                 _lib.check(self._lib.asrb_session_free(self._session))
                 self._session = None
             new_cap = (max(batch, cap[0] if cap else 0), max(max_samples, cap[1] if cap else 0),
-                       max(max_lang, cap[2] if cap else 0), max(max_new, cap[3] if cap else 0))
+                       max(max_lang, cap[2] if cap else 0), max(max_new, cap[3] if cap else 0),
+                       max(max_context, cap[4] if cap else 0))
             s = C.c_void_p()
-            _lib.check(self._lib.asrb_session_create(self._model, new_cap[0], new_cap[1], new_cap[2], new_cap[3],
-                                                     C.byref(s)))
+            _lib.check(self._lib.asrb_session_create_ex(self._model, new_cap[0], new_cap[1], new_cap[2], new_cap[4],
+                                                        new_cap[3], C.byref(s)))
             self._session, self._cap = s, new_cap
             for k, v in self._options.items():
                 _lib.check(self._lib.asrb_session_set_option(s, k.encode(), v.encode()))
@@ -326,6 +356,26 @@ class AsrInference:
                 lens.append(len(a))
                 mx = max(mx, len(a))
         return keep, (C.POINTER(C.c_int64) * batch)(*ptrs), (C.c_int32 * batch)(*lens), mx
+
+    # ---- context biasing (asrb_session_set_context) ------------------------------------------------------
+    def set_context(self, context_ids) -> None:
+        """asrb_session_set_context on the current session: None clears the contexts; else one entry per utterance of
+        the next runs (None or an empty sequence: no context), or a single entry for all of them.  For the stage-level
+        calls; transcribe_ids / transcribe_pcm / transcribe set their own contexts for the call."""
+        self._set_context(self._session, context_ids)
+
+    def _set_context(self, s, context_ids) -> None:
+        if not context_ids:
+            _lib.check(self._lib.asrb_session_set_context(s, 0, None, None))
+            return
+        keep, ptrs, lens, _ = self._pack_lang(context_ids, len(context_ids))
+        _lib.check(self._lib.asrb_session_set_context(s, len(context_ids), ptrs, lens))
+
+    def last_prefill_stats(self) -> Dict[str, int]:
+        """asrb_last_prefill_stats: rows computed, rows taken from a leader's shared context, KV bytes fanned out."""
+        out = (C.c_int64 * 3)()
+        _lib.check(self._lib.asrb_last_prefill_stats(self._session, out, 3))
+        return dict(zip(("rows_computed", "rows_shared", "fanout_kv_bytes"), [int(v) for v in out]))
 
     # ---- per-token log-probabilities (session option "logprobs") ----------------------------
     def _record_logprobs(self, s, on: bool) -> None:
@@ -497,7 +547,7 @@ class AsrInference:
                        max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0,
                        temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
                        logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
-                       length_penalty: Optional[float] = None) -> TranscribeIds:
+                       length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None) -> TranscribeIds:
         """transcribe() steps 2-8 for a batch: host f32 samples in, host token ids out (and, with `logprobs`, the
         log-probability of every id and of the ending EOS, from the kernels that selected them; with `top_logprobs` = k
         in 1..8, also the k best candidates of each of those steps, and the log-probabilities as with `logprobs`).
@@ -506,21 +556,25 @@ class AsrInference:
         (temperature_fallback) with the log-probability record on and `logprob_threshold` (None: off).
         `beam_size` K in 2..6 decodes every utterance with beam search (the session holds batch x K slots; `nbest`
         holds the K ranked hypotheses, `ids` the best) scored with `length_penalty` (None: sum / length); with a
-        schedule, only the attempts at t = 0 use it."""
+        schedule, only the attempts at t = 0 use it.  `context_ids`: None, or per utterance None or the token ids of
+        its context, placed in the prompt's system turn; utterances with identical contexts share its prefill."""
+        ctx = check_context_ids(context_ids, len(clips), self.config.text.vocab_size)
+
         def once(idx, lp, k, t, beam):
             sub = clips if len(idx) == len(clips) else [clips[i] for i in idx]
             lang = None if language_ids is None else [language_ids[i] for i in idx]
-            return self._ids_once(sub, lang, max_new_tokens, lp, k, t, seed, beam)
+            return self._ids_once(sub, lang, max_new_tokens, lp, k, t, seed, beam,
+                                  None if ctx is None else [ctx[i] for i in idx])
         return self._sampled(len(clips), once, temperature, seed, logprob_threshold, logprobs, top_logprobs,
                              beam_size, length_penalty)
 
     def _ids_once(self, clips, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
-                  temperature: Optional[float], seed: int, beam=None) -> TranscribeIds:
+                  temperature: Optional[float], seed: int, beam=None, context_ids=None) -> TranscribeIds:
         B = len(clips)
         K = beam[0] if beam else 1
         arrs, ptrs, lens = self._pack_samples(clips)
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
-        s = self._ensure_session(B * K, max(a.shape[0] for a in arrs), mx, max_new_tokens)
+        s = self._ensure_session(B * K, max(a.shape[0] for a in arrs), mx, max_new_tokens, _max_len(context_ids))
         ids = np.zeros((B, max_new_tokens), dtype=np.int32)
         n = np.zeros(B, dtype=np.int32)
         if logprobs:
@@ -531,11 +585,15 @@ class AsrInference:
         try:
             undo = self._set_sampling(s, temperature, seed)
             undo += self._set_beam(s, K, beam[1] if beam else None)
+            if context_ids is not None:
+                self._set_context(s, context_ids)
             _lib.check(self._lib.asrb_transcribe_ids(
                 s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
                 ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
             return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs, K)
         finally:
+            if context_ids is not None:
+                self._set_context(s, None)
             self._restore(s, undo)
             if logprobs:
                 self._record_logprobs(s, False)
@@ -545,14 +603,15 @@ class AsrInference:
     # ---- GPU-side audio ingest (step 1, src/audio.rs:162-245) -------------------------------------------
     _PCM_FMT = {"int16": 0, "float32": 1, "int32": 2}
 
-    def _ingest(self, pcms: Sequence, rates: Sequence[int], max_lang: int, max_new: int, slots: int = 0):
+    def _ingest(self, pcms: Sequence, rates: Sequence[int], max_lang: int, max_new: int, slots: int = 0,
+                max_context: int = 0):
         B = len(pcms)
         arrs = [np.ascontiguousarray(a if a.ndim == 2 else a.reshape(-1, 1)) for a in pcms]
         for a in arrs:
             if a.dtype.name not in self._PCM_FMT:
                 raise ValueError(f"PCM dtype must be int16 / int32 / float32, got {a.dtype}")
         n_out = [-(-a.shape[0] * MEL_SAMPLE_RATE // int(r)) for a, r in zip(arrs, rates)]
-        s = self._ensure_session(max(B, slots), max(n_out), max_lang, max_new)
+        s = self._ensure_session(max(B, slots), max(n_out), max_lang, max_new, max_context)
         ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in arrs])
         frames = (C.c_int64 * B)(*[a.shape[0] for a in arrs])
         chans = (C.c_int32 * B)(*[a.shape[1] for a in arrs])
@@ -576,23 +635,26 @@ class AsrInference:
                        max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0,
                        temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
                        logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
-                       length_penalty: Optional[float] = None) -> TranscribeIds:
+                       length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None) -> TranscribeIds:
         """transcribe() steps 1-8 for a batch with step 1 on the GPU: raw PCM in, token ids out (`logprobs`,
-        `top_logprobs`, `temperature`, `seed`, `logprob_threshold`, `beam_size`, `length_penalty`: as in
-        transcribe_ids)."""
+        `top_logprobs`, `temperature`, `seed`, `logprob_threshold`, `beam_size`, `length_penalty`, `context_ids`: as
+        in transcribe_ids)."""
+        ctx = check_context_ids(context_ids, len(pcms), self.config.text.vocab_size)
+
         def once(idx, lp, k, t, beam):
             sel = (lambda xs: xs if len(idx) == len(pcms) else [xs[i] for i in idx])
             lang = None if language_ids is None else sel(language_ids)
-            return self._pcm_once(sel(pcms), sel(rates), lang, max_new_tokens, lp, k, t, seed, beam)
+            return self._pcm_once(sel(pcms), sel(rates), lang, max_new_tokens, lp, k, t, seed, beam,
+                                  None if ctx is None else sel(ctx))
         return self._sampled(len(pcms), once, temperature, seed, logprob_threshold, logprobs, top_logprobs,
                              beam_size, length_penalty)
 
     def _pcm_once(self, pcms, rates, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
-                  temperature: Optional[float], seed: int, beam=None) -> TranscribeIds:
+                  temperature: Optional[float], seed: int, beam=None, context_ids=None) -> TranscribeIds:
         B = len(pcms)
         K = beam[0] if beam else 1
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
-        s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens, slots=B * K)
+        s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens, slots=B * K, max_context=_max_len(context_ids))
         ids = np.zeros((B, max_new_tokens), dtype=np.int32)
         n = np.zeros(B, dtype=np.int32)
         if logprobs:
@@ -603,10 +665,14 @@ class AsrInference:
         try:
             undo = self._set_sampling(s, temperature, seed)
             undo += self._set_beam(s, K, beam[1] if beam else None)
+            if context_ids is not None:
+                self._set_context(s, context_ids)
             _lib.check(self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens),
                                                           ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
             return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs, K)
         finally:
+            if context_ids is not None:
+                self._set_context(s, None)
             self._restore(s, undo)
             if logprobs:
                 self._record_logprobs(s, False)
@@ -617,18 +683,20 @@ class AsrInference:
                    max_new_tokens: int = MAX_NEW_TOKENS, gpu_ingest: bool = True, logprobs: bool = False,
                    top_logprobs: int = 0, temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
                    logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
-                   length_penalty: Optional[float] = None) -> TranscribeResult:
+                   length_penalty: Optional[float] = None, context: Optional[str] = None) -> TranscribeResult:
         """AsrInference::transcribe (inference.rs:89-213): step 1 (WAV payload -> mono 16 kHz; on the GPU by default,
         `gpu_ingest=False` = the host loader) -> steps 2-8 on the GPU -> step 9 (detokenise + parse, host; needs
         tokenizer.json, else raw_output is the id list as text).  `logprobs`: also fill token_logprobs / avg_logprob;
         `top_logprobs` = k in 1..8: also fill top_logprobs (and token_logprobs / avg_logprob); `temperature`, `seed`,
         `logprob_threshold`, `beam_size`, `length_penalty`: as in transcribe_ids, and `temperature` of the result is that
-        of the kept attempt; `nbest` holds the beam's hypotheses as (text, score)."""
-        sampling = dict(temperature=temperature, seed=seed, logprob_threshold=logprob_threshold, beam_size=beam_size,
-                        length_penalty=length_penalty)
+        of the kept attempt; `nbest` holds the beam's hypotheses as (text, score).  `context`: text placed in the prompt's
+        system turn to bias recognition (keywords, names, related text; needs tokenizer.json; "" = none)."""
         from .audio import load_wav, read_wav_pcm
-        from .text import language_prompt_ids, parse_asr_output
+        from .text import context_prompt_ids, language_prompt_ids, parse_asr_output
         lang_ids = language_prompt_ids(self.tokenizer, language)
+        ctx_ids = context_prompt_ids(self.tokenizer, context)
+        sampling = dict(temperature=temperature, seed=seed, logprob_threshold=logprob_threshold, beam_size=beam_size,
+                        length_penalty=length_penalty, context_ids=[ctx_ids] if ctx_ids else None)
         if gpu_ingest:
             pcm, rate = read_wav_pcm(audio_path)
             r = self.transcribe_pcm([pcm], [rate], language_ids=[lang_ids] if lang_ids is not None else None,
@@ -657,11 +725,12 @@ class AsrInference:
         return res
 
     # ---- stage-level calls (the calls transcribe() makes; used by the parity tests) ----
-    def mel(self, clips: Sequence[np.ndarray], max_new_tokens: int = 64, max_lang: int = 16) -> List[np.ndarray]:
+    def mel(self, clips: Sequence[np.ndarray], max_new_tokens: int = 64, max_lang: int = 16,
+            max_context: int = 0) -> List[np.ndarray]:
         """WhisperFeatureExtractor::extract (mel.rs:49-96) -> [128, F] per utterance."""
         B = len(clips)
         arrs, ptrs, lens = self._pack_samples(clips)
-        s = self._ensure_session(B, max(a.shape[0] for a in arrs), max_lang, max_new_tokens)
+        s = self._ensure_session(B, max(a.shape[0] for a in arrs), max_lang, max_new_tokens, max_context)
         frames = (C.c_int64 * B)()
         _lib.check(self._lib.asrb_mel(s, ptrs, lens, B, frames))
         out = []

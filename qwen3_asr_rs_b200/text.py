@@ -64,3 +64,12 @@ def language_prompt_ids(tokenizer: Optional[AsrTokenizer], language: Optional[st
     if tokenizer is None:
         raise ValueError("forcing a language needs tokenizer.json (to encode the prompt suffix)")
     return tokenizer.encode(f"language {capitalize_first(language)}")
+
+
+def context_prompt_ids(tokenizer: Optional[AsrTokenizer], context: Optional[str]) -> Optional[List[int]]:
+    """ids of the context text placed in the prompt's system turn (None or "": no context)."""
+    if not context:
+        return None
+    if tokenizer is None:
+        raise ValueError("a context needs tokenizer.json (to encode the text)")
+    return tokenizer.encode(context)

@@ -46,7 +46,10 @@ extern "C" {
     pub fn asrb_model_free(m: *mut asrb_model) -> c_int;
 
     pub fn asrb_session_create(m: *mut asrb_model, max_batch: c_int, max_samples: i64, max_lang_ids: c_int, max_new_tokens: c_int, out: *mut *mut asrb_session) -> c_int;
+    pub fn asrb_session_create_ex(m: *mut asrb_model, max_batch: c_int, max_samples: i64, max_lang_ids: c_int, max_context_ids: c_int, max_new_tokens: c_int, out: *mut *mut asrb_session) -> c_int;
     pub fn asrb_session_free(s: *mut asrb_session) -> c_int;
+    pub fn asrb_session_set_context(s: *mut asrb_session, n_rows: c_int, ids: *const *const i64, n_ids: *const i32) -> c_int;
+    pub fn asrb_last_prefill_stats(s: *mut asrb_session, out: *mut i64, n: c_int) -> c_int;
 
     pub fn asrb_transcribe_ids(s: *mut asrb_session, samples: *const *const f32, n_samples: *const i64, batch: c_int, lang_ids: *const *const i64, n_lang_ids: *const i32, max_new_tokens: c_int, ids_out: *mut i32, lens_out: *mut i32) -> c_int;
 

@@ -25,7 +25,7 @@ impl Drop for Session { fn drop(&mut self) { unsafe { ffi::asrb_session_free(sel
 /// arbitrary-length audio; a session sized for the worst case up front would pin ~1 GB of scratch per minute of audio).
 /// Field order = drop order: session before model before context.
 pub struct B200Engine {
-    session: std::cell::RefCell<Option<(Session, usize, usize)>>,   // (handle, capacity in samples, slots)
+    session: std::cell::RefCell<Option<(Session, usize, usize, usize)>>,   // (handle, capacity in samples, slots, context ids)
     model: Model,
     _ctx: Ctx,
     max_new_tokens: usize,
@@ -54,17 +54,27 @@ impl B200Engine {
 
     /// Session with room for `n_samples` and `slots` decode rows (a beam search of K needs K); neither shrinks.
     fn session_for_slots(&self, n_samples: usize, slots: usize) -> Result<*mut ffi::asrb_session> {
+        self.session_for_context(n_samples, slots, 0)
+    }
+
+    /// Session with room for `n_samples`, `slots` decode rows and `n_context` context ids; none of them shrinks, and
+    /// the context capacity grows in steps of 256 ids.
+    fn session_for_context(&self, n_samples: usize, slots: usize, n_context: usize) -> Result<*mut ffi::asrb_session> {
         let mut slot = self.session.borrow_mut();
-        let mut rows = slots;
-        if let Some((s, cap, have)) = slot.as_ref() {
-            if *cap >= n_samples && *have >= slots { return Ok(s.0); }
+        let (mut rows, mut ctx_cap) = (slots, (n_context + 255) / 256 * 256);
+        if let Some((s, cap, have, have_ctx)) = slot.as_ref() {
+            if *cap >= n_samples && *have >= slots && *have_ctx >= n_context { return Ok(s.0); }
             rows = rows.max(*have);
+            ctx_cap = ctx_cap.max(*have_ctx);
         }
         *slot = None;
         let cap = ((n_samples + 479_999) / 480_000).max(1) * 480_000;
         let mut session = ptr::null_mut();
-        check(unsafe { ffi::asrb_session_create(self.model.0, rows as i32, cap as i64, 16, self.max_new_tokens as i32, &mut session) })?;
-        *slot = Some((Session(session), cap, rows));
+        check(unsafe {
+            ffi::asrb_session_create_ex(self.model.0, rows as i32, cap as i64, 16, ctx_cap as i32, self.max_new_tokens as i32,
+                                        &mut session)
+        })?;
+        *slot = Some((Session(session), cap, rows, ctx_cap));
         Ok(session)
     }
 
@@ -164,6 +174,19 @@ impl B200Engine {
         let run = set.and_then(|_| self.transcribe_ids(samples, lang_ids));
         check(unsafe { ffi::asrb_session_set_option(session, tkey.as_ptr(), zero.as_ptr()) })?;
         check(unsafe { ffi::asrb_session_set_option(session, skey.as_ptr(), zero.as_ptr()) })?;
+        run
+    }
+
+    /// `transcribe_ids` with context biasing: `context_ids` (the tokenizer's ids of a keyword list, names or related
+    /// text) become the content of the prompt's system turn (`asrb_session_set_context`).  An empty slice is the plain
+    /// prompt.  The context is cleared again after the call.
+    pub fn transcribe_ids_with_context(&self, samples: &[f32], lang_ids: Option<&[i64]>, context_ids: &[i64]) -> Result<Vec<i64>> {
+        let session = self.session_for_context(samples.len(), 1, context_ids.len())?;
+        let cp = [context_ids.as_ptr()];
+        let cl = [context_ids.len() as i32];
+        let run = check(unsafe { ffi::asrb_session_set_context(session, 1, cp.as_ptr(), cl.as_ptr()) })
+            .and_then(|_| self.transcribe_ids(samples, lang_ids));
+        check(unsafe { ffi::asrb_session_set_context(session, 0, ptr::null(), ptr::null()) })?;
         run
     }
 
