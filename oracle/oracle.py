@@ -160,18 +160,19 @@ def mel_filterbank(num_mels: int = 128, n_fft: int = N_FFT, sample_rate: int = S
 _FB_CACHE: Dict[Tuple[int, int, int], torch.Tensor] = {}
 
 
-def extract_mel(samples: np.ndarray, num_mels: int = 128) -> torch.Tensor:
-    """f32 samples @16 kHz -> log-mel [num_mels, F], F = ceil(n/160).  src/mel.rs:49-96."""
+def extract_mel(samples: np.ndarray, num_mels: int = 128, dtype: torch.dtype = torch.float32) -> torch.Tensor:
+    """f32 samples @16 kHz -> log-mel [num_mels, F], F = ceil(n/160).  src/mel.rs:49-96.
+    ``dtype=torch.float64``: the f32 samples and the (f32) filterbank widened exactly, every operation in f64."""
     key = (num_mels, N_FFT, SAMPLE_RATE)
     if key not in _FB_CACHE:
         _FB_CACHE[key] = torch.from_numpy(mel_filterbank(num_mels))
-    fb = _FB_CACHE[key]
+    fb = _FB_CACHE[key].to(dtype)
     x = np.asarray(samples, dtype=np.float32)
     padded_len = ((len(x) + HOP - 1) // HOP) * HOP                        # :51
     xp = np.zeros(padded_len, dtype=np.float32)
     xp[: len(x)] = x
-    wave = torch.from_numpy(xp)
-    window = torch.hann_window(N_FFT, dtype=torch.float32)                # periodic (tensor.rs:215)
+    wave = torch.from_numpy(xp).to(dtype)
+    window = torch.hann_window(N_FFT, dtype=dtype)                        # periodic (tensor.rs:215)
     pad = N_FFT // 2
     wave = torch.nn.functional.pad(wave[None, None, :], (pad, pad), mode="reflect")[0, 0]   # :63-65
     stft = torch.stft(wave, N_FFT, hop_length=HOP, win_length=N_FFT, window=window,
@@ -252,26 +253,29 @@ def build_dim_map(sections: Sequence[int], total: int, interleaved: bool) -> Lis
 
 
 def mrope_cos_sin(position_ids: Sequence[Sequence[int]], head_dim: int, theta: float,
-                  sections: Sequence[int], interleaved: bool) -> Tuple[torch.Tensor, torch.Tensor]:
-    """Host f64 table, duplicated halves, -> f32 [S, head_dim].  src/layers.rs:471-522."""
+                  sections: Sequence[int], interleaved: bool,
+                  dtype: torch.dtype = torch.float32) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Host f64 table, duplicated halves, -> [S, head_dim] in ``dtype`` (f32: rounded as the reference does).
+    src/layers.rs:471-522."""
     half = head_dim // 2
     inv_freq = np.array([1.0 / (theta ** (2.0 * i / head_dim)) for i in range(half)], dtype=np.float64)
     dim_map = build_dim_map(sections, half, interleaved)
     pos = np.asarray(position_ids, dtype=np.float64)                      # [3, S]
     sel = pos[np.asarray(dim_map), :].T                                    # [S, half]
     ang = sel * inv_freq[None, :]
-    c, s = np.cos(ang).astype(np.float32), np.sin(ang).astype(np.float32)
+    npdt = torch.empty(0, dtype=dtype).numpy().dtype
+    c, s = np.cos(ang).astype(npdt), np.sin(ang).astype(npdt)
     return (torch.from_numpy(np.concatenate([c, c], axis=1)),
             torch.from_numpy(np.concatenate([s, s], axis=1)))
 
 
-def sinusoid_table(max_len: int, dim: int) -> torch.Tensor:
-    """src/audio_encoder.rs:283-301 (f64 host, sin || cos)."""
+def sinusoid_table(max_len: int, dim: int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
+    """src/audio_encoder.rs:283-301 (f64 host, sin || cos), returned in ``dtype``."""
     half = dim // 2
     inc = math.log(10000.0) / (half - 1)
     inv = np.exp(-np.arange(half, dtype=np.float64) * inc)
     ang = np.arange(max_len, dtype=np.float64)[:, None] * inv[None, :]
-    return torch.from_numpy(np.concatenate([np.sin(ang), np.cos(ang)], axis=1).astype(np.float32))
+    return torch.from_numpy(np.concatenate([np.sin(ang), np.cos(ang)], axis=1)).to(dtype)
 
 
 def feat_extract_output_length(frames: int) -> int:
@@ -283,12 +287,14 @@ def feat_extract_output_length(frames: int) -> int:
 # Model
 # --------------------------------------------------------------------------------------
 class OracleModel:
-    """Holds fp32 weights under the HF names the reference loads (SURVEY.md section 8c)."""
+    """Holds fp32 weights under the HF names the reference loads (SURVEY.md section 8c).  ``dtype=torch.float64``
+    widens the (bf16) weights exactly and runs every stage in f64: the high-precision reference of the same model."""
 
-    def __init__(self, cfg: AsrCfg, weights: Dict[str, torch.Tensor]):
+    def __init__(self, cfg: AsrCfg, weights: Dict[str, torch.Tensor], dtype: torch.dtype = torch.float32):
         self.cfg = cfg
-        self.w = {k: v.to(torch.float32) for k, v in weights.items()}     # weights.rs:74-89
-        self.pos_emb = sinusoid_table(cfg.audio.max_source_positions, cfg.audio.d_model)
+        self.dtype = dtype
+        self.w = {k: v.to(dtype) for k, v in weights.items()}             # weights.rs:74-89
+        self.pos_emb = sinusoid_table(cfg.audio.max_source_positions, cfg.audio.d_model, dtype)
 
     # ---- audio encoder (src/audio_encoder.rs:79-169) ----
     def chunk_plan(self, num_frames: int) -> Tuple[int, List[int]]:
@@ -305,7 +311,7 @@ class OracleModel:
         cpw = self.cfg.audio.n_window_infer // cs
         if cpw == 0 or len(chunk_tokens) <= cpw:
             return None
-        mask = torch.full((1, 1, total, total), float("-inf"), dtype=torch.float32)
+        mask = torch.full((1, 1, total, total), float("-inf"), dtype=self.dtype)
         off = 0
         for w0 in range(0, len(chunk_tokens), cpw):
             n = sum(chunk_tokens[w0:w0 + cpw])
@@ -318,7 +324,7 @@ class OracleModel:
         F_ = mel.shape[1]
         cs, valid = self.chunk_plan(F_)
         C = len(valid)
-        padded = torch.zeros(mel.shape[0], C * cs, dtype=torch.float32)
+        padded = torch.zeros(mel.shape[0], C * cs, dtype=self.dtype)
         padded[:, :F_] = mel                                              # :105-121 zero-pad tail
         batched = padded.reshape(mel.shape[0], C, cs).permute(1, 0, 2).unsqueeze(1)   # [C,1,128,cs]
         x = batched
@@ -407,15 +413,17 @@ class OracleModel:
             return self.w["thinker.model.embed_tokens.weight"]
         return self.w["thinker.lm_head.weight"]
 
-    def decoder_forward(self, hidden, cos, sin, cache, mask, last_only: bool = False):
-        """src/text_decoder.rs:94-113.  ``last_only`` skips the (unused) lm_head rows -- the
-        reference computes all S rows; the values of the last row are identical either way."""
+    def decoder_forward(self, hidden, cos, sin, cache, mask, last_only: bool = False, from_row: int = 0):
+        """src/text_decoder.rs:94-113.  ``last_only`` / ``from_row`` skip (unused) lm_head rows -- the
+        reference computes all S rows; the values of the rows kept are identical either way."""
         x = hidden
         for i in range(self.cfg.text.num_hidden_layers):
             x = self.decoder_layer(x, i, cos, sin, cache, mask)
         x = rms_norm(x, self.w["thinker.model.norm.weight"], self.cfg.text.rms_norm_eps)
         if last_only:
             x = x[:, -1:, :]
+        elif from_row:
+            x = x[:, from_row:, :]
         return x.matmul(self.lm_head_weight().t())
 
     def embed(self, ids: Sequence[int]) -> torch.Tensor:
@@ -423,9 +431,9 @@ class OracleModel:
                                              self.w["thinker.model.embed_tokens.weight"])
 
 
-def causal_mask(seq_len: int, past: int) -> torch.Tensor:
+def causal_mask(seq_len: int, past: int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
     """full(-inf).triu(past+1) -> [1,1,S,past+S].  src/text_decoder.rs:121-131."""
-    m = torch.full((seq_len, past + seq_len), float("-inf"), dtype=torch.float32)
+    m = torch.full((seq_len, past + seq_len), float("-inf"), dtype=dtype)
     return m.triu(past + 1)[None, None]
 
 
@@ -455,9 +463,9 @@ def transcribe_ids(model: OracleModel, samples: np.ndarray, language_ids: Option
                    lm_head_all_rows: bool = True) -> OracleResult:
     """transcribe() steps 2-8, src/inference.rs:94-200: samples -> generated token ids."""
     import time
-    t, tm = model.cfg.text, {}
+    t, tm, dt = model.cfg.text, {}, model.dtype
     t0 = time.perf_counter()
-    mel = extract_mel(samples, model.cfg.audio.num_mel_bins)              # step 2
+    mel = extract_mel(samples, model.cfg.audio.num_mel_bins, dt)          # step 2
     tm["mel"] = time.perf_counter() - t0
     t0 = time.perf_counter()
     audio = model.encode(mel)                                             # step 3
@@ -468,9 +476,9 @@ def transcribe_ids(model: OracleModel, samples: np.ndarray, language_ids: Option
     hidden = model.embed(ids).unsqueeze(0)                                # step 5
     hidden[0, a0:a0 + audio.shape[0], :] = audio                          # == T slice_scatter calls (:115-124)
     pos = list(range(S))                                                  # build_position_ids :259-266
-    cos, sin = mrope_cos_sin([pos, pos, pos], t.head_dim, t.rope_theta, t.mrope_section, t.mrope_interleaved)
+    cos, sin = mrope_cos_sin([pos, pos, pos], t.head_dim, t.rope_theta, t.mrope_section, t.mrope_interleaved, dt)
     cache = [None] * t.num_hidden_layers
-    logits = model.decoder_forward(hidden, cos, sin, cache, causal_mask(S, 0),
+    logits = model.decoder_forward(hidden, cos, sin, cache, causal_mask(S, 0, dt),
                                    last_only=not lm_head_all_rows)         # step 7
     nxt = logits[:, -1, :]
     tm["prefill"] = time.perf_counter() - t0
@@ -485,11 +493,32 @@ def transcribe_ids(model: OracleModel, samples: np.ndarray, language_ids: Option
             break
         out.append(tok)
         h = model.embed([tok]).unsqueeze(0)
-        c1, s1 = mrope_cos_sin([[cur]] * 3, t.head_dim, t.rope_theta, t.mrope_section, t.mrope_interleaved)
+        c1, s1 = mrope_cos_sin([[cur]] * 3, t.head_dim, t.rope_theta, t.mrope_section, t.mrope_interleaved, dt)
         past = cache[0][0].shape[2]
-        nxt = model.decoder_forward(h, c1, s1, cache, causal_mask(1, past))[:, 0, :]
+        nxt = model.decoder_forward(h, c1, s1, cache, causal_mask(1, past, dt))[:, 0, :]
         if keep_logits:
             step_logits.append(nxt[0].clone())
         cur += 1
     tm["decode"] = time.perf_counter() - t0
     return OracleResult(out, mel, audio, prefill_logits, step_logits, tm)
+
+
+def score_ids(model: OracleModel, samples: np.ndarray, ids: Sequence[int],
+              language_ids: Optional[Sequence[int]] = None) -> torch.Tensor:
+    """Teacher-forced scoring: ONE causal forward over prompt + ``ids`` (positions 0..S + len(ids) - 1), in the
+    model's dtype -> logits [len(ids) + 1, V].  Row i is what the greedy loop of transcribe_ids computes before
+    choosing ids[i] (row 0: the prefill's last row); the last row follows the last id.  This makes the reference a
+    function of any implementation's own ids, so comparisons do not depend on it reproducing the oracle's."""
+    t, dt = model.cfg.text, model.dtype
+    mel = extract_mel(samples, model.cfg.audio.num_mel_bins, dt)
+    audio = model.encode(mel)
+    prompt, a0 = build_prompt(audio.shape[0], language_ids)
+    S = len(prompt)
+    toks = list(prompt) + [int(i) for i in ids]
+    hidden = model.embed(toks).unsqueeze(0)
+    hidden[0, a0:a0 + audio.shape[0], :] = audio
+    pos = list(range(len(toks)))
+    cos, sin = mrope_cos_sin([pos, pos, pos], t.head_dim, t.rope_theta, t.mrope_section, t.mrope_interleaved, dt)
+    logits = model.decoder_forward(hidden, cos, sin, [None] * t.num_hidden_layers, causal_mask(len(toks), 0, dt),
+                                   from_row=S - 1)
+    return logits[0]
