@@ -134,6 +134,37 @@ ASRB_API int asrb_ingested_read(asrb_session* s, int b, float* out /* [n_samples
 ASRB_API int asrb_transcribe_ingested(asrb_session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids,
                              int max_new_tokens, int32_t* ids_out, int32_t* lens_out);
 
+/* ---- long-form audio: cut recordings at low-energy points, decode the pieces as one batch -------------------------- */
+/* asrb_ingest_pcm's ingest (same arguments, same kernels) into a separate long-audio buffer that the session grows on
+ * demand: files are not bounded by max_samples, and what asrb_ingest_pcm / asrb_transcribe_ingested consume is left as
+ * it is.  File f keeps n_samples_out[f] 16 kHz samples until the next asrb_ingest_long; a failed call leaves none. */
+ASRB_API int asrb_ingest_long(asrb_session* s, const void* const* pcm, const int64_t* n_frames, const int32_t* channels,
+                              const int32_t* sample_rate, const int32_t* format, int n_files, int64_t* n_samples_out);
+ASRB_API int asrb_long_read(asrb_session* s, int file, float* out /* [n_samples[file]] */);
+/* Cut points of every ingested file, on the GPU.  Window energy e[j] = sum x[i]^2, i in [160 j, 160 j + 1600) (100 ms
+ * every 10 ms, f32 samples accumulated in fp64, deterministic).  For a file of N samples: c_0 = 0; while
+ * N - c_k > max_segment_samples, c_{k+1} is the window centre p = 160 j + 800 with the least e[j] among
+ *   c_k + max_segment_samples - search_samples <= p <= min(c_k + max_segment_samples, N - 16000),
+ * ties to the largest p.  The segments are [c_k, c_{k+1}) and [c_K, N): each at most max_segment_samples, the last at
+ * least 1 s; a file of at most max_segment_samples is the one segment [0, N).
+ *   n_segments_out   [n_files] segments per file
+ *   start_out/end_out [max_segments] sample offsets within the file, in (file, time) order
+ * ASRB_ERR_INVALID: max_segment_samples / search_samples not multiples of 160, max_segment_samples < 80000 (5 s),
+ * search_samples < 32000 (2 s) or > max_segment_samples / 2; or more segments than max_segments, in which case
+ * n_segments_out is still filled so the caller can retry.  ASRB_ERR_STATE if nothing was ingested. */
+ASRB_API int asrb_segment_long(asrb_session* s, int64_t max_segment_samples, int64_t search_samples, int max_segments,
+                               int32_t* n_segments_out, int64_t* start_out, int64_t* end_out);
+/* asrb_transcribe_ids on n views [start[i], end[i]) of ingested file file[i] as one batch of n utterances, read in place
+ * by the mel (no copy).  The views may come from asrb_segment_long or from the caller (their own VAD).  Everything that
+ * applies to asrb_transcribe_ids applies unchanged: options, contexts, asrb_last_logprobs / _top_logprobs / _nbest /
+ * _timings / _prefill_stats, asrb_session_device_ids; the sampling row r is the view's position in this call.
+ * ASRB_ERR_INVALID before any work: a file index out of range, start >= end, end past the file, a view longer than
+ * max_samples or shorter than 201 samples, n < 1, or n (x beam_size) > max_batch.  ASRB_ERR_STATE if nothing was
+ * ingested with asrb_ingest_long. */
+ASRB_API int asrb_transcribe_segments(asrb_session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
+                                      const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
+                                      int32_t* ids_out, int32_t* lens_out);
+
 /* Stage entry points = the calls transcribe() makes (each runs on the session stream;
  * *_read functions synchronise and copy to host, for parity tests). */
 /* WhisperFeatureExtractor::extract, src/mel.rs:49-96 (called at src/inference.rs:95) */

@@ -7,11 +7,14 @@ anywhere on the line, and `Temperature: x` reports the temperature of the kept a
 `--beam-size N` (N in 1..6) decodes with beam search and prints an `N-best:` block of the ranked hypotheses with their
 scores; `--length-penalty A` (A in [0, 10]) scores them with ((5 + n) / 6) ** A instead of the length.
 `--context TEXT` or `--context-file PATH` (UTF-8), anywhere on the line, places TEXT in the prompt's system turn to bias
-recognition towards its words (names, jargon, a keyword list)."""
+recognition towards its words (names, jargon, a keyword list).
+`--max-segment S` (seconds, anywhere on the line) cuts the recording at quiet points into segments of at most S seconds,
+decodes them as batches and prints a `Segments:` block of `[start - end] text` lines."""
 import sys
 
 USAGE = ("Usage: python -m qwen3_asr_rs_b200 <model_dir> <audio_file> [language] [--logprobs] [--top-logprobs N] "
-         "[--temperature T[,T...]] [--seed N] [--beam-size N] [--length-penalty A] [--context TEXT | --context-file PATH]")
+         "[--temperature T[,T...]] [--seed N] [--beam-size N] [--length-penalty A] [--context TEXT | --context-file PATH] "
+         "[--max-segment S]")
 
 
 def parse_args(argv):
@@ -129,6 +132,28 @@ def split_context(argv):
     return f[0], text
 
 
+def split_max_segment(argv):
+    """Remove `--max-segment S` from argv -> (remaining argv, S in seconds; None when absent), or None when the value is
+    missing or not a valid segment length (a whole number of 10 ms, at least 5 s)."""
+    from .inference import check_segmenting, default_search_s
+    m = _take_flag(argv, "--max-segment")
+    if m is None:
+        return None
+    if m[1] is None:
+        return m[0], None
+    try:
+        s = float(m[1])
+        check_segmenting(s, default_search_s(s))
+    except ValueError:
+        return None
+    return m[0], s
+
+
+def format_segment(start_s: float, end_s: float, text: str) -> str:
+    """One line of the `Segments:` block."""
+    return f"  [{start_s:.2f} - {end_s:.2f}] {text}"
+
+
 def format_candidates(cands, decode) -> str:
     """One line of candidates: `'text' -0.0123` pairs, best first; `decode([id])` gives each candidate's text."""
     return "  ".join(f"{decode([i])!r} {lp:.4f}" for i, lp in cands)
@@ -136,6 +161,11 @@ def format_candidates(cands, decode) -> str:
 
 def main(argv=None) -> int:
     argv = list(sys.argv[1:] if argv is None else argv)
+    seg = split_max_segment(argv)
+    if seg is None:
+        print(USAGE, file=sys.stderr)
+        return 1
+    argv, max_segment = seg
     ctx = split_context(argv)
     beam = split_beam(ctx[0]) if ctx is not None else None
     sampling = split_sampling(beam[0]) if beam is not None else None
@@ -161,6 +191,8 @@ def main(argv=None) -> int:
             kw.update(beam_size=beam_size, length_penalty=length_penalty)
         if ctx[1]:
             kw.update(context=ctx[1])
+        if max_segment is not None:
+            kw.update(max_segment_s=max_segment)
         r = eng.transcribe(audio, language, logprobs=logprobs, top_logprobs=top, **kw)
         decode = eng.tokenizer.decode if eng.tokenizer is not None else (lambda ids: " ".join(str(i) for i in ids))
     finally:
@@ -181,6 +213,10 @@ def main(argv=None) -> int:
         print("N-best:")
         for j, (text, score) in enumerate(r.nbest):
             print(f"  [{j}] {score:.4f} {text}")
+    if r.segments is not None:
+        print("Segments:")
+        for start_s, end_s, text in r.segments:
+            print(format_segment(start_s, end_s, text))
     return 0
 
 

@@ -18,6 +18,7 @@ SYMBOLS = [
     "asrb_debug_mega_timeline", "asrb_session_stats", "asrb_session_device_ids", "asrb_model_lossy_tensors", "asrb_ingest_pcm", "asrb_ingested_read", "asrb_transcribe_ingested",
     "asrb_last_logprobs", "asrb_last_top_logprobs", "asrb_last_nbest", "asrb_last_beam_stats",
     "asrb_session_create_ex", "asrb_session_set_context", "asrb_last_prefill_stats",
+    "asrb_ingest_long", "asrb_long_read", "asrb_segment_long", "asrb_transcribe_segments",
 ]
 
 
@@ -88,6 +89,10 @@ def load_library() -> C.CDLL:
         "asrb_session_create_ex": [vp, C.c_int, i64, C.c_int, C.c_int, C.c_int, P(vp)],
         "asrb_session_set_context": [vp, C.c_int, P(P(i64)), P(i32)],
         "asrb_last_prefill_stats": [vp, P(i64), C.c_int],
+        "asrb_ingest_long": [vp, P(vp), P(i64), P(i32), P(i32), P(i32), C.c_int, P(i64)],
+        "asrb_long_read": [vp, C.c_int, P(C.c_float)],
+        "asrb_segment_long": [vp, i64, i64, C.c_int, P(i32), P(i64), P(i64)],
+        "asrb_transcribe_segments": [vp, C.c_int, P(i32), P(i64), P(i64), P(P(i64)), P(i32), C.c_int, P(i32), P(i32)],
     }
     for name, args in sig.items():
         fn = getattr(lib, name)

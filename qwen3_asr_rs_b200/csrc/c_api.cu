@@ -30,6 +30,14 @@ void session_last_top_logprobs(Session* s, int max_new_tokens, int k, int32_t* i
 void session_ingest_pcm(Session* s, const void* const* pcm, const int64_t* n_frames, const int32_t* channels, const int32_t* rate,
                         const int32_t* format, int batch, int64_t* n_samples_out);
 void session_ingested_read(Session* s, int b, float* out);
+void session_ingest_long(Session* s, const void* const* pcm, const int64_t* n_frames, const int32_t* channels, const int32_t* rate,
+                         const int32_t* format, int n_files, int64_t* n_samples_out);
+void session_long_read(Session* s, int f, float* out);
+void session_segment_long(Session* s, int64_t max_seg, int64_t search, int max_segments, int32_t* n_seg_out, int64_t* start_out,
+                          int64_t* end_out);
+void session_transcribe_segments(Session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
+                                 const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
+                                 int32_t* ids_out, int32_t* lens_out);
 void session_device_ids(Session* s, const int32_t** ids, const int32_t** lens, int* stride, int* batch);
 void session_last_nbest(Session* s, int max_new_tokens, int k, int32_t* ids_out, int32_t* lens_out, float* sum_out,
                         float* score_out, int32_t* eos_out);
@@ -196,6 +204,23 @@ int asrb_ingested_read(asrb_session* s, int b, float* out) { return guarded([&] 
 int asrb_transcribe_ingested(asrb_session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
                              int32_t* ids_out, int32_t* lens_out) {
     return guarded([&] { NONNULL(s); session_transcribe_ids(s->s, nullptr, nullptr, 0, lang_ids, n_lang_ids, max_new_tokens, ids_out, lens_out); });
+}
+int asrb_ingest_long(asrb_session* s, const void* const* pcm, const int64_t* n_frames, const int32_t* channels,
+                     const int32_t* sample_rate, const int32_t* format, int n_files, int64_t* n_samples_out) {
+    return guarded([&] { NONNULL(s); NONNULL(pcm); NONNULL(n_frames); NONNULL(channels); NONNULL(sample_rate); NONNULL(format);
+                         session_ingest_long(s->s, pcm, n_frames, channels, sample_rate, format, n_files, n_samples_out); });
+}
+int asrb_long_read(asrb_session* s, int file, float* out) { return guarded([&] { NONNULL(s); NONNULL(out); session_long_read(s->s, file, out); }); }
+int asrb_segment_long(asrb_session* s, int64_t max_segment_samples, int64_t search_samples, int max_segments,
+                      int32_t* n_segments_out, int64_t* start_out, int64_t* end_out) {
+    return guarded([&] { NONNULL(s); NONNULL(n_segments_out); NONNULL(start_out); NONNULL(end_out);
+                         session_segment_long(s->s, max_segment_samples, search_samples, max_segments, n_segments_out, start_out, end_out); });
+}
+int asrb_transcribe_segments(asrb_session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
+                             const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
+                             int32_t* ids_out, int32_t* lens_out) {
+    return guarded([&] { NONNULL(s); NONNULL(file); NONNULL(start); NONNULL(end); NONNULL(ids_out); NONNULL(lens_out);
+                         session_transcribe_segments(s->s, n, file, start, end, lang_ids, n_lang_ids, max_new_tokens, ids_out, lens_out); });
 }
 int asrb_session_device_ids(asrb_session* s, const int32_t** ids_dev, const int32_t** lens_dev, int* row_stride, int* batch) {
     return guarded([&] { NONNULL(s); NONNULL(ids_dev); NONNULL(lens_dev); NONNULL(row_stride); NONNULL(batch);

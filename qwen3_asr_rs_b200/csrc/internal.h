@@ -139,6 +139,9 @@ void launch_gemm_simt(const GemmA& A, const bf16* W, int N, const GemmEpi& E, cu
 void launch_mel(const Model& m, const float* samples, const int64_t* d_soff, const int64_t* d_n,
                 const int64_t* d_npad, const int64_t* d_foff, int batch, int max_frames,
                 float* mel_out, int* d_maxkey, cudaStream_t st);
+// segment.cu: window energies and cut points of the long-audio files (DESIGN.md section 4.6)
+void launch_segment(const float* d_long, const int64_t* d_plan, int n_files, int64_t total_blocks, int64_t max_seg,
+                    int64_t search, double* d_blk, int64_t* d_cuts, int64_t* d_ncuts, int sm_count, cudaStream_t st);
 // elementwise.cu
 void launch_conv1(const Model& m, const float* mel, const int* d_chunk_clip, const int* d_chunk_f0,
                   const int64_t* d_foff, const int64_t* d_frames, int n_chunks,

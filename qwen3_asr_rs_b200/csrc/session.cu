@@ -101,10 +101,19 @@ struct Session {
     int ctx_rows = 0;
     std::vector<std::vector<int>> ctx;
     int64_t pf_rows = 0, pf_shared_rows = 0, pf_fan_bytes = 0;   // last prefill: rows computed / taken from a leader, KV bytes fanned out
+    // long-form audio (asrb_ingest_long): file f holds long_n[f] samples at d_long + long_off[f], zero padded to a
+    // multiple of 160; not bounded by max_samples, grown on demand.  Segment views of it are decoded in place.
+    float* d_long = nullptr; size_t long_cap = 0;
+    std::vector<int64_t> long_n, long_off;
+    double* d_seg_blk = nullptr; size_t seg_blk_cap = 0;      // asrb_segment_long scratch: 160-sample block energies
+    int64_t* d_seg_i64 = nullptr; size_t seg_i64_cap = 0;     // ... its plan, cut counts and cuts
     ~Session();
 };
 
 Session::~Session() {
+    if (d_long) cudaFree(d_long);
+    if (d_seg_blk) cudaFree(d_seg_blk);
+    if (d_seg_i64) cudaFree(d_seg_i64);
     if (step_graph) cudaGraphExecDestroy(step_graph);
     for (auto& e : ev) if (e) cudaEventDestroy(e);
     for (void* p : owned) cudaFree(p);
@@ -251,21 +260,25 @@ void session_free(Session* s) { delete s; }
 // -------------------------------------------------------------------------------------------------
 // step 2: mel  (inference.rs:95)
 // -------------------------------------------------------------------------------------------------
-void session_mel(Session* s, const float* const* samples, const int64_t* n_samples, int batch, int64_t* n_frames_out) {
+// view_off != nullptr: utterance b is the view of n_samples[b] samples at d_long + view_off[b] (asrb_transcribe_segments),
+// read in place by the mel kernel, which reads sample j only for j < n
+static void mel_impl(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* view_off,
+                     int64_t* n_frames_out) {
     ASRB_REQUIRE(batch >= 1 && batch <= s->max_batch, ASRB_ERR_INVALID, "batch exceeds session capacity");
     ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
-    const bool ingested = (samples == nullptr);          // samples already in HBM, written by asrb_ingest_pcm
+    const bool views = view_off != nullptr;
+    const bool ingested = (samples == nullptr) && !views;   // samples already in HBM, written by asrb_ingest_pcm
     if (ingested) ASRB_REQUIRE((int)s->ingested_n.size() == batch, ASRB_ERR_STATE, "no ingested audio for this batch");
     s->B = batch; s->stage = 0;
     s->n.assign(batch, 0); s->npad.assign(batch, 0); s->F.assign(batch, 0); s->foff.assign(batch, 0); s->soff.assign(batch, 0);
     int64_t so = 0, fo = 0; int maxF = 0;
     for (int b = 0; b < batch; ++b) {
         int64_t n = ingested ? s->ingested_n[b] : n_samples[b];
-        ASRB_REQUIRE((ingested || samples[b]) && n > 0 && n <= s->max_samples, ASRB_ERR_INVALID, "n_samples out of session capacity");
+        ASRB_REQUIRE((ingested || views || samples[b]) && n > 0 && n <= s->max_samples, ASRB_ERR_INVALID, "n_samples out of session capacity");
         int64_t np = ((n + 159) / 160) * 160;                                       // mel.rs:51
         ASRB_REQUIRE(np > 200, ASRB_ERR_INVALID, "utterance too short for reflect padding (needs > 200 samples)");
-        s->n[b] = n; s->npad[b] = np; s->F[b] = np / 160; s->soff[b] = so; s->foff[b] = fo;
-        if (!s->resident && !ingested) {
+        s->n[b] = n; s->npad[b] = np; s->F[b] = np / 160; s->soff[b] = views ? view_off[b] : so; s->foff[b] = fo;
+        if (!s->resident && !ingested && !views) {
             memcpy(s->h_samples + so, samples[b], n * sizeof(float));
             if (np > n) memset(s->h_samples + so + n, 0, (np - n) * sizeof(float));
         }
@@ -275,15 +288,18 @@ void session_mel(Session* s, const float* const* samples, const int64_t* n_sampl
     int64_t* h = s->h_i64; const int Bm = s->max_batch;
     for (int b = 0; b < batch; ++b) { h[b] = s->soff[b]; h[Bm + b] = s->n[b]; h[2 * Bm + b] = s->npad[b]; h[3 * Bm + b] = s->foff[b]; h[4 * Bm + b] = s->F[b]; }
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_i64, h, 5 * Bm * sizeof(int64_t), cudaMemcpyHostToDevice, s->st));
-    if (!s->resident && !ingested)
+    if (!s->resident && !ingested && !views)
         ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_samples, s->h_samples, so * sizeof(float), cudaMemcpyHostToDevice, s->st));
     if (ingested) s->ingested_n.clear();                 // consumed
     if (s->timing) ASRB_CUDA_CHECK(cudaEventRecord(s->ev[1], s->st));
-    launch_mel(*s->m, s->d_samples, s->d_i64, s->d_i64 + Bm, s->d_i64 + 2 * Bm, s->d_i64 + 3 * Bm, batch, maxF, s->d_mel,
-               s->d_maxkey, s->st);
+    launch_mel(*s->m, views ? s->d_long : s->d_samples, s->d_i64, s->d_i64 + Bm, s->d_i64 + 2 * Bm, s->d_i64 + 3 * Bm, batch,
+               maxF, s->d_mel, s->d_maxkey, s->st);
     s->launches += 3;
     if (n_frames_out) for (int b = 0; b < batch; ++b) n_frames_out[b] = s->F[b];
     s->stage = 1;
+}
+void session_mel(Session* s, const float* const* samples, const int64_t* n_samples, int batch, int64_t* n_frames_out) {
+    mel_impl(s, samples, n_samples, batch, nullptr, n_frames_out);
 }
 
 // step 1 on the GPU (src/audio.rs:162-245): raw interleaved PCM -> mono 16 kHz f32 in the session's sample buffer
@@ -304,6 +320,83 @@ void session_ingested_read(Session* s, int b, float* out) {
     int64_t so = 0;
     for (int i = 0; i < b; ++i) so += ((s->ingested_n[i] + 159) / 160) * 160;
     ASRB_CUDA_CHECK(cudaMemcpy(out, s->d_samples + so, (size_t)s->ingested_n[b] * sizeof(float), cudaMemcpyDeviceToHost));
+}
+
+// (re)allocate a session scratch buffer that is not in `owned` to at least `bytes`; its contents are not kept
+template <typename T> static void grow(Session* s, T** p, size_t* cap, size_t n) {
+    if (n <= *cap && *p) return;
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));      // the old buffer may still be read
+    if (*p) { cudaFree(*p); *p = nullptr; *cap = 0; }
+    ASRB_CUDA_CHECK(cudaMalloc(p, std::max<size_t>(n, 1) * sizeof(T)));
+    *cap = n;
+}
+
+// asrb_ingest_long: the ingest of asrb_ingest_pcm into the long-audio buffer; a failed call leaves nothing ingested
+void session_ingest_long(Session* s, const void* const* pcm, const int64_t* n_frames, const int32_t* channels, const int32_t* rate,
+                         const int32_t* format, int n_files, int64_t* n_samples_out) {
+    ASRB_REQUIRE(n_files >= 1, ASRB_ERR_INVALID, "n_files must be >= 1");
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    s->long_n.clear(); s->long_off.clear();
+    size_t total = 0;
+    for (int f = 0; f < n_files; ++f) {
+        ASRB_REQUIRE(n_frames[f] > 0 && rate[f] >= 1000 && rate[f] <= 768000, ASRB_ERR_INVALID, "ingest: bad PCM description");
+        const int64_t nout = (n_frames[f] * 16000 + rate[f] - 1) / rate[f];       // = ingest_pcm's output length
+        total += (size_t)((nout + 159) / 160) * 160;
+    }
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));      // the ingest staging buffers may still be in use
+    grow(s, &s->d_long, &s->long_cap, total);
+    if (!s->ingest) s->ingest = ingest_state_new();
+    std::vector<int64_t> n((size_t)n_files), so((size_t)n_files);
+    ingest_pcm(s->ingest, s->st, pcm, n_frames, channels, rate, format, n_files, s->d_long, std::numeric_limits<int64_t>::max(),
+               n.data(), so.data());
+    s->long_n = n; s->long_off = so;
+    if (n_samples_out) for (int f = 0; f < n_files; ++f) n_samples_out[f] = n[f];
+}
+void session_long_read(Session* s, int f, float* out) {
+    ASRB_REQUIRE(f >= 0 && f < (int)s->long_n.size(), ASRB_ERR_STATE, "long_read: nothing ingested for this index");
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    ASRB_CUDA_CHECK(cudaMemcpy(out, s->d_long + s->long_off[f], (size_t)s->long_n[f] * sizeof(float), cudaMemcpyDeviceToHost));
+}
+
+// asrb_segment_long: the cut rule of segment.cu on every long-audio file; segments in (file, time) order
+void session_segment_long(Session* s, int64_t max_seg, int64_t search, int max_segments, int32_t* n_seg_out, int64_t* start_out,
+                          int64_t* end_out) {
+    ASRB_REQUIRE(!s->long_n.empty(), ASRB_ERR_STATE, "segment_long: nothing ingested with asrb_ingest_long");
+    ASRB_REQUIRE(max_seg % 160 == 0 && search % 160 == 0 && max_seg >= 80000 && search >= 32000 && 2 * search <= max_seg,
+                 ASRB_ERR_INVALID, "segment_long: need multiples of 160 with max_segment >= 80000 and 32000 <= search <= max_segment / 2");
+    ASRB_REQUIRE(max_segments >= 0, ASRB_ERR_INVALID, "max_segments must be >= 0");
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    const int F = (int)s->long_n.size();
+    std::vector<int64_t> plan((size_t)4 * F + 1);         // off | n | boff[F + 1] | coff
+    int64_t* off = plan.data(); int64_t* n = off + F; int64_t* boff = n + F; int64_t* coff = boff + F + 1;
+    int64_t nblk = 0, ncut = 0;
+    for (int f = 0; f < F; ++f) {
+        off[f] = s->long_off[f]; n[f] = s->long_n[f];
+        boff[f] = nblk; nblk += n[f] / 160;
+        coff[f] = ncut; ncut += n[f] / (max_seg - search) + 1;   // each cut advances by >= max_seg - search
+    }
+    boff[F] = nblk;
+    grow(s, &s->d_seg_blk, &s->seg_blk_cap, (size_t)nblk);
+    grow(s, &s->d_seg_i64, &s->seg_i64_cap, plan.size() + F + ncut);
+    int64_t* d_ncuts = s->d_seg_i64 + plan.size(); int64_t* d_cuts = d_ncuts + F;
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_seg_i64, plan.data(), plan.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s->st));
+    launch_segment(s->d_long, s->d_seg_i64, F, nblk, max_seg, search, s->d_seg_blk, d_cuts, d_ncuts, s->m->ctx->sm_count, s->st);
+    std::vector<int64_t> res((size_t)F + ncut);
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(res.data(), d_ncuts, res.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, s->st));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    int64_t total = 0;
+    for (int f = 0; f < F; ++f) { total += res[f] + 1; if (n_seg_out) n_seg_out[f] = (int32_t)(res[f] + 1); }
+    ASRB_REQUIRE(total <= max_segments, ASRB_ERR_INVALID,
+                 "segment_long: " + std::to_string(total) + " segments do not fit in max_segments (n_segments_out holds the counts)");
+    int64_t o = 0;
+    for (int f = 0; f < F; ++f) {
+        const int64_t* c = res.data() + F + coff[f];
+        for (int64_t k = 0; k <= res[f]; ++k, ++o) {
+            start_out[o] = k == 0 ? 0 : c[k - 1];
+            end_out[o] = k == res[f] ? n[f] : c[k];
+        }
+    }
 }
 
 void session_mel_read(Session* s, int b, float* out) {
@@ -821,11 +914,11 @@ void session_generate(Session* s, int max_new_tokens, int32_t* ids_out, int32_t*
     }
 }
 
-void session_transcribe_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch,
+static void transcribe_impl(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* view_off,
                             const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
                             int32_t* ids_out, int32_t* lens_out) {
     ASRB_REQUIRE(ids_out && lens_out, ASRB_ERR_INVALID, "null output");
-    if (samples == nullptr) batch = (int)s->ingested_n.size();      // asrb_transcribe_ingested
+    if (samples == nullptr && view_off == nullptr) batch = (int)s->ingested_n.size();      // asrb_transcribe_ingested
     check_sampling_options(s, batch);
     check_context(s, batch);
     ASRB_REQUIRE(max_new_tokens >= 1 && max_new_tokens <= s->max_new, ASRB_ERR_INVALID, "max_new_tokens exceeds session capacity");
@@ -833,7 +926,7 @@ void session_transcribe_ids(Session* s, const float* const* samples, const int64
     s->launches = 0; s->decode_steps = 0;
     ASRB_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
     s->timing = true;
-    try { session_mel(s, samples, n_samples, batch, nullptr); } catch (...) { s->timing = false; throw; }   // records ev[1] after the H2D
+    try { mel_impl(s, samples, n_samples, batch, view_off, nullptr); } catch (...) { s->timing = false; throw; }   // records ev[1] after the H2D
     s->timing = false;
     ASRB_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
     session_encode(s, nullptr);
@@ -845,6 +938,31 @@ void session_transcribe_ids(Session* s, const float* const* samples, const int64
     ASRB_CUDA_CHECK(cudaEventSynchronize(s->ev[5]));
     for (int i = 0; i < 5; ++i) ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[i], s->ev[i], s->ev[i + 1]));
     ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[5], s->ev[0], s->ev[5]));
+}
+void session_transcribe_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch,
+                            const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
+                            int32_t* ids_out, int32_t* lens_out) {
+    transcribe_impl(s, samples, n_samples, batch, nullptr, lang_ids, n_lang_ids, max_new_tokens, ids_out, lens_out);
+}
+
+// asrb_transcribe_segments: n views [start, end) of the long-audio files as one batch, every argument checked first
+void session_transcribe_segments(Session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
+                                 const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
+                                 int32_t* ids_out, int32_t* lens_out) {
+    ASRB_REQUIRE(!s->long_n.empty(), ASRB_ERR_STATE, "transcribe_segments: nothing ingested with asrb_ingest_long");
+    ASRB_REQUIRE(n >= 1 && n <= s->max_batch, ASRB_ERR_INVALID, "transcribe_segments: n must be in [1, max_batch]");
+    std::vector<int64_t> off((size_t)n), len((size_t)n);
+    for (int i = 0; i < n; ++i) {
+        const int f = file[i];
+        ASRB_REQUIRE(f >= 0 && f < (int)s->long_n.size(), ASRB_ERR_INVALID, "transcribe_segments: file index out of range");
+        ASRB_REQUIRE(start[i] >= 0 && start[i] < end[i] && end[i] <= s->long_n[f], ASRB_ERR_INVALID,
+                     "transcribe_segments: need 0 <= start < end <= the file's samples");
+        len[i] = end[i] - start[i];
+        ASRB_REQUIRE(len[i] >= 201 && len[i] <= s->max_samples, ASRB_ERR_INVALID,
+                     "transcribe_segments: a view must hold 201 .. max_samples samples");
+        off[i] = s->long_off[f] + start[i];
+    }
+    transcribe_impl(s, nullptr, len.data(), n, off.data(), lang_ids, n_lang_ids, max_new_tokens, ids_out, lens_out);
 }
 
 void session_last_timings(Session* s, float* ms6, int64_t* kernels, int64_t* steps) {

@@ -179,6 +179,53 @@ def _max_len(rows) -> int:
     return max((len(r) for r in rows if r is not None), default=0) if rows is not None else 0
 
 
+def check_segmenting(max_segment_s, search_s) -> Tuple[int, int]:
+    """The `max_segment_s` / `search_s` arguments of transcribe_long as 16 kHz sample counts: each a whole number of
+    10 ms, with max_segment_s >= 5 and 2 <= search_s <= max_segment_s / 2, else ValueError."""
+    out = []
+    for name, v in (("max_segment_s", max_segment_s), ("search_s", search_s)):
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating)) or not math.isfinite(float(v)):
+            raise ValueError(f"{name} must be a finite number of seconds, got {v!r}")
+        n = int(round(float(v) * MEL_SAMPLE_RATE))
+        if n % 160 or abs(n - float(v) * MEL_SAMPLE_RATE) > 1e-6 * max(1.0, n):
+            raise ValueError(f"{name} must be a whole number of 10 ms, got {v!r}")
+        out.append(n)
+    max_seg, search = out
+    if max_seg < 5 * MEL_SAMPLE_RATE or search < 2 * MEL_SAMPLE_RATE or 2 * search > max_seg:
+        raise ValueError(f"need max_segment_s >= 5 and 2 <= search_s <= max_segment_s / 2, got {max_segment_s!r}, {search_s!r}")
+    return max_seg, search
+
+
+def default_search_s(max_segment_s: float) -> float:
+    """The search window transcribe() and the CLI use with `max_segment_s`: 5 s, or half of it in whole 10 ms when
+    that is shorter."""
+    return min(5.0, math.floor(float(max_segment_s) * 100 / 2) / 100)
+
+
+def _pcm_arrays(pcms) -> List[np.ndarray]:
+    """PCM arrays as contiguous [frames, channels] of a supported dtype, else ValueError."""
+    arrs = [np.ascontiguousarray(a if a.ndim == 2 else a.reshape(-1, 1)) for a in pcms]
+    for a in arrs:
+        if a.dtype.name not in AsrInference._PCM_FMT:
+            raise ValueError(f"PCM dtype must be int16 / int32 / float32, got {a.dtype}")
+    return arrs
+
+
+def _concat_runs(runs: Sequence["TranscribeIds"]) -> "TranscribeIds":
+    """The TranscribeIds of consecutive waves as one: per-utterance fields concatenated, times and counters summed."""
+    if len(runs) == 1:
+        return runs[0]
+    r = TranscribeIds(sum((x.ids for x in runs), []), {}, sum(x.kernels_launched for x in runs),
+                      sum(x.decode_steps for x in runs))
+    for x in runs:
+        for name, ms in x.stage_ms.items():
+            r.stage_ms[name] = r.stage_ms.get(name, 0.0) + ms
+    for field in ("logprobs", "eos_logprobs", "top_logprobs", "eos_top_logprobs", "nbest"):
+        if getattr(runs[0], field) is not None:
+            setattr(r, field, sum((getattr(x, field) for x in runs), []))
+    return r
+
+
 @dataclass
 class TranscribeResult:           # inference.rs:270-274
     text: str
@@ -192,6 +239,33 @@ class TranscribeResult:           # inference.rs:270-274
     eos_top_logprobs: Optional[List[Tuple[int, float]]] = None   # ... of the step that selected EOS (None: stopped by the cap)
     temperature: Optional[float] = None             # transcribe(temperature=...): that of the kept attempt
     nbest: Optional[List[Tuple[str, float]]] = None   # transcribe(beam_size=K > 1): the K hypotheses as (text, score), ranked
+    # transcribe(max_segment_s=...): the segments as (start_s, end_s, text), in time order
+    segments: Optional[List[Tuple[float, float, str]]] = None
+
+
+@dataclass
+class LongSegment:
+    """One segment of a long recording (transcribe_long): its time span, ids and the per-utterance fields of
+    TranscribeIds for it."""
+    start_s: float
+    end_s: float
+    ids: List[int]
+    logprobs: Optional[List[float]] = None
+    eos_logprob: Optional[float] = None
+    top_logprobs: Optional[List[List[Tuple[int, float]]]] = None
+    eos_top_logprobs: Optional[List[Tuple[int, float]]] = None
+    temperature: Optional[float] = None
+    nbest: Optional[List[Tuple[List[int], float, float, int]]] = None
+
+
+@dataclass
+class LongResult:
+    files: List[List[LongSegment]]   # per file, its segments in time order
+    stage_ms: Dict[str, float]       # device time per stage, summed over the waves
+    kernels_launched: int
+    decode_steps: int
+    n_segments: int
+    n_waves: int                     # asrb_transcribe_segments calls, fallback re-runs included
 
 
 @dataclass
@@ -575,6 +649,15 @@ class AsrInference:
         arrs, ptrs, lens = self._pack_samples(clips)
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
         s = self._ensure_session(B * K, max(a.shape[0] for a in arrs), mx, max_new_tokens, _max_len(context_ids))
+        return self._run(s, B, max_new_tokens, logprobs, top_logprobs, temperature, seed, beam, context_ids,
+                         lambda ids, n: self._lib.asrb_transcribe_ids(s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
+                                                                      ids, n))
+
+    def _run(self, s, B: int, max_new_tokens: int, logprobs: bool, top_logprobs: int, temperature: Optional[float],
+             seed: int, beam, context_ids, call) -> TranscribeIds:
+        """One decode call on session s with this call's options set and restored around it: `call(ids_out, lens_out)`
+        runs the library's transcribe entry point for B utterances and returns its status."""
+        K = beam[0] if beam else 1
         ids = np.zeros((B, max_new_tokens), dtype=np.int32)
         n = np.zeros(B, dtype=np.int32)
         if logprobs:
@@ -587,9 +670,7 @@ class AsrInference:
             undo += self._set_beam(s, K, beam[1] if beam else None)
             if context_ids is not None:
                 self._set_context(s, context_ids)
-            _lib.check(self._lib.asrb_transcribe_ids(
-                s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
-                ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
+            _lib.check(call(ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
             return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs, K)
         finally:
             if context_ids is not None:
@@ -655,48 +736,155 @@ class AsrInference:
         K = beam[0] if beam else 1
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
         s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens, slots=B * K, max_context=_max_len(context_ids))
-        ids = np.zeros((B, max_new_tokens), dtype=np.int32)
-        n = np.zeros(B, dtype=np.int32)
-        if logprobs:
-            self._record_logprobs(s, True)
-        if top_logprobs:
-            self._record_top_logprobs(s, top_logprobs, True)
-        undo = []
-        try:
-            undo = self._set_sampling(s, temperature, seed)
-            undo += self._set_beam(s, K, beam[1] if beam else None)
-            if context_ids is not None:
-                self._set_context(s, context_ids)
-            _lib.check(self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens),
-                                                          ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
-            return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs, K)
-        finally:
-            if context_ids is not None:
-                self._set_context(s, None)
-            self._restore(s, undo)
-            if logprobs:
-                self._record_logprobs(s, False)
-            if top_logprobs:
-                self._record_top_logprobs(s, top_logprobs, False)
+        return self._run(s, B, max_new_tokens, logprobs, top_logprobs, temperature, seed, beam, context_ids,
+                         lambda ids, n: self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens), ids, n))
+
+    # ---- long-form audio: cut at low-energy points on the GPU, decode the pieces in waves -----------------------
+    def ingest_long(self, pcms: Sequence, rates: Sequence[int]) -> List[np.ndarray]:
+        """asrb_ingest_long + asrb_long_read (tests): interleaved PCM arrays [frames, channels] -> mono f32 @ 16 kHz in
+        the session's long-audio buffer, read back."""
+        s, n = self._ingest_long(pcms, rates, self._ensure_session(1, 16000, 0, 1))
+        self._long_files = len(n)
+        out = []
+        for f, m in enumerate(n):
+            a = np.empty(m, dtype=np.float32)
+            _lib.check(self._lib.asrb_long_read(s, f, a.ctypes.data_as(C.POINTER(C.c_float))))
+            out.append(a)
+        return out
+
+    def _ingest_long(self, pcms: Sequence, rates: Sequence[int], s):
+        arrs = _pcm_arrays(pcms)
+        B = len(arrs)
+        ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in arrs])
+        frames = (C.c_int64 * B)(*[a.shape[0] for a in arrs])
+        chans = (C.c_int32 * B)(*[a.shape[1] for a in arrs])
+        rts = (C.c_int32 * B)(*[int(r) for r in rates])
+        fmts = (C.c_int32 * B)(*[self._PCM_FMT[a.dtype.name] for a in arrs])
+        n = (C.c_int64 * B)()
+        _lib.check(self._lib.asrb_ingest_long(s, ptrs, frames, chans, rts, fmts, B, n))
+        return s, list(n)
+
+    def segment_long(self, max_segment_samples: int, search_samples: int) -> List[List[Tuple[int, int]]]:
+        """asrb_segment_long on the files of the last ingest: per file, its segments as (start, end) sample offsets."""
+        s = self._session
+        n_files = self._long_files
+        cap = 64 * n_files
+        while True:
+            nseg = (C.c_int32 * n_files)()
+            st, en = (C.c_int64 * cap)(), (C.c_int64 * cap)()
+            code = self._lib.asrb_segment_long(s, int(max_segment_samples), int(search_samples), cap, nseg, st, en)
+            if code == 1 and sum(nseg) > cap:                # did not fit: the counts are filled, retry with room
+                cap = sum(nseg)
+                continue
+            _lib.check(code)
+            break
+        out, o = [], 0
+        for f in range(n_files):
+            out.append([(int(st[o + k]), int(en[o + k])) for k in range(nseg[f])])
+            o += nseg[f]
+        return out
+
+    def transcribe_long(self, pcms: Sequence, rates: Sequence[int], max_segment_s: float = 30.0, search_s: float = 5.0,
+                        batch: int = 16, language_ids: Optional[Sequence] = None, max_new_tokens: int = MAX_NEW_TOKENS,
+                        logprobs: bool = False, top_logprobs: int = 0,
+                        temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
+                        logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
+                        length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None) -> "LongResult":
+        """Long recordings: ingest the files (raw PCM, as transcribe_pcm) into the long-audio buffer, cut them on the GPU
+        into segments of at most `max_segment_s` at the quietest 100 ms window of the last `search_s` before each limit
+        (asrb_segment_long), and decode the segments as views of that buffer (asrb_transcribe_segments) in waves of
+        `batch` segments in (file, time) order, `batch // beam_size` with a beam.  `max_new_tokens` applies per segment.
+        Every other keyword is that of transcribe_pcm, per segment: the language ids and context of a file apply to each
+        of its segments; temperature fallback re-runs only the failing segments, in waves of their own.
+        Returns per file its segments in time order."""
+        max_seg, search = check_segmenting(max_segment_s, search_s)
+        n_files = len(pcms)
+        if len(rates) != n_files or n_files < 1:
+            raise ValueError("pcms and rates must be non-empty and of equal length")
+        if isinstance(batch, bool) or not isinstance(batch, (int, np.integer)) or batch < 1:
+            raise ValueError(f"batch must be an int >= 1, got {batch!r}")
+        tk = check_top_logprobs(top_logprobs)
+        check_temperature(temperature)
+        check_seed(seed)
+        K, _ = check_beam(beam_size, length_penalty)
+        if batch // K < 1:
+            raise ValueError(f"batch ({batch}) must be >= beam_size ({K})")
+        ctx = check_context_ids(context_ids, n_files, self.config.text.vocab_size)
+        arrs = _pcm_arrays(pcms)
+        if language_ids is not None and len(language_ids) != n_files:
+            raise ValueError("language_ids must be None or one entry per file")
+        longest = max(-(-a.shape[0] * MEL_SAMPLE_RATE // int(r)) for a, r in zip(arrs, rates))
+        mx = _max_len(language_ids)
+        s = self._ensure_session(batch, min(max_seg, max(longest, 201)), mx, max_new_tokens, _max_len(ctx))
+        s, n = self._ingest_long(arrs, rates, s)
+        self._long_files = n_files
+        cuts = self.segment_long(max_seg, search)
+        segs = [(f, a, b) for f in range(n_files) for a, b in cuts[f]]
+        self._long_waves = 0
+
+        def once(idx, lp, k, t, beam):
+            W = batch // (beam[0] if beam else 1)
+            runs = []
+            for w0 in range(0, len(idx), W):
+                wave = [segs[i] for i in idx[w0:w0 + W]]
+                m = len(wave)
+                fl = (C.c_int32 * m)(*[x[0] for x in wave])
+                st = (C.c_int64 * m)(*[x[1] for x in wave])
+                en = (C.c_int64 * m)(*[x[2] for x in wave])
+                lang = None if language_ids is None else [language_ids[x[0]] for x in wave]
+                keep, lptrs, llens, _ = self._pack_lang(lang, m)
+                wctx = None if ctx is None else [ctx[x[0]] for x in wave]
+                runs.append(self._run(s, m, max_new_tokens, lp, k, t, seed, beam, wctx,
+                                      lambda ids, nn: self._lib.asrb_transcribe_segments(
+                                          s, m, fl, st, en, lptrs, llens, int(max_new_tokens), ids, nn)))
+                self._long_waves += 1
+            return _concat_runs(runs)
+        r = self._sampled(len(segs), once, temperature, seed, logprob_threshold, logprobs, tk, beam_size, length_penalty)
+        out: List[List[LongSegment]] = [[] for _ in range(n_files)]
+        for i, (f, a, b) in enumerate(segs):
+            seg = LongSegment(a / MEL_SAMPLE_RATE, b / MEL_SAMPLE_RATE, r.ids[i])
+            if r.logprobs is not None:
+                seg.logprobs, seg.eos_logprob = r.logprobs[i], r.eos_logprobs[i]
+            if r.top_logprobs is not None:
+                seg.top_logprobs, seg.eos_top_logprobs = r.top_logprobs[i], r.eos_top_logprobs[i]
+            if r.temperatures is not None:
+                seg.temperature = r.temperatures[i]
+            if r.nbest is not None:
+                seg.nbest = r.nbest[i]
+            out[f].append(seg)
+        return LongResult(out, r.stage_ms, r.kernels_launched, r.decode_steps, len(segs), self._long_waves)
 
     def transcribe(self, audio_path: str, language: Optional[str] = None,
                    max_new_tokens: int = MAX_NEW_TOKENS, gpu_ingest: bool = True, logprobs: bool = False,
                    top_logprobs: int = 0, temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
                    logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
-                   length_penalty: Optional[float] = None, context: Optional[str] = None) -> TranscribeResult:
+                   length_penalty: Optional[float] = None, context: Optional[str] = None,
+                   max_segment_s: Optional[float] = None) -> TranscribeResult:
         """AsrInference::transcribe (inference.rs:89-213): step 1 (WAV payload -> mono 16 kHz; on the GPU by default,
         `gpu_ingest=False` = the host loader) -> steps 2-8 on the GPU -> step 9 (detokenise + parse, host; needs
         tokenizer.json, else raw_output is the id list as text).  `logprobs`: also fill token_logprobs / avg_logprob;
         `top_logprobs` = k in 1..8: also fill top_logprobs (and token_logprobs / avg_logprob); `temperature`, `seed`,
         `logprob_threshold`, `beam_size`, `length_penalty`: as in transcribe_ids, and `temperature` of the result is that
         of the kept attempt; `nbest` holds the beam's hypotheses as (text, score).  `context`: text placed in the prompt's
-        system turn to bias recognition (keywords, names, related text; needs tokenizer.json; "" = none)."""
+        system turn to bias recognition (keywords, names, related text; needs tokenizer.json; "" = none).
+        `max_segment_s`: None decodes the file in one pass; a number of seconds runs transcribe_long with it (search
+        window min(5 s, half of it, in whole 10 ms)) and `max_new_tokens` per segment: see _long_result."""
         from .audio import load_wav, read_wav_pcm
         from .text import context_prompt_ids, language_prompt_ids, parse_asr_output
         lang_ids = language_prompt_ids(self.tokenizer, language)
         ctx_ids = context_prompt_ids(self.tokenizer, context)
         sampling = dict(temperature=temperature, seed=seed, logprob_threshold=logprob_threshold, beam_size=beam_size,
                         length_penalty=length_penalty, context_ids=[ctx_ids] if ctx_ids else None)
+        if max_segment_s is not None:
+            if gpu_ingest:
+                pcm, rate = read_wav_pcm(audio_path)
+            else:
+                pcm, rate = load_wav(audio_path, MEL_SAMPLE_RATE), MEL_SAMPLE_RATE
+            lr = self.transcribe_long([pcm], [rate], max_segment_s=max_segment_s, search_s=default_search_s(max_segment_s),
+                                      language_ids=[lang_ids] if lang_ids is not None else None,
+                                      max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs,
+                                      **sampling)
+            return self._long_result(lr.files[0], language, logprobs, top_logprobs)
         if gpu_ingest:
             pcm, rate = read_wav_pcm(audio_path)
             r = self.transcribe_pcm([pcm], [rate], language_ids=[lang_ids] if lang_ids is not None else None,
@@ -722,6 +910,41 @@ class AsrInference:
         if top_logprobs:
             res.top_logprobs = r.top_logprobs[0]
             res.eos_top_logprobs = r.eos_top_logprobs[0]
+        return res
+
+    def _long_result(self, segs: List[LongSegment], language: Optional[str], logprobs: bool,
+                     top_logprobs: int) -> TranscribeResult:
+        """The TranscribeResult of one segmented file: `segments` = (start_s, end_s, text) per segment; `text` = the
+        non-empty segment texts joined by text.join_segment_texts; `language` = the most frequent language of the
+        segments with text (of all segments when none has text), or "forced"; `raw_output` = the segments' raw outputs,
+        one per line; `ids`, `token_logprobs` and `top_logprobs` = the segments' concatenated; `avg_logprob` over all
+        ids and each segment's EOS; `eos_top_logprobs` = the last segment's; `temperature` = the highest kept one;
+        no `nbest` (a beam's hypotheses are per segment: transcribe_long returns them)."""
+        from .text import join_segment_texts, majority_language, parse_asr_output
+        parsed = []
+        for sg in segs:
+            raw = self.tokenizer.decode(sg.ids) if self.tokenizer is not None else " ".join(str(i) for i in sg.ids)
+            lang, text = parse_asr_output(raw, language is not None) if self.tokenizer is not None else ("unknown", raw)
+            parsed.append((raw, lang, text))
+        if language is not None:
+            lang = "forced"
+            join_lang = language
+        else:
+            with_text = [p[1] for p in parsed if p[2]]
+            lang = join_lang = majority_language(with_text or [p[1] for p in parsed])
+        res = TranscribeResult(text=join_segment_texts([p[2] for p in parsed], join_lang), language=lang,
+                               raw_output="\n".join(p[0] for p in parsed), ids=sum((sg.ids for sg in segs), []))
+        res.segments = [(sg.start_s, sg.end_s, p[2]) for sg, p in zip(segs, parsed)]
+        temps = [sg.temperature for sg in segs if sg.temperature is not None]
+        if temps:
+            res.temperature = max(temps)
+        if (logprobs or top_logprobs or temps) and segs[0].logprobs is not None:
+            res.token_logprobs = sum((sg.logprobs for sg in segs), [])
+            vals = res.token_logprobs + [sg.eos_logprob for sg in segs if sg.eos_logprob is not None]
+            res.avg_logprob = sum(vals) / len(vals) if vals else None
+        if top_logprobs:
+            res.top_logprobs = sum((sg.top_logprobs for sg in segs), [])
+            res.eos_top_logprobs = segs[-1].eos_top_logprobs
         return res
 
     # ---- stage-level calls (the calls transcribe() makes; used by the parity tests) ----

@@ -34,6 +34,24 @@ def parse_asr_output(raw: str, language_forced: bool) -> Tuple[str, str]:
     return "unknown", raw
 
 
+NO_SPACE_LANGUAGES = ("chinese", "japanese", "cantonese")   # written without spaces between words
+
+
+def join_segment_texts(texts: List[str], language: Optional[str]) -> str:
+    """The text of a segmented recording: the non-empty segment texts in order, joined with a space, or with nothing
+    when `language` is Chinese, Japanese or Cantonese (case-insensitive)."""
+    sep = "" if (language or "").strip().lower() in NO_SPACE_LANGUAGES else " "
+    return sep.join(t for t in texts if t)
+
+
+def majority_language(languages: List[str]) -> str:
+    """The most frequent of `languages`, the first to appear on ties ("unknown" when empty)."""
+    counts: dict = {}
+    for lang in languages:
+        counts[lang] = counts.get(lang, 0) + 1
+    return max(counts, key=lambda k: counts[k]) if counts else "unknown"
+
+
 class AsrTokenizer:
     """tokenizer.json wrapper (tokenizer.rs:4-50): encode without special tokens, decode skipping them."""
 

@@ -225,4 +225,51 @@ impl B200Engine {
         check(unsafe { ffi::asrb_session_set_option(session, lkey.as_ptr(), none.as_ptr()) })?;
         run
     }
+
+    /// Long recordings: 16 kHz mono f32 `samples` of any length are cut on the GPU at the quietest 100 ms window of
+    /// the last `search_samples` before every `max_segment_samples` (`asrb_segment_long`; both multiples of 160,
+    /// `max_segment_samples` >= 80000, 32000 <= `search_samples` <= `max_segment_samples` / 2), and the segments are
+    /// decoded as views of the ingested audio (`asrb_transcribe_segments`) in batches of up to `batch` segments.
+    /// Returns the segments in time order as (start, end in samples, ids); `max_new_tokens` applies per segment.
+    pub fn transcribe_long(&self, samples: &[f32], lang_ids: Option<&[i64]>, max_segment_samples: usize, search_samples: usize,
+                           batch: usize) -> Result<Vec<(i64, i64, Vec<i64>)>> {
+        if batch == 0 { return Err(anyhow!("batch must be >= 1")); }
+        let session = self.session_for_slots(max_segment_samples.min(samples.len()).max(201), batch)?;
+        let pcm = [samples.as_ptr() as *const std::os::raw::c_void];
+        let (frames, chans, rate, fmt) = ([samples.len() as i64], [1i32], [16000i32], [1i32]);   // ASRB_PCM_F32
+        let mut n = 0i64;
+        check(unsafe { ffi::asrb_ingest_long(session, pcm.as_ptr(), frames.as_ptr(), chans.as_ptr(), rate.as_ptr(), fmt.as_ptr(), 1, &mut n) })?;
+        let mut cap = 64usize;
+        let (starts, ends) = loop {
+            let mut nseg = 0i32;
+            let (mut st, mut en) = (vec![0i64; cap], vec![0i64; cap]);
+            let status = unsafe {
+                ffi::asrb_segment_long(session, max_segment_samples as i64, search_samples as i64, cap as i32, &mut nseg,
+                                       st.as_mut_ptr(), en.as_mut_ptr())
+            };
+            if status == ffi::ASRB_ERR_INVALID && nseg as usize > cap { cap = nseg as usize; continue; }
+            check(status)?;
+            st.truncate(nseg as usize);
+            en.truncate(nseg as usize);
+            break (st, en);
+        };
+        let m = self.max_new_tokens;
+        let mut out = Vec::with_capacity(starts.len());
+        for w0 in (0..starts.len()).step_by(batch) {
+            let k = batch.min(starts.len() - w0);
+            let files = vec![0i32; k];
+            let lp = vec![lang_ids.map_or(ptr::null(), |v| v.as_ptr()); k];
+            let ll = vec![lang_ids.map_or(0, |v| v.len() as i32); k];
+            let mut ids = vec![0i32; k * m];
+            let mut lens = vec![0i32; k];
+            check(unsafe {
+                ffi::asrb_transcribe_segments(session, k as i32, files.as_ptr(), starts[w0..].as_ptr(), ends[w0..].as_ptr(),
+                                              lp.as_ptr(), ll.as_ptr(), m as i32, ids.as_mut_ptr(), lens.as_mut_ptr())
+            })?;
+            for j in 0..k {
+                out.push((starts[w0 + j], ends[w0 + j], ids[j * m..j * m + lens[j] as usize].iter().map(|&t| t as i64).collect()));
+            }
+        }
+        Ok(out)
+    }
 }
