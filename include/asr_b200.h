@@ -93,7 +93,10 @@ ASRB_API int asrb_model_free(asrb_model* m);
 /* ---- session --------------------------------------------------------------------- */
 /* Capacity: up to max_batch utterances of up to max_samples samples each, prompt
  * suffix of up to max_lang_ids forced-language ids, up to max_new_tokens generated
- * ids (the reference caps at 4096, src/inference.rs:153). */
+ * ids (the reference caps at 4096, src/inference.rs:153).
+ * ASRB_ERR_INVALID when the context (audio tokens + prompt + max_new_tokens positions) exceeds the RoPE table, or when
+ * group * (128 + context) fp32 values (group = num_attention_heads / num_key_value_heads) do not fit the shared memory a
+ * block may opt in to: the per-phase decode attention keeps one score per (query head of a group, key) there. */
 ASRB_API int asrb_session_create(asrb_model* m, int max_batch, int64_t max_samples,
                         int max_lang_ids, int max_new_tokens, asrb_session** out);
 /* asrb_session_create with room for up to max_context_ids context ids per utterance (asrb_session_set_context);

@@ -463,6 +463,12 @@ void launch_lmhead_argmax(const Model& m, const float* x_rows, const int* d_row_
     }
 }
 
+static constexpr size_t DEC_ATTN_STATIC_SMEM = (128 + 32) * sizeof(float);   // tmp + red of dec_attn_kernel
+size_t dec_attn_smem_bytes(const Model& m, int max_ctx) {
+    const size_t group = m.d.c.num_attention_heads / m.d.c.num_key_value_heads;
+    return group * (128 + (size_t)max_ctx) * sizeof(float) + DEC_ATTN_STATIC_SMEM;
+}
+
 void launch_decode_step_phases(const Model& m, const DecodeBufs& ball, int Ball, float* kcache_all, float* vcache_all,
                                size_t cache_layer_stride, size_t cache_seq_stride, int max_ctx, bool write_logits,
                                cudaStream_t st, int64_t* launches) {
@@ -471,7 +477,7 @@ void launch_decode_step_phases(const Model& m, const DecodeBufs& ball, int Ball,
     ASRB_REQUIRE(c.head_dim == 128, ASRB_ERR_INVALID, "decode attention needs head_dim 128");
     const int sms = m.ctx->sm_count;
     const int group = c.num_attention_heads / c.num_key_value_heads;
-    size_t attn_smem = (size_t)(group * 128 + group * max_ctx) * sizeof(float);
+    const size_t attn_smem = dec_attn_smem_bytes(m, max_ctx) - DEC_ATTN_STATIC_SMEM;
     if (attn_smem > 48 * 1024)     // per device attribute: set on every launch (a process may drive several GPUs)
         ASRB_CUDA_CHECK(cudaFuncSetAttribute(dec_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_smem));
     for (int b0 = 0; b0 < Ball; b0 += 8) {           // sub-batches of 8 sequences (weights are re-streamed per sub-batch)

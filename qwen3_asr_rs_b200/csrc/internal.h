@@ -217,6 +217,9 @@ struct DecodeBufs {
 void launch_decode_step_phases(const Model& m, const DecodeBufs& b, int B, float* kcache, float* vcache,
                                size_t cache_layer_stride, size_t cache_seq_stride, int max_ctx,
                                bool write_logits, cudaStream_t st, int64_t* launches);
+// shared memory the per-phase decode attention needs for a session of max_ctx positions: the queries of one GQA group,
+// one fp32 score per (query head, key), and its static reduction scratch.  Checked at session creation.
+size_t dec_attn_smem_bytes(const Model& m, int max_ctx);
 // final-norm + lm_head + argmax on arbitrary rows of a residual stream (prefill last rows);
 // also performs the greedy bookkeeping of src/inference.rs:161-170 (EOS check, append, embed)
 struct MegaBufs { unsigned* bar = nullptr; float* part = nullptr; long long* dbg = nullptr; size_t part_bytes = 0; unsigned* steps_issued = nullptr;

@@ -156,6 +156,13 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
         s->maxS = s->maxT + 15 + max_lang + max_context;
         s->max_ctx = s->maxS + max_new;
         ASRB_REQUIRE(s->max_ctx <= m->rope_max_pos, ASRB_ERR_INVALID, "context exceeds RoPE table");
+        // the per-phase decode step (asrb_decode_step with logits, any model or context the fused steps decline) holds a
+        // score per (query head of a GQA group, key) in shared memory: refuse here what its launch would refuse mid-decode
+        ASRB_REQUIRE(dec_attn_smem_bytes(*m, s->max_ctx) <= m->ctx->smem_optin, ASRB_ERR_INVALID,
+                     "session context of " + std::to_string(s->max_ctx) + " positions (audio tokens + prompt + max_new_tokens) with GQA group " +
+                         std::to_string(c.num_attention_heads / c.num_key_value_heads) + " needs " +
+                         std::to_string(dec_attn_smem_bytes(*m, s->max_ctx)) + " bytes of shared memory for decode attention, the device offers " +
+                         std::to_string(m->ctx->smem_optin) + ": lower max_samples or max_new_tokens");
         ASRB_CUDA_CHECK(cudaStreamCreateWithFlags(&s->st, cudaStreamNonBlocking));
         for (auto& e : s->ev) ASRB_CUDA_CHECK(cudaEventCreate(&e));
         const size_t Bm = max_batch;

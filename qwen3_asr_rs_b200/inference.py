@@ -395,7 +395,7 @@ class AsrInference:
                 or max_context > cap[4]:
             if self._session is not None:
                 _lib.check(self._lib.asrb_session_free(self._session))
-                self._session = None
+                self._session, self._cap = None, None        # a refused create below leaves no session, not a stale capacity
             new_cap = (max(batch, cap[0] if cap else 0), max(max_samples, cap[1] if cap else 0),
                        max(max_lang, cap[2] if cap else 0), max(max_new, cap[3] if cap else 0),
                        max(max_context, cap[4] if cap else 0))
