@@ -246,7 +246,21 @@ ASRB_API int asrb_session_stats(asrb_session* s, int64_t* out, int n);
  * "logprobs", asrb_last_logprobs (its per-token values and its EOS value).  Read all K with asrb_last_nbest.
  * Refused with ASRB_ERR_INVALID before any work: beam_size > 1 with temperature > 0, with top_logprobs >= 1, or with
  * batch * beam_size > max_batch; asrb_decode_step in a beam run.  A beam run takes one asrb_generate per prefill (its
- * end writes the result rows, which are also beam 0's slots); a second one returns ASRB_ERR_STATE. */
+ * end writes the result rows, which are also beam 0's slots); a second one returns ASRB_ERR_STATE.
+ * "no_repeat_ngram_size" = "0" (default: off) or N in "1".."16", and "repetition_penalty" = "1" (default: off) or a
+ * decimal in [1, 10], parsed in double and converted once to the fp32 theta; both latched at the prefill and applied to
+ * the whole run, on every decode path.  For sequence b at step n the history is ids[b][0 .. n), the ids this run
+ * generated for it: never the prompt, context, audio pad or forced-language ids, and never EOS.  Before any use of the
+ * step's logits every path replaces each logit l_v by l'_v:
+ *   1. penalty: v in the history: l'_v = l_v < 0 ? l_v * theta : l_v / theta (IEEE fp32 multiply and round-to-nearest
+ *      divide, the rule of HF's RepetitionPenaltyLogitsProcessor); otherwise l'_v = l_v;
+ *   2. ban: N >= 1 and some i in [0, n - N] with ids[i .. i+N-2] == ids[n-N+1 .. n-1]: l'_{ids[i+N-1]} = -inf (HF's
+ *      NoRepeatNGramLogitsProcessor restricted to the history; N = 1 bans every id already generated).
+ * Every use then sees l': the greedy argmax, the sampling keys fmaf(l', 1 / T, g), "logprobs" (log-probabilities under
+ * softmax(l')), the top-8 records, the beam candidates and their sums, and the logits asrb_decode_step returns.  Token 0
+ * has an empty history (l' = l).  A banned id is never selected: the vocabulary keeps more than 8 finite logits.  With
+ * both at their defaults the ids, records and kernels are exactly those above.  An invalid value is refused with
+ * ASRB_ERR_INVALID and the previous value is kept. */
 ASRB_API int asrb_session_set_option(asrb_session* s, const char* key, const char* value);
 
 /* Per-token log-probabilities of the last run (asrb_generate / asrb_transcribe_ids / asrb_transcribe_ingested, or

@@ -8,13 +8,15 @@ anywhere on the line, and `Temperature: x` reports the temperature of the kept a
 scores; `--length-penalty A` (A in [0, 10]) scores them with ((5 + n) / 6) ** A instead of the length.
 `--context TEXT` or `--context-file PATH` (UTF-8), anywhere on the line, places TEXT in the prompt's system turn to bias
 recognition towards its words (names, jargon, a keyword list).
+`--no-repeat-ngram N` (N in 0..16) bans every token that would repeat an N-gram of the tokens generated so far, and
+`--repetition-penalty P` (P in [1, 10]) penalises the logits of tokens generated so far; both anywhere on the line.
 `--max-segment S` (seconds, anywhere on the line) cuts the recording at quiet points into segments of at most S seconds,
 decodes them as batches and prints a `Segments:` block of `[start - end] text` lines."""
 import sys
 
 USAGE = ("Usage: python -m qwen3_asr_rs_b200 <model_dir> <audio_file> [language] [--logprobs] [--top-logprobs N] "
          "[--temperature T[,T...]] [--seed N] [--beam-size N] [--length-penalty A] [--context TEXT | --context-file PATH] "
-         "[--max-segment S]")
+         "[--no-repeat-ngram N] [--repetition-penalty P] [--max-segment S]")
 
 
 def parse_args(argv):
@@ -113,6 +115,25 @@ def split_beam(argv):
     return a[0], size, alpha
 
 
+def split_repetition(argv):
+    """Remove `--no-repeat-ngram N` and `--repetition-penalty P` from argv -> (remaining argv, N; 0 when absent, P; 1.0
+    when absent), or None when a value is missing or invalid."""
+    from .inference import check_repetition
+    n = _take_flag(argv, "--no-repeat-ngram")
+    if n is None:
+        return None
+    p = _take_flag(n[0], "--repetition-penalty")
+    if p is None:
+        return None
+    try:
+        if n[1] is not None and not n[1].isdigit():
+            return None
+        size, penalty = check_repetition(int(n[1]) if n[1] is not None else 0, float(p[1]) if p[1] is not None else 1.0)
+    except ValueError:
+        return None
+    return p[0], size, penalty
+
+
 def split_context(argv):
     """Remove `--context TEXT` and `--context-file PATH` from argv -> (remaining argv, context text; None when absent),
     or None when a value is missing, both are given, or the file cannot be read as UTF-8."""
@@ -166,7 +187,8 @@ def main(argv=None) -> int:
         print(USAGE, file=sys.stderr)
         return 1
     argv, max_segment = seg
-    ctx = split_context(argv)
+    rep = split_repetition(argv)
+    ctx = split_context(rep[0]) if rep is not None else None
     beam = split_beam(ctx[0]) if ctx is not None else None
     sampling = split_sampling(beam[0]) if beam is not None else None
     split = split_top_logprobs(sampling[0]) if sampling is not None else None
@@ -193,6 +215,8 @@ def main(argv=None) -> int:
             kw.update(context=ctx[1])
         if max_segment is not None:
             kw.update(max_segment_s=max_segment)
+        if rep[1] or rep[2] != 1.0:
+            kw.update(no_repeat_ngram_size=rep[1], repetition_penalty=rep[2])
         r = eng.transcribe(audio, language, logprobs=logprobs, top_logprobs=top, **kw)
         decode = eng.tokenizer.decode if eng.tokenizer is not None else (lambda ids: " ".join(str(i) for i in ids))
     finally:

@@ -5,7 +5,8 @@
 // the top candidate is EOS).  Around that:
 //   beam_step_kernel<true>   after the prefill: the token-0 walk on the single record, and the prompt expansion plan
 //   beam_step_kernel<false>  after every decode step: the walk over the K beams' records and the slot assignment
-//   beam_kv_copy_kernel      the KV copies those plans describe (positions after the last common ancestor only)
+//   beam_kv_copy_kernel      the KV copies those plans describe (positions after the last common ancestor only; the
+//                            ids_out entries of the same positions are copied by beam_step_kernel<false>)
 //   beam_finalize_kernel     backtracks the ranked hypotheses through the per-step history
 // The walk (one thread; at most BEAM_MAX * (BEAM_MAX + 2) = 48 candidates):
 //   candidates  the first K + 2 entries of each alive beam's record (at most two are EOS), sum = sum_parent + lp (fp32)
@@ -143,6 +144,13 @@ __global__ void __launch_bounds__(BEAM_THREADS) beam_step_kernel(BeamArgs a, con
                 for (int i = tid; i < a.hidden; i += BEAM_THREADS) a.x[(size_t)(j * B + b) * a.hidden + i] = 0.f;
         return;
     }
+    if constexpr (!FIRST)                          // a reassigned slot takes its new lineage's ids with its K/V: the same
+        for (int r = 0; r < K; ++r) {              // positions, ids[common + 1 .. t - 1] (the repetition controls' history)
+            const int s = new_slot[r], n = a.cp_n[s], i0 = a.cp_p0[s] - u.S;
+            const int* src = a.ids_out + (size_t)a.cp_src[s] * a.max_new + i0;
+            int* dst = a.ids_out + (size_t)s * a.max_new + i0;
+            for (int i = tid; i < n; i += BEAM_THREADS) dst[i] = src[i];
+        }
     for (int r = 0; r < K; ++r) {                  // the next token's embedding (text_decoder.rs:90-92)
         const bf16* e = a.embed + (size_t)new_tok[r] * a.hidden;
         float* xr = a.x + (size_t)new_slot[r] * a.hidden;

@@ -236,6 +236,57 @@ __device__ __forceinline__ void sample_merge_xor(int o, float& best_v, int& best
     if (ov > best_v || (ov == best_v && oi < best_i)) { best_v = ov; best_i = oi; if constexpr (LOGPROB) sel = osel; }
 }
 
+// ---- repetition controls: no-repeat n-gram bans and a repetition penalty --------------------------------
+// For sequence b at step n the history is ids[0 .. n), the ids this run generated for it (ids_out; never the prompt,
+// context, audio or forced-language ids, never EOS).  Before any use of the step's logits, logit l_v becomes
+//   penalty  v in the history:  l_v < 0 ? l_v * theta : l_v / theta       (IEEE fp32 multiply / round-to-nearest divide)
+//   ban      N >= 1 and some i in [0, n - N] with ids[i .. i+N-2] == ids[n-N+1 .. n-1], v = ids[i+N-1]:  -inf
+// Each sequence's rule is a pair of bit arrays over a range of ids, "in history" and "banned", built from its ids_out row
+// (rep_mark) and tested once per lm_head row at the fold (rep_logit).  The fused steps build them per CTA for the CTA's
+// own lm_head rows while layer 0's weights stream in; the per-phase path builds them over the whole vocabulary in
+// rep_mask_kernel.  A banned row takes part in no fold: its exp is 0, it is never the argmax, never a sampling draw and
+// never a candidate (the vocabulary always keeps more than TK_MAX finite logits).
+struct RepParams {          // device-resident, written at the prefill: a captured graph reads the values of its run
+    float theta;            // penalty, 1 = off
+    int ngram;              // N, 0 = off
+};
+// one sequence's bit arrays: bit (v & 31) of word (v >> 5) - w0 of hist / ban, for ids v of the range they cover
+struct RepBits {
+    const uint32_t* hist; const uint32_t* ban; int w0; float theta;
+};
+// set the bits of ids in [lo, hi) (w0 = lo >> 5) for history ids[0 .. n); thread t of nt; the arrays are zeroed and the
+// caller's threads synchronised before, and again before the bits are read
+__device__ __forceinline__ void rep_mark(const int* __restrict__ ids, int n, int N, int lo, int hi, uint32_t* hist,
+                                         uint32_t* ban, int t, int nt) {
+    const int w0 = lo >> 5;
+    for (int i = t; i < n; i += nt) {
+        const int v = __ldcg(ids + i);
+        if (v >= lo && v < hi) atomicOr(hist + ((v >> 5) - w0), 1u << (v & 31));
+        if (N >= 1 && i <= n - N) {            // the N-gram starting at i continues the current (N-1)-suffix
+            bool match = true;
+            for (int j = 0; j < N - 1 && match; ++j) match = __ldcg(ids + i + j) == __ldcg(ids + n - N + 1 + j);
+            if (match) {
+                const int u = __ldcg(ids + i + N - 1);
+                if (u >= lo && u < hi) atomicOr(ban + ((u >> 5) - w0), 1u << (u & 31));
+            }
+        }
+    }
+}
+// l <- the processed logit of row v; false: v is banned (l' = -inf) and takes part in no fold
+__device__ __forceinline__ bool rep_logit(const RepBits& r, int v, float& l) {
+    const int w = (v >> 5) - r.w0;
+    const uint32_t bit = 1u << (v & 31);
+    if (r.ban[w] & bit) { l = -INFINITY; return false; }
+    if (r.hist[w] & bit) l = l < 0.f ? l * r.theta : l / r.theta;
+    return true;
+}
+// the fold sites' form: REP = false compiles to nothing
+template <bool REP>
+__device__ __forceinline__ bool rep_keep(const RepBits* r, int v, float& l) {
+    if constexpr (REP) return rep_logit(*r, v, l);
+    else return true;
+}
+
 // order-preserving float <-> int key (for atomicMax on floats of either sign)
 __device__ __host__ __forceinline__ int float_to_ordered(float f) {
 #ifdef __CUDA_ARCH__

@@ -14,6 +14,7 @@
 // bookkeeping kernel (argmax, EOS check, append, embed next token; inference.rs:161-170) -- the
 // 151936 logits are only written in parity mode and no host sync happens per token.
 #include <algorithm>
+#include <type_traits>
 #include "internal.h"
 
 namespace asrb {
@@ -42,16 +43,27 @@ struct GemvSample {
     float* part_max; float* part_sel;               // ARGMAX_GUMBEL_LSE: [B][gridDim.x]
 };
 
-template <typename... S> __device__ __forceinline__ const GemvSample& gemv_sample(const S&... s) { return (s, ...); }
+// ARGMAX epilogues with the repetition controls: one more kernel argument, after the `sample` pack when there is one
+struct GemvRep {
+    const uint32_t* mask; int words;                // [B][2][words] each sequence's bit arrays (common.cuh), built before the step
+    const RepParams* rep;                           // the run's penalty
+};
 
-template <int MAXB, bool PRE_NORM, int EPI, typename... Sample>
-__global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p, Sample... sample) {
+// the extra argument of type T
+template <typename T, typename S0, typename... S> __device__ __forceinline__ const T& gemv_arg(const S0& s0, const S&... s) {
+    if constexpr (std::is_same_v<T, S0>) return s0;
+    else return gemv_arg<T>(s...);
+}
+
+template <int MAXB, bool PRE_NORM, int EPI, typename... Extra>
+__global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p, Extra... extra) {
     extern __shared__ float xs[];          // [MAXB][K]
     __shared__ float red[32];
     __shared__ float bestv[DG_WARPS][MAXB];
     __shared__ int besti[DG_WARPS][MAXB];
     constexpr bool SMP = EPI == DE_ARGMAX_GUMBEL || EPI == DE_ARGMAX_GUMBEL_LSE, SLSE = EPI == DE_ARGMAX_GUMBEL_LSE;
     constexpr bool ARGMAX = EPI == DE_ARGMAX || EPI == DE_ARGMAX_LSE || SMP, LSE = EPI == DE_ARGMAX_LSE;
+    constexpr bool REP = (std::is_same_v<GemvRep, Extra> || ...);
     const int K = p.K, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     for (int b = 0; b < MAXB; ++b) {
         if (b < p.B) {
@@ -82,7 +94,7 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p, Samp
     if constexpr (SMP) {
 #pragma unroll
         for (int b = 0; b < MAXB; ++b) {
-            const GemvSample& ps = gemv_sample(sample...);
+            const GemvSample& ps = gemv_arg<GemvSample>(extra...);
             dr[b] = make_draw(ps.smp, b < p.B ? __ldg(ps.n_out + b) : 0, ps.row0 + b);
             if constexpr (SLSE) { bs[b] = 0.f; bm[b] = -INFINITY; bsel[b] = 0.f; }
         }
@@ -123,7 +135,14 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p, Samp
                 if (EPI == DE_RESID) p.out[(size_t)b * p.ldo + u] += acc[0][b];
                 if (EPI == DE_SWIGLU) p.out[(size_t)b * p.ldo + u] = silu(acc[0][b]) * acc[RSTEP - 1][b];
                 if (ARGMAX) {
+                    bool keep = true;                // REP: the processed logit replaces the raw one everywhere
+                    if constexpr (REP) {
+                        const GemvRep& pr = gemv_arg<GemvRep>(extra...);
+                        const uint32_t* h = pr.mask + (size_t)b * 2 * pr.words;
+                        keep = rep_logit(RepBits{h, h + pr.words, 0, __ldg(&pr.rep->theta)}, u, acc[0][b]);
+                    }
                     if (p.logits) p.logits[(size_t)b * p.ldl + u] = acc[0][b];
+                    if (!keep) continue;             // banned: -inf in the logits, no part in any fold
                     if constexpr (SMP) {
                         float unused = 0.f;
                         if constexpr (SLSE) sample_fold<true>(dr[b], acc[0][b], u, bv[b], bi[b], bs[b], bm[b], bsel[b]);
@@ -179,20 +198,35 @@ __global__ void __launch_bounds__(DG_THREADS) dec_gemv_kernel(GemvParams p, Samp
             float sum = 0.f;                     // the warps' raw sums rescaled to the CTA's raw maximum, in warp order
             for (int w = 0; w < DG_WARPS; ++w) sum += lse_rescale(bests[w][tid], bestm[w][tid], M);
             const size_t o = (size_t)tid * gridDim.x + blockIdx.x;
-            const GemvSample& ps = gemv_sample(sample...);
+            const GemvSample& ps = gemv_arg<GemvSample>(extra...);
             p.part_val[o] = v; p.part_idx[o] = idx; p.part_sum[o] = sum; ps.part_max[o] = M; ps.part_sel[o] = bestsel[ws][tid];
         }
     }
 }
 
+template <int MB, bool PRE_NORM, int EPI, typename... Extra>
+static void launch_gemv_kernel(const GemvParams& p, int grid, size_t smem, cudaStream_t st, const Extra&... extra) {
+    auto kern = dec_gemv_kernel<MB, PRE_NORM, EPI, Extra...>;
+    if (smem > 48 * 1024) ASRB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, DG_THREADS, smem, st>>>(p, extra...);
+}
+
 template <bool PRE_NORM, int EPI>
-static void run_gemv(const GemvParams& p, int grid, cudaStream_t st, const GemvSample* ps = nullptr) {
+static void run_gemv(const GemvParams& p, int grid, cudaStream_t st, const GemvSample* ps = nullptr, const GemvRep* pr = nullptr) {
     size_t smem_of[4] = {(size_t)1 * p.K * 4, (size_t)2 * p.K * 4, (size_t)4 * p.K * 4, (size_t)8 * p.K * 4};
     ASRB_REQUIRE(p.K % 256 == 0, ASRB_ERR_INVALID, "decode GEMV needs K % 256 == 0");
     ASRB_REQUIRE(p.B >= 1 && p.B <= 8, ASRB_ERR_INVALID, "per-phase decode supports batch 1..8");
 #define ASRB_GEMV_CASE(MB, IDX)                                                                              \
     {                                                                                                        \
-        if constexpr (EPI == DE_ARGMAX_GUMBEL || EPI == DE_ARGMAX_GUMBEL_LSE) {                              \
+        if constexpr (EPI == DE_ARGMAX || EPI == DE_ARGMAX_LSE || EPI == DE_ARGMAX_GUMBEL || EPI == DE_ARGMAX_GUMBEL_LSE) \
+            if (pr) {                                                                                        \
+                if constexpr (EPI == DE_ARGMAX_GUMBEL || EPI == DE_ARGMAX_GUMBEL_LSE)                        \
+                    launch_gemv_kernel<MB, PRE_NORM, EPI>(p, grid, smem_of[IDX], st, *ps, *pr);              \
+                else launch_gemv_kernel<MB, PRE_NORM, EPI>(p, grid, smem_of[IDX], st, *pr);                  \
+                ASRB_CUDA_CHECK(cudaGetLastError());                                                         \
+                return;                                                                                      \
+            }                                                                                                \
+        if constexpr (EPI == DE_ARGMAX_GUMBEL || EPI == DE_ARGMAX_GUMBEL_LSE) {                       \
             auto kern = dec_gemv_kernel<MB, PRE_NORM, EPI, GemvSample>;                                      \
             if (smem_of[IDX] > 48 * 1024)                                                                    \
                 ASRB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_of[IDX])); \
@@ -423,6 +457,23 @@ void launch_greedy(const Model& m, const DecodeBufs& b, int B, cudaStream_t st, 
     if (launches) *launches += 1;
 }
 
+// repetition controls, per-phase path: one CTA per sequence builds its bit arrays over the whole vocabulary from its
+// generated ids (common.cuh), before the step
+__global__ void __launch_bounds__(256) rep_mask_kernel(const int* __restrict__ ids_out, const int* __restrict__ n_out, int max_new,
+                                                       const RepParams* __restrict__ rep, uint32_t* __restrict__ mask, int words, int vocab) {
+    const int b = blockIdx.x;
+    uint32_t* h = mask + (size_t)b * 2 * words;
+    for (int i = threadIdx.x; i < 2 * words; i += blockDim.x) h[i] = 0u;
+    __syncthreads();
+    rep_mark(ids_out + (size_t)b * max_new, min(n_out[b], max_new), __ldg(&rep->ngram), 0, vocab, h, h + words, threadIdx.x, blockDim.x);
+}
+
+void launch_rep_mask(const DecodeBufs& b, int R, cudaStream_t st, int64_t* launches) {
+    rep_mask_kernel<<<R, 256, 0, st>>>(b.ids_out, b.n_out, b.max_new, b.rep_params, b.rep_mask, b.rep_words, 32 * b.rep_words);
+    ASRB_CUDA_CHECK(cudaGetLastError());
+    if (launches) *launches += 1;
+}
+
 static DecodeBufs offset_bufs(const DecodeBufs& b, int b0, const Model& m) {
     const asrb_dims& c = m.d.c;
     DecodeBufs o = b;
@@ -448,17 +499,19 @@ void launch_lmhead_argmax(const Model& m, const float* x_rows, const int* d_row_
         p.norm_w = m.final_norm; p.eps = (float)c.rms_norm_eps;
         p.logits = (write_logits || (b.topk && !b.sample)) ? ob.logits : nullptr; p.ldl = c.vocab_size;   // TOPK: greedy_kernel reads them
         p.part_val = ob.part_val; p.part_idx = ob.part_idx; p.B = nb;
+        GemvRep pr{b.rep_mask + (size_t)b0 * 2 * b.rep_words, b.rep_words, b.rep_params};
+        const GemvRep* prp = b.rep ? &pr : nullptr;  // the repetition controls: the processed logits everywhere below
         if (b.sample) {                              // the draw's row is global: b0 + the sequence's index in the launch
             GemvSample ps{};
             ps.smp = b.smp; ps.n_out = ob.n_out; ps.row0 = b0;
             if (b.logprobs) {
                 p.part_sum = ob.part_sum; ps.part_max = ob.part_max; ps.part_sel = ob.part_sel;
-                run_gemv<true, DE_ARGMAX_GUMBEL_LSE>(p, b.n_part, st, &ps);
+                run_gemv<true, DE_ARGMAX_GUMBEL_LSE>(p, b.n_part, st, &ps, prp);
             }
-            else run_gemv<true, DE_ARGMAX_GUMBEL>(p, b.n_part, st, &ps);
+            else run_gemv<true, DE_ARGMAX_GUMBEL>(p, b.n_part, st, &ps, prp);
         }
-        else if (b.logprobs) { p.part_sum = ob.part_sum; run_gemv<true, DE_ARGMAX_LSE>(p, b.n_part, st); }
-        else run_gemv<true, DE_ARGMAX>(p, b.n_part, st);
+        else if (b.logprobs) { p.part_sum = ob.part_sum; run_gemv<true, DE_ARGMAX_LSE>(p, b.n_part, st, nullptr, prp); }
+        else run_gemv<true, DE_ARGMAX>(p, b.n_part, st, nullptr, prp);
         if (launches) *launches += 1;
     }
 }

@@ -69,6 +69,10 @@ struct Params {
     const SampleParams* smp;     // 1 / temperature and seed of the run
     int row0;                    // row of sequence 0 of this launch in the call's batch (the draw's counter)
     float* part_max; float* part_sel;       // LOGPROB: [nb][n_part] raw maximum logit, raw logit of the best-key row
+    // REP instantiations only (appended as well)
+    uint32_t* rep_bits;                     // [gridDim.x][NB][2][rep_words] each CTA's history / banned bits of its lm_head rows
+    int rep_words;
+    const RepParams* rep;                   // the run's penalty and N
 };
 
 __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
@@ -167,7 +171,9 @@ enum { BE_STORE = 0, BE_SWIGLU = 1, BE_ARGMAX = 2 };
 // SAMPLE: each (tile row, sequence) thread folds the sampling keys of draw (p.row0 + sequence, n = p.n_out[sequence])
 // instead of the logits (common.cuh); with LOGPROB the tile-row, CTA and last-CTA merges also carry the raw (max, sum)
 // record and the raw logit of the best-key row
-template <int H, int QD, int I, int NB, int NS, int KVK, bool LOGPROB, bool TOPK = false, bool SAMPLE = false>
+// REP: each (tile row, sequence) thread first replaces the logit by its processed value under its sequence's bit arrays
+// (repetition controls, common.cuh), built for the CTA's lm_head rows while layer 0's weights stream in
+template <int H, int QD, int I, int NB, int NS, int KVK, bool LOGPROB, bool TOPK = false, bool SAMPLE = false, bool REP = false>
 __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params p) {   // 9 warps are allocated as 12 (granularity 4): 168 registers
     static_assert(NB % 8 == 0 && NB <= 16, "NB must be 8 or 16");
     static_assert(H % 256 == 0 && QD % H == 0 && I % H == 0, "chunking needs QD, I multiples of H, H multiple of 256");
@@ -320,6 +326,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
     Draw dr{};                                               // SAMPLE: the draw of its sequence (n_out changes only after
     float smx = -INFINITY, ssel = 0.f;                       // every CTA's ticket); SLP: raw maximum, raw logit of the best key
     if constexpr (SAMPLE) if (tid < 16 * NB && tid % NB < nb) dr = make_draw(p.smp, __ldcg(p.n_out + tid % NB), p.row0 + tid % NB);
+    RepBits rb{};                                            // REP: the bit arrays of its sequence (n_out changes only after
+    if constexpr (REP) {                                     // every CTA's ticket)
+        const Slice sl = make_slice(nullptr, p.V, H, 1);
+        uint32_t* rbits = p.rep_bits + (size_t)blockIdx.x * NB * 2 * p.rep_words;   // this CTA's [NB][2][rep_words]
+        const int W = p.rep_words, N = __ldg(&p.rep->ngram);
+        for (int i = tid; i < NB * 2 * W; i += NCONS) rbits[i] = 0u;
+        cons_sync();
+        for (int b = 0; b < nb; ++b)
+            rep_mark(p.ids_out + (size_t)b * p.max_new, min(__ldcg(p.n_out + b), p.max_new), N, sl.r0, sl.r1, rbits + b * 2 * W,
+                     rbits + b * 2 * W + W, tid, NCONS);
+        const uint32_t* h = rbits + (tid % NB) * 2 * W;
+        rb = RepBits{h, h + W, sl.r0 >> 5, __ldg(&p.rep->theta)};
+    }
     // merging CTA: which (sequence, kv head), and which record slots will be written for it -- slot u holds a record iff a
     // run starts at split u, i.e. u == 0 or item base + u opens its owner's range.  Positions do not change within the
     // step, so this is computed once, not per layer (the owner search is a dozen integer divisions per slot).
@@ -504,7 +523,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
                 }
                 cons_sync();
                 if (tid < 16 * NB) {
-                    const float v = tile_sum(ppar);
+                    float v = tile_sum(ppar);
                     const int rr = t0 + tid / NB, sq = tid % NB, row = r + rr;
                     const bool valid = rr < rows && sq < nb;
                     if (epi == BE_STORE) {
@@ -513,14 +532,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_batch_kernel(const Params 
                         const float up = __shfl_down_sync(0xffffffffu, v, NB);     // rows 2j (gate) and 2j + 1 (up): NB threads apart
                         if (valid && !(rr & 1)) sx_store(sxo + (size_t)sq * I + (row >> 1), silu(v) * up);
                     } else if constexpr (SAMPLE) {
-                        if (valid) sample_fold<LOGPROB>(dr, v, row, best_v, best_i, best_s, smx, ssel);   // rows ascend per thread
+                        if (valid && rep_keep<REP>(&rb, row, v))
+                            sample_fold<LOGPROB>(dr, v, row, best_v, best_i, best_s, smx, ssel);   // rows ascend per thread
                     } else if constexpr (LOGPROB) {
-                        if (valid) {
+                        if (valid && rep_keep<REP>(&rb, row, v)) {
                             lse_fold(v, row, best_v, best_i, best_s);     // rows ascend per thread: ties keep the first
                             if constexpr (TOPK) tk_insert(tk, v, row);
                         }
                     } else {
-                        if (valid && (v > best_v || (v == best_v && row < best_i))) { best_v = v; best_i = row; }
+                        if (valid && rep_keep<REP>(&rb, row, v) && (v > best_v || (v == best_v && row < best_i))) { best_v = v; best_i = row; }
                     }
                 }
                 ppar ^= 1;
@@ -1004,6 +1024,24 @@ size_t decode_batch_sx_bytes(const Model& m) {
     return (size_t)2 * c.num_hidden_layers * 16 * ((size_t)2 * c.hidden_size + m.d.q_dim + c.intermediate_size) * 4;
 }
 
+// the instantiation for the model's dims, NB and the run's options: sampling (with or without the log-probability
+// record) is never combined with the candidate lists
+template <bool LP, bool TK, bool SM, bool RP>
+static const void* batch_fn_dims(const asrb_dims& c, int NB) {
+    if (bdims_match<1024, 2048, 3072>(c))
+        return NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, LP, TK, SM, RP>
+                       : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, LP, TK, SM, RP>;
+    return NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, LP, TK, SM, RP>
+                   : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, LP, TK, SM, RP>;
+}
+template <bool RP>
+static const void* batch_fn(const DecodeBufs& b, const asrb_dims& c, int NB) {
+    if (b.sample) return b.logprobs ? batch_fn_dims<true, false, true, RP>(c, NB) : batch_fn_dims<false, false, true, RP>(c, NB);
+    if (b.topk) return batch_fn_dims<true, true, false, RP>(c, NB);
+    if (b.logprobs) return batch_fn_dims<true, false, false, RP>(c, NB);
+    return batch_fn_dims<false, false, false, RP>(c, NB);
+}
+
 void launch_decode_step_batch(const Model& m, const DecodeBufs& b, int B, float* kcache, float* vcache,
                               size_t cache_layer_stride, size_t cache_seq_stride, int max_ctx, int ctx_now, const MegaBufs& mb,
                               cudaStream_t st, int64_t* launches) {
@@ -1015,46 +1053,7 @@ void launch_decode_step_batch(const Model& m, const DecodeBufs& b, int B, float*
         const int nb = std::min(16, B - b0);
         const BatchCfg k = batch_cfg(nb);
         const size_t smem = batch_smem_bytes(c.hidden_size, k);
-        const void* fn = nullptr;
-        if (b.sample) {     // with or without the log-probability record; never with the candidate lists
-            if (b.logprobs) {
-                if (bdims_match<1024, 2048, 3072>(c))
-                    fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, true, false, true>
-                                   : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, true, false, true>;
-                else
-                    fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, true, false, true>
-                                   : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, true, false, true>;
-            } else {
-                if (bdims_match<1024, 2048, 3072>(c))
-                    fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, false, false, true>
-                                   : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, false, false, true>;
-                else
-                    fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, false, false, true>
-                                   : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, false, false, true>;
-            }
-        }
-        else if (b.topk) {
-            if (bdims_match<1024, 2048, 3072>(c))
-                fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, true, true>
-                               : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, true, true>;
-            else
-                fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, true, true>
-                               : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, true, true>;
-        }
-        else if (b.logprobs) {
-            if (bdims_match<1024, 2048, 3072>(c))
-                fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, true>
-                               : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, true>;
-            else
-                fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, true>
-                               : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, true>;
-        }
-        else if (bdims_match<1024, 2048, 3072>(c))
-            fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 8, 5, 64, false>
-                           : (const void*)megab::decode_batch_kernel<1024, 2048, 3072, 16, 3, 64, false>;
-        else
-            fn = k.NB == 8 ? (const void*)megab::decode_batch_kernel<256, 512, 512, 8, 5, 64, false>
-                           : (const void*)megab::decode_batch_kernel<256, 512, 512, 16, 3, 64, false>;
+        const void* fn = b.rep ? batch_fn<true>(b, c, k.NB) : batch_fn<false>(b, c, k.NB);
         ASRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         megab::Params p{};
         p.layers = m.d_dec_layers_b; p.lm_head = m.lm_head_b; p.embed = m.embed; p.final_norm = m.final_norm;
@@ -1090,6 +1089,7 @@ void launch_decode_step_batch(const Model& m, const DecodeBufs& b, int B, float*
             p.smp = b.smp; p.row0 = b0;
             if (b.logprobs) { p.part_max = b.part_max + (size_t)b0 * b.n_part; p.part_sel = b.part_sel + (size_t)b0 * b.n_part; }
         }
+        if (b.rep) { p.rep_bits = b.rep_mask; p.rep_words = rep_cta_words(c, G); p.rep = b.rep_params; }
         { static const int fl = getenv("ASRB_BATCH_FLAGS") ? atoi(getenv("ASRB_BATCH_FLAGS")) : 0; p.flags = fl; }   // bit 0 (K/V L2 prefetch): measured slower, off
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {   // tags must stay monotonic: wipe long before the epoch wraps
             ASRB_CUDA_CHECK(cudaMemsetAsync(mb.part, 0, mb.part_bytes, st));

@@ -63,6 +63,10 @@ struct Params {
     const SampleParams* smp;     // 1 / temperature and seed of the run
     int row;                     // the sequence's row in the call's batch (the draw's counter)
     float* part_max; float* part_sel;       // LOGPROB: [gridDim.x] raw maximum logit, raw logit of the best-key row
+    // REP instantiations only (appended as well)
+    uint32_t* rep_bits;          // [gridDim.x][2][rep_words] each CTA's history / banned bits of its lm_head rows
+    int rep_words;
+    const RepParams* rep;        // the run's penalty and N
 };
 
 static_assert(KV_KEYS * HD * 4 == SLOT_BYTES, "K / V tiles travel through the weight ring: one tile per slot");
@@ -277,11 +281,11 @@ __device__ __forceinline__ void consume_ksplit(const Slice& s, const Ring& ring,
 }
 
 // K <= 1024 GEMVs (qkv, gate/up, lm_head of the 0.6B dims): four rows per warp and turn, two ring slots (32 rows) per turn.
-template <int K, int EPI, bool LOGPROB, bool TOPK, bool SAMPLE>
+template <int K, int EPI, bool LOGPROB, bool TOPK, bool SAMPLE, bool REP>
 __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
                                              uint32_t tag, uint32_t* sxo, float& best_v, int& best_i, float& best_s,
                                              const float* norm_w, float norm_r, long long* fine, TopK* tk,
-                                             const Draw* dr, float* smx, float* ssel) {
+                                             const Draw* dr, float* smx, float* ssel, const RepBits* rb) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int fi = 0;
 #define CF() do { if (fine && threadIdx.x == 0 && fi < 24) fine[fi++] = clock64(); } while (0)
@@ -313,7 +317,7 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
                 const int ri = i0 + (i < nv ? i : 0);
                 rp[i] = ri < rowsA ? baseA + (size_t)ri * NU : baseB + (size_t)(ri - rowsA) * NU;
             }
-            const float v = row_dot4<K>(rp[0], rp[1], rp[2], rp[3], xr, lane);
+            float v = row_dot4<K>(rp[0], rp[1], rp[2], rp[3], xr, lane);
             const int row = r + i0 + j;
             if (EPI == ME_SWIGLU) {                // rows (gate, up, gate, up): lanes 0 / 16 hold a gate, lanes 8 / 24 its up row
                 const float up = __shfl_xor_sync(0xffffffffu, v, 8);
@@ -321,14 +325,15 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
             } else if (EPI == ME_STORE) {
                 if ((lane & 7) == 0 && j < nv) ll_store(out + row, v, tag);
             } else if constexpr (SAMPLE) {         // ME_ARGMAX over the sampling keys (+ the raw record with LOGPROB)
-                if ((lane & 7) == 0 && j < nv) sample_fold<LOGPROB>(*dr, v, row, best_v, best_i, best_s, *smx, *ssel);
+                if ((lane & 7) == 0 && j < nv && rep_keep<REP>(rb, row, v))
+                    sample_fold<LOGPROB>(*dr, v, row, best_v, best_i, best_s, *smx, *ssel);
             } else if constexpr (LOGPROB) {        // ME_ARGMAX + running sum of exponentials (the lanes that keep best_v)
-                if ((lane & 7) == 0 && j < nv) {
+                if ((lane & 7) == 0 && j < nv && rep_keep<REP>(rb, row, v)) {
                     lse_fold(v, row, best_v, best_i, best_s);
                     if constexpr (TOPK) tk_insert(*tk, v, row);           // TOPK: + the lane's best TK_MAX rows
                 }
             } else {                               // ME_ARGMAX: rows arrive in increasing order per lane, strict > keeps the first maximum
-                if ((lane & 7) == 0 && j < nv && v > best_v) { best_v = v; best_i = row; }
+                if ((lane & 7) == 0 && j < nv && rep_keep<REP>(rb, row, v) && v > best_v) { best_v = v; best_i = row; }
             }
         }
         CF();
@@ -344,14 +349,17 @@ __device__ __forceinline__ void consume_quad(const Slice& s, const Ring& ring, u
 // Results are published as tagged words to `out` (ME_STORE), as self-validating words to `sxo` (ME_SWIGLU), or folded
 // into the running argmax (ME_ARGMAX; with LOGPROB also into the running sum of exponentials `best_s`, with TOPK also
 // into the sorted candidate list `*tk`; with SAMPLE the argmax is over the sampling keys of the draw `*dr`, and LOGPROB
-// keeps the raw (max `*smx`, sum `best_s`) record and the raw logit `*ssel` of the best-key row).
-template <int K, int EPI, bool LOGPROB = false, bool TOPK = false, bool SAMPLE = false>
+// keeps the raw (max `*smx`, sum `best_s`) record and the raw logit `*ssel` of the best-key row; with REP every logit is
+// first replaced by its processed value under the bit arrays `*rb`, common.cuh).
+template <int K, int EPI, bool LOGPROB = false, bool TOPK = false, bool SAMPLE = false, bool REP = false>
 __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32_t& q, const float* xs, uint2* out,
                                         uint32_t tag, uint32_t* sxo, float& best_v, int& best_i, float& best_s,
                                         const float* norm_w = nullptr, float norm_r = 1.f, long long* fine = nullptr,
-                                        TopK* tk = nullptr, const Draw* dr = nullptr, float* smx = nullptr, float* ssel = nullptr) {
+                                        TopK* tk = nullptr, const Draw* dr = nullptr, float* smx = nullptr, float* ssel = nullptr,
+                                        const RepBits* rb = nullptr) {
     if constexpr (K <= 1024) {
-        consume_quad<K, EPI, LOGPROB, TOPK, SAMPLE>(s, ring, q, xs, out, tag, sxo, best_v, best_i, best_s, norm_w, norm_r, fine, tk, dr, smx, ssel);
+        consume_quad<K, EPI, LOGPROB, TOPK, SAMPLE, REP>(s, ring, q, xs, out, tag, sxo, best_v, best_i, best_s, norm_w, norm_r, fine, tk,
+                                                         dr, smx, ssel, rb);
         return;
     }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -413,14 +421,14 @@ __device__ __forceinline__ void consume(const Slice& s, const Ring& ring, uint32
                 if (EPI == ME_STORE) {
                     if (act) ll_store(out + row, v0, tag);
                 } else if constexpr (SAMPLE) {
-                    if (act) sample_fold<LOGPROB>(*dr, v0, row, best_v, best_i, best_s, *smx, *ssel);
+                    if (act && rep_keep<REP>(rb, row, v0)) sample_fold<LOGPROB>(*dr, v0, row, best_v, best_i, best_s, *smx, *ssel);
                 } else if constexpr (LOGPROB) {
-                    if (act) {
+                    if (act && rep_keep<REP>(rb, row, v0)) {
                         lse_fold(v0, row, best_v, best_i, best_s);
                         if constexpr (TOPK) tk_insert(*tk, v0, row);
                     }
                 } else {
-                    if (act && v0 > best_v) { best_v = v0; best_i = row; }
+                    if (act && rep_keep<REP>(rb, row, v0) && v0 > best_v) { best_v = v0; best_i = row; }
                 }
             }
         }
@@ -543,7 +551,8 @@ __device__ __forceinline__ void head_norm_rope(const uint2* __restrict__ src, ui
 // warps and CTAs, and the last CTA records the step's candidates (p.tk_ids / p.tk_lp, or the EOS row)
 // SAMPLE: the lm_head folds the sampling keys of draw (p.row, n = *p.n_out) instead of the logits (common.cuh); with
 // LOGPROB the lanes, warps and CTAs also carry the raw (max, sum) record and the raw logit of the best-key row
-template <int H, int QD, int I, int NS, bool LOGPROB, bool TOPK = false, bool SAMPLE = false>
+// REP: every lm_head logit is replaced by its processed value (repetition controls, common.cuh) before any fold
+template <int H, int QD, int I, int NS, bool LOGPROB, bool TOPK = false, bool SAMPLE = false, bool REP = false>
 __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p) {
     constexpr int XS_FLOATS = (I > XS_MIN ? I : XS_MIN) + 64;
     extern __shared__ __align__(128) uint8_t smem[];
@@ -671,6 +680,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     const float* cs = ropes;
     const float* sn = ropes + half;
     const unsigned G = gridDim.x;
+    RepBits rb{};                                     // REP: this CTA's bits of its lm_head rows, built while layer 0's
+    if constexpr (REP) {                              // weights stream in (n_out changes only after every CTA's ticket)
+        const Slice sl = make_slice(nullptr, p.V, H, 1);
+        uint32_t* hist = p.rep_bits + (size_t)blockIdx.x * 2 * p.rep_words;
+        for (int i = tid; i < 2 * p.rep_words; i += NCONS) hist[i] = 0u;
+        cons_sync();
+        rep_mark(p.ids_out, min(__ldcg(p.n_out), p.max_new), __ldg(&p.rep->ngram), sl.r0, sl.r1, hist, hist + p.rep_words, tid, NCONS);
+        rb = RepBits{hist, hist + p.rep_words, sl.r0 >> 5, __ldg(&p.rep->theta)};
+    }
     float best_v = -INFINITY; int best_i = 0x7fffffff;
     float best_s = 0.f;                               // LOGPROB: sum of exp(logit - best_v) over the rows this lane folded
     static_assert(!TOPK || LOGPROB, "the candidates' log-probabilities need the sum of exponentials");
@@ -982,8 +1000,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     Draw dr{};
     float smx = -INFINITY, ssel = 0.f;                 // SLP: this lane's raw maximum logit, raw logit of its best-key row
     if constexpr (SAMPLE) dr = make_draw(p.smp, __ldcg(p.n_out), p.row);   // n_out changes only after every CTA's ticket
-    consume<H, ME_ARGMAX, LOGPROB, TOPK, SAMPLE>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i,
-                                                 best_s, pbuf + (p.L & 1) * PARAM_FLOATS, nrf, nullptr, &tk, &dr, &smx, &ssel);
+    consume<H, ME_ARGMAX, LOGPROB, TOPK, SAMPLE, REP>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i,
+                                                      best_s, pbuf + (p.L & 1) * PARAM_FLOATS, nrf, nullptr, &tk, &dr, &smx, &ssel, &rb);
     MEGA_MARK();
     // candidates live in lanes 0, 8, 16, 24 of every warp (the four rows of a turn; lanes 0 / 16 in the two-row form):
     // merge them, lane 0 publishes the warp's best
@@ -1162,6 +1180,22 @@ size_t decode_mega_sx_bytes(const Model& m) {
     return 2 * (size_t)c.num_hidden_layers * (2 * (size_t)c.hidden_size + m.d.q_dim + c.intermediate_size) * sizeof(uint32_t);
 }
 
+// the instantiation for the model's dims and the run's options: sampling (with or without the log-probability record)
+// is never combined with the candidate lists
+template <bool LP, bool TK, bool SM, bool RP>
+static const void* step_fn_dims(const asrb_dims& c) {
+    if (dims_match<1024, 2048, 3072>(c)) return (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, LP, TK, SM, RP>;   // Qwen3-ASR-0.6B
+    if (dims_match<2048, 2048, 6144>(c)) return (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, LP, TK, SM, RP>;   // Qwen3-ASR-1.7B
+    return (const void*)mega::decode_step_kernel<256, 512, 512, 6, LP, TK, SM, RP>;                                           // test config
+}
+template <bool RP>
+static const void* step_fn(const DecodeBufs& b, const asrb_dims& c) {
+    if (b.sample) return b.logprobs ? step_fn_dims<true, false, true, RP>(c) : step_fn_dims<false, false, true, RP>(c);
+    if (b.topk) return step_fn_dims<true, true, false, RP>(c);
+    if (b.logprobs) return step_fn_dims<true, false, false, RP>(c);
+    return step_fn_dims<false, false, false, RP>(c);
+}
+
 void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* kcache, float* vcache,
                              size_t cache_layer_stride, size_t cache_seq_stride, int max_ctx, int ctx_now, const MegaBufs& mb,
                              cudaStream_t st, int64_t* launches) {
@@ -1173,31 +1207,7 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
     // split count is fixed per session (buffer layout); splits beyond the current context are simply empty
     const int nsplit = std::min(mega::MAX_SPLITS, std::min(G / c.num_key_value_heads, (max_ctx + mega::KV_KEYS - 1) / mega::KV_KEYS));
     const size_t smem = mega_smem_bytes(c.hidden_size, c.intermediate_size, mega_nslot(c));
-    const void* fn = nullptr;
-    if (b.sample) {         // with or without the log-probability record; never with the candidate lists
-        if (b.logprobs) {
-            if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, true, false, true>;
-            else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, true, false, true>;
-            else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, true, false, true>;
-        } else {
-            if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, false, false, true>;
-            else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, false, false, true>;
-            else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, false, false, true>;
-        }
-    }
-    else if (b.topk) {
-        if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, true, true>;
-        else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, true, true>;
-        else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, true, true>;
-    }
-    else if (b.logprobs) {
-        if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, true>;
-        else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, true>;
-        else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, true>;
-    }
-    else if (dims_match<1024, 2048, 3072>(c)) fn = (const void*)mega::decode_step_kernel<1024, 2048, 3072, 6, false>;   // Qwen3-ASR-0.6B
-    else if (dims_match<2048, 2048, 6144>(c)) fn = (const void*)mega::decode_step_kernel<2048, 2048, 6144, 5, false>;   // Qwen3-ASR-1.7B
-    else fn = (const void*)mega::decode_step_kernel<256, 512, 512, 6, false>;                                           // test config
+    const void* fn = b.rep ? step_fn<true>(b, c) : step_fn<false>(b, c);
     ASRB_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // The kernel handles one sequence.  A batch runs as B launches on the stream (weights are re-streamed per sequence:
     // 2.0 k tokens/s at any batch size, still ~1.8x the per-phase path at batch 8); a sequence that has finished
@@ -1232,6 +1242,7 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
             p.smp = b.smp; p.row = sb;
             if (b.logprobs) { p.part_max = b.part_max; p.part_sel = b.part_sel; }
         }
+        if (b.rep) { p.rep_bits = b.rep_mask; p.rep_words = rep_cta_words(c, G); p.rep = b.rep_params; }
         // tags must stay monotonic for red.max publication: long before the 24-bit epoch wraps, wipe the tagged exchange
         // buffers (the self-validating words live elsewhere and are left alone: to them 0 would be a published 0.0)
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {

@@ -213,7 +213,18 @@ struct DecodeBufs {
     const SampleParams* smp;  // device: 1 / temperature and the seed of the current run
     float* part_max;          // [B][n_part] sampling with logprobs: raw maximum logit per argmax partial (part_val holds keys)
     float* part_sel;          // [B][n_part] raw logit of each partial's best-key row (allocated when first needed)
+    // repetition controls (session options "no_repeat_ngram_size" / "repetition_penalty", latched at the prefill): the
+    // REP kernel variants fold the processed logits.  The fused steps build their bit arrays themselves; before a
+    // per-phase step launch_rep_mask builds each sequence's over the whole vocabulary
+    bool rep;                     // the REP kernel variants
+    const RepParams* rep_params;  // device: the penalty and N of the current run
+    uint32_t* rep_mask;           // per-phase: [B][2][rep_words] bits; fused steps: [G][sequences][2][rep_cta_words]
+    int rep_words;                // (vocab + 31) / 32
 };
+void launch_rep_mask(const DecodeBufs& b, int R, cudaStream_t st, int64_t* launches);
+// words of one repetition bit array covering a fused step CTA's lm_head rows (a contiguous range of at most
+// ceil(vocab / G) rows, which may start mid-word)
+inline int rep_cta_words(const asrb_dims& c, int G) { return ((c.vocab_size + G - 1) / G + 31) / 32 + 1; }
 void launch_decode_step_phases(const Model& m, const DecodeBufs& b, int B, float* kcache, float* vcache,
                                size_t cache_layer_stride, size_t cache_seq_stride, int max_ctx,
                                bool write_logits, cudaStream_t st, int64_t* launches);

@@ -87,6 +87,10 @@ struct Session {
     // and the device-resident db.smp, so they apply to the whole run
     double temperature = 0.0; uint64_t seed = 0;
     SampleParams* d_smp = nullptr;
+    // repetition controls: options "no_repeat_ngram_size" (0 = off) and "repetition_penalty" (1 = off), latched at the
+    // prefill into db.rep and the device-resident db.rep_params, so they apply to the whole run
+    int ngram = 0; double rep_penalty = 1.0;
+    RepParams* d_rep = nullptr;
     // beam search: options "beam_size" (1 = greedy) and "length_penalty" (< 0: none), latched at the prefill into run_k /
     // run_alpha.  A beam run decodes nslots = B * run_k slots; B stays the number of utterances.
     int beam_k = 1, run_k = 1, nslots = 0;
@@ -219,6 +223,8 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
         b.max_new = max_new;
         s->d_smp = salloc<SampleParams>(s, 1, true);
         b.smp = s->d_smp;
+        s->d_rep = salloc<RepParams>(s, 1, true);
+        b.rep_params = s->d_rep; b.rep_words = (c.vocab_size + 31) / 32;   // per-phase bit arrays: the whole vocabulary
         s->d_lastrow = salloc<int>(s, Bm);
         s->mega.bar = salloc<unsigned>(s, 4, true);
         { const unsigned one = 1; ASRB_CUDA_CHECK(cudaMemcpy(s->mega.bar + 1, &one, sizeof(one), cudaMemcpyHostToDevice)); }   // epoch 1
@@ -702,6 +708,7 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
         ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_smp, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
         ensure_sample_bufs(s);
     }
+    s->db.rep = false;                     // token 0 has no history: the prefill's lm_head folds the raw logits
     s->tk_valid = s->top_k;
     if (s->db.topk) {                      // ids -1, values NaN (0xFFFFFFFF): nothing recorded yet
         const size_t rows = (size_t)B * s->max_new * TK_MAX;
@@ -751,6 +758,14 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     // beam search: the token-0 walk on each utterance's record, then its prompt KV copied into its other K - 1 slots
     if (s->run_k > 1) launch_beam_step(beam_args(s), true, di + (pos0 - hi), st, &s->launches);
     s->greedy_done = 1;
+    s->db.rep = s->ngram > 0 || s->rep_penalty != 1.0;   // latched: every decode step of the run applies this run's rule
+    if (s->db.rep) {
+        const RepParams hp{(float)s->rep_penalty, s->ngram};
+        ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_rep, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
+        if (!s->db.rep_mask)                // per-phase: [max_batch][2][vocab words]; fused steps: [G][up to 16][2][CTA words]
+            s->db.rep_mask = salloc<uint32_t>(s, std::max((size_t)s->max_batch * 2 * s->db.rep_words,
+                                                          (size_t)m.ctx->sm_count * 16 * 2 * rep_cta_words(c, m.ctx->sm_count)));
+    }
     if (seq_lens_out) for (int b = 0; b < B; ++b) seq_lens_out[b] = s->S[b];
     if (last_logits) {
         ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -800,6 +815,7 @@ static void forward_step(Session* s, bool write_logits) {
         s->n_mega_steps += 1;
     } else {
         s->n_phase_steps += 1;
+        if (s->db.rep) launch_rep_mask(s->db, R, s->st, &s->launches);     // the fused steps build their own bits
         launch_decode_step_phases(m, s->db, R, s->kcache, s->vcache, s->cache_layer_stride, s->cache_seq_stride, s->max_ctx,
                                   write_logits, s->st, &s->launches);
         launch_greedy(m, s->db, R, s->st, &s->launches);
@@ -880,7 +896,7 @@ void session_generate(Session* s, int max_new_tokens, int32_t* ids_out, int32_t*
     // (inference.rs:160-200); that wasted forward is not issued here.
     const int steps = std::max(0, max_new_tokens - s->greedy_done);
     auto ensure_graph = [&]() {   // per-phase path: ~142 launches per step -> replay them as one CUDA graph
-        const int mode_key = ((((int)s->db.sample * 2 + (int)s->db.topk) * 2 + (int)s->db.logprobs) * 2 + s->decode_mode) * (s->max_batch + 1) + R;   // unique per (sample, topk, logprobs, mode, decode rows)
+        const int mode_key = (((((int)s->db.rep * 2 + (int)s->db.sample) * 2 + (int)s->db.topk) * 2 + (int)s->db.logprobs) * 2 + s->decode_mode) * (s->max_batch + 1) + R;   // unique per (rep, sample, topk, logprobs, mode, decode rows)
         if (s->step_graph == nullptr || s->graph_mode != mode_key) {
             if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
             cudaGraph_t g = nullptr;
@@ -1123,6 +1139,25 @@ static double parse_length_penalty(const std::string& v) {     // "none" is hand
                  "length_penalty must be none or a decimal in [0, 10]");
     return a;
 }
+// repetition controls: N a decimal integer in 0..16; the penalty a decimal in [1, 10], parsed in double
+static int parse_ngram(const std::string& v) {
+    ASRB_REQUIRE(!v.empty() && v.size() <= 2 && v.find_first_not_of("0123456789") == std::string::npos, ASRB_ERR_INVALID,
+                 "no_repeat_ngram_size must be 0..16");
+    const int n = atoi(v.c_str());
+    ASRB_REQUIRE(n >= 0 && n <= 16, ASRB_ERR_INVALID, "no_repeat_ngram_size must be 0..16");
+    return n;
+}
+static double parse_rep_penalty(const std::string& v) {
+    ASRB_REQUIRE(!v.empty() && (isdigit((unsigned char)v[0]) || v[0] == '.') &&
+                 v.find_first_not_of("0123456789.eE+-") == std::string::npos,
+                 ASRB_ERR_INVALID, "repetition_penalty must be a decimal number");   // no sign, space, hex, inf or nan
+    errno = 0;
+    char* end = nullptr;
+    const double t = strtod(v.c_str(), &end);
+    ASRB_REQUIRE(end && *end == '\0' && errno == 0 && std::isfinite(t) && t >= 1.0 && t <= 10.0, ASRB_ERR_INVALID,
+                 "repetition_penalty must be a decimal in [1, 10]");
+    return t;
+}
 static uint64_t parse_seed(const std::string& v) {
     ASRB_REQUIRE(!v.empty() && isdigit((unsigned char)v[0]), ASRB_ERR_INVALID, "seed must be a decimal unsigned 64-bit integer");
     errno = 0;
@@ -1167,6 +1202,10 @@ void session_set_option(Session* s, const char* key, const char* value) {
         apply_record_options(s);
     } else if (k == "length_penalty") {
         s->length_penalty = v == "none" ? -1.0 : parse_length_penalty(v);
+    } else if (k == "no_repeat_ngram_size") {
+        s->ngram = parse_ngram(v);
+    } else if (k == "repetition_penalty") {
+        s->rep_penalty = parse_rep_penalty(v);
     } else throw Error(ASRB_ERR_INVALID, "unknown option: " + k);
 }
 

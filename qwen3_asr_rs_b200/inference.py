@@ -93,6 +93,24 @@ def check_beam(beam_size, length_penalty) -> Tuple[int, Optional[float]]:
     return int(beam_size), length_penalty
 
 
+def check_repetition(no_repeat_ngram_size, repetition_penalty) -> Tuple[int, float]:
+    """The `no_repeat_ngram_size` (an int in 0..16; 0: off) and `repetition_penalty` (a finite value in [1, 10]; 1: off)
+    arguments, validated."""
+    n = no_repeat_ngram_size
+    if not isinstance(n, (int, np.integer)) or isinstance(n, bool) or not 0 <= n <= 16:
+        raise ValueError(f"no_repeat_ngram_size must be an int in 0..16, got {n!r}")
+    p = repetition_penalty
+    if isinstance(p, bool) or not isinstance(p, (int, float, np.integer, np.floating)) or not math.isfinite(float(p)) \
+            or not 1.0 <= float(p) <= 10.0:
+        raise ValueError(f"repetition_penalty must be a finite value in [1, 10], got {p!r}")
+    return int(n), float(p)
+
+
+def repetition_penalty_option(p: float) -> str:
+    """The session option string of a repetition penalty: repr round-trips the double exactly."""
+    return "1" if p == 1.0 else repr(float(p))
+
+
 def length_penalty_option(a: Optional[float]) -> str:
     """The session option string of length penalty a (None: "none")."""
     return "none" if a is None else repr(float(a))
@@ -574,6 +592,17 @@ class AsrInference:
                 undo.append((key, conf))
         return undo
 
+    # ---- repetition controls (session options "no_repeat_ngram_size" / "repetition_penalty") ------------------
+    def _set_repetition(self, s, rep: Tuple[int, float]) -> List[Tuple[str, str]]:
+        """Set N and the penalty for one call; returns the (option, configured value) pairs to restore."""
+        undo = []
+        for key, val in (("no_repeat_ngram_size", str(rep[0])), ("repetition_penalty", repetition_penalty_option(rep[1]))):
+            conf = self._options.get(key, {"no_repeat_ngram_size": "0", "repetition_penalty": "1"}[key])
+            if conf != val:
+                _lib.check(self._lib.asrb_session_set_option(s, key.encode(), val.encode()))
+                undo.append((key, conf))
+        return undo
+
     def _restore(self, s, undo) -> None:
         for key, conf in undo:
             _lib.check(self._lib.asrb_session_set_option(s, key.encode(), conf.encode()))
@@ -621,7 +650,8 @@ class AsrInference:
                        max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0,
                        temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
                        logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
-                       length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None) -> TranscribeIds:
+                       length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None,
+                       no_repeat_ngram_size: int = 0, repetition_penalty: float = 1.0) -> TranscribeIds:
         """transcribe() steps 2-8 for a batch: host f32 samples in, host token ids out (and, with `logprobs`, the
         log-probability of every id and of the ending EOS, from the kernels that selected them; with `top_logprobs` = k
         in 1..8, also the k best candidates of each of those steps, and the log-probabilities as with `logprobs`).
@@ -631,19 +661,23 @@ class AsrInference:
         `beam_size` K in 2..6 decodes every utterance with beam search (the session holds batch x K slots; `nbest`
         holds the K ranked hypotheses, `ids` the best) scored with `length_penalty` (None: sum / length); with a
         schedule, only the attempts at t = 0 use it.  `context_ids`: None, or per utterance None or the token ids of
-        its context, placed in the prompt's system turn; utterances with identical contexts share its prefill."""
+        its context, placed in the prompt's system turn; utterances with identical contexts share its prefill.
+        `no_repeat_ngram_size` N >= 1 bans every id that would repeat an N-gram of the ids generated so far, and
+        `repetition_penalty` > 1 divides the positive (multiplies the negative) logits of ids generated so far, in every
+        attempt, beam and path (include/asr_b200.h); the prompt and context never count."""
         ctx = check_context_ids(context_ids, len(clips), self.config.text.vocab_size)
+        rep = check_repetition(no_repeat_ngram_size, repetition_penalty)
 
         def once(idx, lp, k, t, beam):
             sub = clips if len(idx) == len(clips) else [clips[i] for i in idx]
             lang = None if language_ids is None else [language_ids[i] for i in idx]
             return self._ids_once(sub, lang, max_new_tokens, lp, k, t, seed, beam,
-                                  None if ctx is None else [ctx[i] for i in idx])
+                                  None if ctx is None else [ctx[i] for i in idx], rep)
         return self._sampled(len(clips), once, temperature, seed, logprob_threshold, logprobs, top_logprobs,
                              beam_size, length_penalty)
 
     def _ids_once(self, clips, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
-                  temperature: Optional[float], seed: int, beam=None, context_ids=None) -> TranscribeIds:
+                  temperature: Optional[float], seed: int, beam=None, context_ids=None, rep=(0, 1.0)) -> TranscribeIds:
         B = len(clips)
         K = beam[0] if beam else 1
         arrs, ptrs, lens = self._pack_samples(clips)
@@ -651,12 +685,12 @@ class AsrInference:
         s = self._ensure_session(B * K, max(a.shape[0] for a in arrs), mx, max_new_tokens, _max_len(context_ids))
         return self._run(s, B, max_new_tokens, logprobs, top_logprobs, temperature, seed, beam, context_ids,
                          lambda ids, n: self._lib.asrb_transcribe_ids(s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
-                                                                      ids, n))
+                                                                      ids, n), rep)
 
     def _run(self, s, B: int, max_new_tokens: int, logprobs: bool, top_logprobs: int, temperature: Optional[float],
-             seed: int, beam, context_ids, call) -> TranscribeIds:
+             seed: int, beam, context_ids, call, rep=(0, 1.0)) -> TranscribeIds:
         """One decode call on session s with this call's options set and restored around it: `call(ids_out, lens_out)`
-        runs the library's transcribe entry point for B utterances and returns its status."""
+        runs the library's transcribe entry point for B utterances and returns its status; `rep` = (N, penalty)."""
         K = beam[0] if beam else 1
         ids = np.zeros((B, max_new_tokens), dtype=np.int32)
         n = np.zeros(B, dtype=np.int32)
@@ -668,6 +702,7 @@ class AsrInference:
         try:
             undo = self._set_sampling(s, temperature, seed)
             undo += self._set_beam(s, K, beam[1] if beam else None)
+            undo += self._set_repetition(s, rep)
             if context_ids is not None:
                 self._set_context(s, context_ids)
             _lib.check(call(ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
@@ -716,28 +751,31 @@ class AsrInference:
                        max_new_tokens: int = MAX_NEW_TOKENS, logprobs: bool = False, top_logprobs: int = 0,
                        temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
                        logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
-                       length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None) -> TranscribeIds:
+                       length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None,
+                       no_repeat_ngram_size: int = 0, repetition_penalty: float = 1.0) -> TranscribeIds:
         """transcribe() steps 1-8 for a batch with step 1 on the GPU: raw PCM in, token ids out (`logprobs`,
-        `top_logprobs`, `temperature`, `seed`, `logprob_threshold`, `beam_size`, `length_penalty`, `context_ids`: as
-        in transcribe_ids)."""
+        `top_logprobs`, `temperature`, `seed`, `logprob_threshold`, `beam_size`, `length_penalty`, `context_ids`,
+        `no_repeat_ngram_size`, `repetition_penalty`: as in transcribe_ids)."""
         ctx = check_context_ids(context_ids, len(pcms), self.config.text.vocab_size)
+        rep = check_repetition(no_repeat_ngram_size, repetition_penalty)
 
         def once(idx, lp, k, t, beam):
             sel = (lambda xs: xs if len(idx) == len(pcms) else [xs[i] for i in idx])
             lang = None if language_ids is None else sel(language_ids)
             return self._pcm_once(sel(pcms), sel(rates), lang, max_new_tokens, lp, k, t, seed, beam,
-                                  None if ctx is None else sel(ctx))
+                                  None if ctx is None else sel(ctx), rep)
         return self._sampled(len(pcms), once, temperature, seed, logprob_threshold, logprobs, top_logprobs,
                              beam_size, length_penalty)
 
     def _pcm_once(self, pcms, rates, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
-                  temperature: Optional[float], seed: int, beam=None, context_ids=None) -> TranscribeIds:
+                  temperature: Optional[float], seed: int, beam=None, context_ids=None, rep=(0, 1.0)) -> TranscribeIds:
         B = len(pcms)
         K = beam[0] if beam else 1
         keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
         s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens, slots=B * K, max_context=_max_len(context_ids))
         return self._run(s, B, max_new_tokens, logprobs, top_logprobs, temperature, seed, beam, context_ids,
-                         lambda ids, n: self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens), ids, n))
+                         lambda ids, n: self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens), ids, n),
+                         rep)
 
     # ---- long-form audio: cut at low-energy points on the GPU, decode the pieces in waves -----------------------
     def ingest_long(self, pcms: Sequence, rates: Sequence[int]) -> List[np.ndarray]:
@@ -789,7 +827,8 @@ class AsrInference:
                         logprobs: bool = False, top_logprobs: int = 0,
                         temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
                         logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
-                        length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None) -> "LongResult":
+                        length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None,
+                        no_repeat_ngram_size: int = 0, repetition_penalty: float = 1.0) -> "LongResult":
         """Long recordings: ingest the files (raw PCM, as transcribe_pcm) into the long-audio buffer, cut them on the GPU
         into segments of at most `max_segment_s` at the quietest 100 ms window of the last `search_s` before each limit
         (asrb_segment_long), and decode the segments as views of that buffer (asrb_transcribe_segments) in waves of
@@ -807,6 +846,7 @@ class AsrInference:
         check_temperature(temperature)
         check_seed(seed)
         K, _ = check_beam(beam_size, length_penalty)
+        rep = check_repetition(no_repeat_ngram_size, repetition_penalty)
         if batch // K < 1:
             raise ValueError(f"batch ({batch}) must be >= beam_size ({K})")
         ctx = check_context_ids(context_ids, n_files, self.config.text.vocab_size)
@@ -836,7 +876,7 @@ class AsrInference:
                 wctx = None if ctx is None else [ctx[x[0]] for x in wave]
                 runs.append(self._run(s, m, max_new_tokens, lp, k, t, seed, beam, wctx,
                                       lambda ids, nn: self._lib.asrb_transcribe_segments(
-                                          s, m, fl, st, en, lptrs, llens, int(max_new_tokens), ids, nn)))
+                                          s, m, fl, st, en, lptrs, llens, int(max_new_tokens), ids, nn), rep))
                 self._long_waves += 1
             return _concat_runs(runs)
         r = self._sampled(len(segs), once, temperature, seed, logprob_threshold, logprobs, tk, beam_size, length_penalty)
@@ -859,12 +899,14 @@ class AsrInference:
                    top_logprobs: int = 0, temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
                    logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
                    length_penalty: Optional[float] = None, context: Optional[str] = None,
-                   max_segment_s: Optional[float] = None) -> TranscribeResult:
+                   max_segment_s: Optional[float] = None, no_repeat_ngram_size: int = 0,
+                   repetition_penalty: float = 1.0) -> TranscribeResult:
         """AsrInference::transcribe (inference.rs:89-213): step 1 (WAV payload -> mono 16 kHz; on the GPU by default,
         `gpu_ingest=False` = the host loader) -> steps 2-8 on the GPU -> step 9 (detokenise + parse, host; needs
         tokenizer.json, else raw_output is the id list as text).  `logprobs`: also fill token_logprobs / avg_logprob;
         `top_logprobs` = k in 1..8: also fill top_logprobs (and token_logprobs / avg_logprob); `temperature`, `seed`,
-        `logprob_threshold`, `beam_size`, `length_penalty`: as in transcribe_ids, and `temperature` of the result is that
+        `logprob_threshold`, `beam_size`, `length_penalty`, `no_repeat_ngram_size`, `repetition_penalty`: as in
+        transcribe_ids, and `temperature` of the result is that
         of the kept attempt; `nbest` holds the beam's hypotheses as (text, score).  `context`: text placed in the prompt's
         system turn to bias recognition (keywords, names, related text; needs tokenizer.json; "" = none).
         `max_segment_s`: None decodes the file in one pass; a number of seconds runs transcribe_long with it (search
@@ -874,7 +916,8 @@ class AsrInference:
         lang_ids = language_prompt_ids(self.tokenizer, language)
         ctx_ids = context_prompt_ids(self.tokenizer, context)
         sampling = dict(temperature=temperature, seed=seed, logprob_threshold=logprob_threshold, beam_size=beam_size,
-                        length_penalty=length_penalty, context_ids=[ctx_ids] if ctx_ids else None)
+                        length_penalty=length_penalty, context_ids=[ctx_ids] if ctx_ids else None,
+                        no_repeat_ngram_size=no_repeat_ngram_size, repetition_penalty=repetition_penalty)
         if max_segment_s is not None:
             if gpu_ingest:
                 pcm, rate = read_wav_pcm(audio_path)

@@ -177,6 +177,32 @@ impl B200Engine {
         run
     }
 
+    /// `transcribe_ids` with the repetition controls, the options "no_repeat_ngram_size" / "repetition_penalty"
+    /// (`include/asr_b200.h`): `no_repeat_ngram_size` N in 0..=16 (0: off) bans every id that would repeat an N-gram of
+    /// the ids generated so far, `repetition_penalty` in [1, 10] (1: off) divides the positive and multiplies the negative
+    /// logits of those ids.  The options are set for this call and restored to off afterwards.
+    pub fn transcribe_ids_no_repeat(&self, samples: &[f32], lang_ids: Option<&[i64]>, no_repeat_ngram_size: u32,
+                                    repetition_penalty: f64) -> Result<Vec<i64>> {
+        if no_repeat_ngram_size > 16 { return Err(anyhow!("no_repeat_ngram_size must be in 0..=16, got {no_repeat_ngram_size}")); }
+        if !(1.0..=10.0).contains(&repetition_penalty) {
+            return Err(anyhow!("repetition_penalty must be in [1, 10], got {repetition_penalty}"));
+        }
+        let session = self.session_for(samples.len())?;
+        let nkey = CString::new("no_repeat_ngram_size")?;
+        let pkey = CString::new("repetition_penalty")?;
+        let nval = CString::new(no_repeat_ngram_size.to_string())?;
+        let pval = CString::new(format!("{repetition_penalty:?}"))?;
+        let (zero, one) = (CString::new("0")?, CString::new("1")?);
+        let set = (|| -> Result<()> {
+            check(unsafe { ffi::asrb_session_set_option(session, nkey.as_ptr(), nval.as_ptr()) })?;
+            check(unsafe { ffi::asrb_session_set_option(session, pkey.as_ptr(), pval.as_ptr()) })
+        })();
+        let run = set.and_then(|_| self.transcribe_ids(samples, lang_ids));
+        check(unsafe { ffi::asrb_session_set_option(session, nkey.as_ptr(), zero.as_ptr()) })?;
+        check(unsafe { ffi::asrb_session_set_option(session, pkey.as_ptr(), one.as_ptr()) })?;
+        run
+    }
+
     /// `transcribe_ids` with context biasing: `context_ids` (the tokenizer's ids of a keyword list, names or related
     /// text) become the content of the prompt's system turn (`asrb_session_set_context`).  An empty slice is the plain
     /// prompt.  The context is cleared again after the call.
