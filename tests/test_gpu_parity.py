@@ -195,8 +195,8 @@ def test_full_size_0p6b_one_clip(report):
 
 def test_full_size_1p7b_short_clip(report):
     """Qwen3-ASR-1.7B dims (BASELINE.json configs[3] model; dims as recalled in SURVEY.md section 8), one 10 s clip,
-    synthetic weights: exact ids + logits tolerance.  These dims are outside the fused decode step's table, so this
-    also covers the per-phase decode path at full size."""
+    synthetic weights: exact ids + logits tolerance.  The 6 ids run on the fused single-sequence step's 1.7B
+    instantiation; the per-phase path at 1.7B widths is covered by tests/test_decode_variants_fp64.py."""
     from qwen3_asr_rs_b200 import AsrInference, config_1p7b
     cfg = O.cfg_1p7b()
     w = synth.make_weights(cfg, 3)
@@ -243,8 +243,9 @@ def test_model_load_from_directory(tiny, tmp_path, shards):
 
 
 def test_token_ids_batch_larger_than_8(tiny, tiny_engine):
-    """batch > 8: the per-phase decode path walks sub-batches of 8 sequences; utterances stay independent
-    (the reference is batch-1, so batch semantics == B independent runs of it)."""
+    """batch 11: the batched fused step at NB = 16 (the per-phase path's sub-batches of 8 are covered by
+    tests/test_decode_variants_fp64.py); utterances stay independent (the reference is batch-1, so batch semantics ==
+    B independent runs of it)."""
     _, _, model = tiny
     secs = [1.1, 2.3, 0.7, 4.9, 3.1, 1.9, 2.2, 0.9, 5.3, 1.4, 2.8]
     clips = [synth.make_clip(200 + i, s) for i, s in enumerate(secs)]

@@ -334,14 +334,27 @@ def test_shared_context_prefill(tiny, tiny64, eng, report):
 
 
 # ---- fused decode records ------------------------------------------------------------------------------------------
-def record_errs(m32, m64, clips, r, top: bool):
+def _processed_log_softmax(logits, ids, rep):
+    """log_softmax of every row of score_ids([T + 1, V], float64); with rep = (N, theta) != (0, 1), row t first processed
+    by the repetition controls with history ids[:t] (test_repetition.process)."""
+    if rep == (0, 1.0):
+        return torch.log_softmax(logits, -1).numpy()
+    from test_repetition import process
+    l = logits.numpy()
+    return torch.log_softmax(torch.from_numpy(np.stack([process(l[t], ids[:t], *rep) for t in range(len(l))])), -1).numpy()
+
+
+def record_errs(m32, m64, clips, r, top: bool, rep=(0, 1.0), seqs=None, scores=None):
     """Err of the recorded log-probabilities against log_softmax of score_ids at the GPU's own ids: with `top`, every
-    entry (id, lp) of every top-k row, EOS step included; else the log-probability of each id and of the ending EOS."""
+    entry (id, lp) of every top-k row, EOS step included; else the log-probability of each id and of the ending EOS.
+    rep = (no_repeat_ngram_size, repetition_penalty): against the processed logits.  `seqs`: the sequences checked (all
+    by default); `scores(b, ids)`: (fp32, fp64) score_ids of sequence b, for a caller that caches them."""
     err = Err(False)
-    for b, x in enumerate(clips):
-        ids = r.ids[b]
-        l32 = torch.log_softmax(O.score_ids(m32, x, ids).double(), -1).numpy()
-        l64 = torch.log_softmax(O.score_ids(m64, x, ids), -1).numpy()
+    for b in range(len(clips)) if seqs is None else seqs:
+        x, ids = clips[b], r.ids[b]
+        s32, s64 = scores(b, ids) if scores else (O.score_ids(m32, x, ids), O.score_ids(m64, x, ids))
+        l32 = _processed_log_softmax(s32.double(), ids, rep)
+        l64 = _processed_log_softmax(s64, ids, rep)
         if top:
             rows = list(r.top_logprobs[b]) + ([r.eos_top_logprobs[b]] if r.eos_top_logprobs[b] is not None else [])
             assert len(rows) >= len(ids) and all(row[0][0] == t for row, t in zip(rows, ids))
