@@ -204,7 +204,10 @@ ASRB_API int asrb_session_device_ids(asrb_session* s, const int32_t** ids_dev, c
  *   [0] decoder forwards on the batch-aware fused step   [1] on the single-sequence fused step
  *   [2] on the per-phase kernels (fallback: logits requested, unsupported dims, context beyond the fused limit)
  *   [3] GEMMs that fell back from wgmma to the SIMT kernel (process-wide)   [4] wgmma GEMM launches (process-wide)
- * writes min(n, 5) values */
+ *   greedy single-sequence fused step, lm_head read from its int8 copy (DESIGN.md section 4.1):
+ *   [5] rows recomputed from bf16 as candidates for the argmax   [6] most rows recomputed in one step
+ *   [7] CTA slices recomputed in full (candidate list overflow or a non-finite bound)
+ * writes min(n, 8) values (n > 5 waits for the session's stream) */
 ASRB_API int asrb_session_stats(asrb_session* s, int64_t* out, int n);
 /* knobs: "gemm" = "tc"|"simt", "decode" = "mega"|"phases", "batch_step" = "1"|"0", "planes" = "1"|"2"|"3",
  * "resident" = "1"|"0" (1: the samples uploaded by the previous call are reused, no H2D),

@@ -26,6 +26,8 @@
 //     embedding of the next token), so there is no host sync and no extra launch per token.
 // Reference semantics per phase: see decode.cu.  The kernel advances ONE sequence; a batch is B back-to-back launches
 // (decode.cu remains the path for logits output, other model dimensions and contexts beyond 1152 keys).
+#include <cfloat>
+#include <climits>
 #include "mega_common.cuh"
 
 namespace asrb {
@@ -67,6 +69,10 @@ struct Params {
     uint32_t* rep_bits;          // [gridDim.x][2][rep_words] each CTA's history / banned bits of its lm_head rows
     int rep_words;
     const RepParams* rep;        // the run's penalty and N
+    // default (greedy) instantiations only (appended as well): the lm_head streams from its int8 copy
+    const int8_t* lm_head_q;     // [V][H]
+    const float2* lm_head_sc;    // [V] {scale s_r, bound constant C_r} (model.cu quantize_head_kernel)
+    unsigned long long* hq_stats;   // [0] rows recomputed in this step, [1] in all steps, [2] most in one step, [3] fallbacks
 };
 
 static_assert(KV_KEYS * HD * 4 == SLOT_BYTES, "K / V tiles travel through the weight ring: one tile per slot");
@@ -184,6 +190,149 @@ __device__ __forceinline__ float row_dot4(const uint4* w0, const uint4* w1, cons
 #pragma unroll
     for (int o = 4; o > 0; o >>= 1) keep += __shfl_xor_sync(0xffffffffu, keep, o);
     return keep;
+}
+
+// 4 int8 weights (one word, element 0 in the low byte) -> 4 exact floats: byte b + 128 becomes the low mantissa byte of
+// 2^23, and 2^23 + 128 is subtracted (one PRMT and one FADD per element instead of a quarter-rate I2F)
+__device__ __forceinline__ void i8x4_f32(uint32_t w, float (&f)[4]) {
+    const uint32_t u = w ^ 0x80808080u;
+    f[0] = __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7540)) - 8388736.f;
+    f[1] = __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7541)) - 8388736.f;
+    f[2] = __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7542)) - 8388736.f;
+    f[3] = __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7543)) - 8388736.f;
+}
+// sum_i q_i x_i of four int8 rows (8 bytes per lane and 256-element chunk, the elements of row_dot4's lane mapping), with
+// row_dot4's structure: two FMA chains of K / 64 terms per lane and row, one add, a 5-level butterfly.  The total of row j
+// ends up in the lanes with (lane >> 3) == j.
+template <int K>
+__device__ __forceinline__ float row_dot4_q(const uint2* w0, const uint2* w1, const uint2* w2, const uint2* w3,
+                                            const float (&xr)[K / 32], int lane) {
+    float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f, c0 = 0.f, c1 = 0.f, d0 = 0.f, d1 = 0.f;
+#pragma unroll
+    for (int c = 0; c < K / 256; ++c) {
+        const uint2 wa = w0[c * 32 + lane], wb = w1[c * 32 + lane], wc = w2[c * 32 + lane], wd = w3[c * 32 + lane];
+        float fa[4], fb[4], fc[4], fd[4];
+#define ROWQ_STEP(F, O)                                                                                               \
+        i8x4_f32(wa.F, fa); i8x4_f32(wb.F, fb); i8x4_f32(wc.F, fc); i8x4_f32(wd.F, fd);                               \
+        a0 = fmaf(fa[0], xr[c * 8 + O], a0); a1 = fmaf(fa[1], xr[c * 8 + O + 1], a1);                                 \
+        b0 = fmaf(fb[0], xr[c * 8 + O], b0); b1 = fmaf(fb[1], xr[c * 8 + O + 1], b1);                                 \
+        c0 = fmaf(fc[0], xr[c * 8 + O], c0); c1 = fmaf(fc[1], xr[c * 8 + O + 1], c1);                                 \
+        d0 = fmaf(fd[0], xr[c * 8 + O], d0); d1 = fmaf(fd[1], xr[c * 8 + O + 1], d1);                                 \
+        a0 = fmaf(fa[2], xr[c * 8 + O + 2], a0); a1 = fmaf(fa[3], xr[c * 8 + O + 3], a1);                             \
+        b0 = fmaf(fb[2], xr[c * 8 + O + 2], b0); b1 = fmaf(fb[3], xr[c * 8 + O + 3], b1);                             \
+        c0 = fmaf(fc[2], xr[c * 8 + O + 2], c0); c1 = fmaf(fc[3], xr[c * 8 + O + 3], c1);                             \
+        d0 = fmaf(fd[2], xr[c * 8 + O + 2], d0); d1 = fmaf(fd[3], xr[c * 8 + O + 3], d1);
+        ROWQ_STEP(x, 0)
+        ROWQ_STEP(y, 4)
+#undef ROWQ_STEP
+    }
+    const float ra = a0 + a1, rb = b0 + b1, rc = c0 + c1, rd = d0 + d1;
+    const bool h16 = lane & 16, h8 = lane & 8;
+    float k0 = (h16 ? rc : ra) + __shfl_xor_sync(0xffffffffu, h16 ? ra : rc, 16);
+    float k1 = (h16 ? rd : rb) + __shfl_xor_sync(0xffffffffu, h16 ? rb : rd, 16);
+    float keep = (h8 ? k1 : k0) + __shfl_xor_sync(0xffffffffu, h8 ? k0 : k1, 8);
+#pragma unroll
+    for (int o = 4; o > 0; o >>= 1) keep += __shfl_xor_sync(0xffffffffu, keep, o);
+    return keep;
+}
+// order-preserving int image of a float (-0 and +0 map to the same value): lets a CTA keep its running threshold with
+// one shared-memory atomicMax
+__device__ __forceinline__ int f32_ord(float f) { const int i = __float_as_int(f); return i >= 0 ? i : -(i & 0x7fffffff); }
+
+static constexpr int HQ_CAP = 256;                      // candidate rows one CTA lists per step (xs region)
+
+// Greedy lm_head of the default instantiation (DESIGN.md section 4.1, "lm_head from its int8 copy").  The producer
+// streams the CTA's rows of the int8 copy (SLOT_BYTES / K rows per slot).  Row r yields a_r = s_r * sum_i q_ri x_i and
+// B_r = |x|_2 C_r, rounded outwards, with the logit f_r the bf16 row gives under row_dot4 / row_dot in [a_r - B_r, a_r + B_r].
+// The CTA keeps T = max_r (a_r - B_r) and lists the rows with a_r + B_r >= T (the threshold only grows, so a row left out
+// when it was seen stays out).  Every row whose f_r equals the CTA's maximum is listed; the listed rows whose upper bound
+// reaches the final T are recomputed from their bf16 rows with row_dot -- row_dot4's arithmetic, so f_r is bit for bit
+// that of the bf16 form -- and folded by (value, lower id).  A list longer than HQ_CAP, or a non-finite bound, recomputes
+// every row of the slice instead.  best_v / best_i end up the same in every lane of a warp.  xs holds the candidate list
+// after the register load; its header st: [0] T as f32_ord, [1] rows listed, [2] non-finite bound seen, [3] rows recomputed.
+template <int K>
+__device__ __forceinline__ void consume_head_q(const Slice& s, const Ring& ring, uint32_t& q, float* xs, const float2* hsc,
+                                               float& best_v, int& best_i, const float* norm_w, float norm_r) {
+    static_assert(SLOT_BYTES / K == 16 || (SLOT_BYTES / K) % 32 == 0, "a turn is 32 rows: one slot, or a pair of 16-row slots");
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    constexpr int NU = K / 8;                      // 8-byte groups per int8 row
+    float xr[K / 32];
+    load_xr_norm<K>(xs, norm_w, norm_r, xr, lane);
+    float ss = 0.f;
+#pragma unroll
+    for (int i = 0; i < K / 32; ++i) ss = fmaf(xr[i], xr[i], ss);
+    // |x|_2 rounded up: the relative 2^-12 covers the rounding of the squares' sum, the square root and the product below
+    ss = warp_sum(ss);
+    const float nx = __fmul_ru(sqrtf(ss), 1.f + 0x1p-12f);
+    int* const st = reinterpret_cast<int*>(xs);
+    int2* const cl = reinterpret_cast<int2*>(xs + 4);              // [HQ_CAP] (row, f32_ord of its upper bound)
+    cons_sync();                                   // every warp holds its copy: xs becomes the candidate list
+    // below |x|_2^2 = 2^-60 the squares may have underflowed and |x|_2 no longer bounds anything: recompute in full
+    if (threadIdx.x == 0) { st[0] = INT_MIN; st[1] = 0; st[2] = !(ss >= 0x1p-60f); st[3] = 0; }
+    cons_sync();
+    // a lane's t-th row is s.r0 + 32 t + 4 warp + (lane >> 3) (every turn but the last is 32 rows); the 8 lanes of a row
+    // group fetch {s_r, C_r} of 8 turns ahead, one turn each, so the loads have 8 turns to arrive
+    const int j = lane >> 3;
+    auto fetch = [&](int t) { return __ldg(hsc + min(s.r0 + 32 * t + 4 * warp + j, s.r1 - 1)); };
+    float2 win = fetch(lane & 7), nxt = fetch(8 + (lane & 7));
+    int t = 0;
+    for (int r = s.r0; r < s.r1;) {
+        const int rowsA = min(s.rpc, s.r1 - r);
+        const uint32_t slotA = q % ring.nslot;
+        mbar_wait(&ring.full[slotA], (q / ring.nslot) & 1);
+        const bool pair = s.rpc < 32 && r + rowsA < s.r1;
+        const int rowsB = pair ? min(s.rpc, s.r1 - r - rowsA) : 0;
+        const uint32_t slotB = (q + 1) % ring.nslot;
+        if (pair) mbar_wait(&ring.full[slotB], ((q + 1) / ring.nslot) & 1);
+        const uint2* baseA = reinterpret_cast<const uint2*>(ring.slots + (size_t)slotA * SLOT_BYTES);
+        const uint2* baseB = reinterpret_cast<const uint2*>(ring.slots + (size_t)slotB * SLOT_BYTES);
+        const int R = rowsA + rowsB;
+        for (int i0 = 4 * warp; i0 < R; i0 += 4 * NCONS_WARPS, ++t) {
+            const int nv = min(4, R - i0);
+            const uint2* rp[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int ri = i0 + (i < nv ? i : 0);
+                rp[i] = ri < rowsA ? baseA + (size_t)ri * NU : baseB + (size_t)(ri - rowsA) * NU;
+            }
+            const float g = row_dot4_q<K>(rp[0], rp[1], rp[2], rp[3], xr, lane);
+            const int src = (lane & 24) | (t & 7);
+            const float sr = __shfl_sync(0xffffffffu, win.x, src), cr = __shfl_sync(0xffffffffu, win.y, src);
+            if ((t & 7) == 7) { win = nxt; nxt = fetch(t + 9 + (lane & 7)); }
+            const float a = g * sr;
+            const float b = __fadd_ru(__fmul_ru(nx, cr), 0x1p-100f);   // + a floor for results flushed to zero
+            const float lo = __fsub_rd(a, b), hi = __fadd_ru(a, b);
+            const bool mine = (lane & 7) == 0 && j < nv;
+            const bool finite = fabsf(lo) <= FLT_MAX && fabsf(hi) <= FLT_MAX;
+            if (mine && !finite) st[2] = 1;
+            int tw = mine && finite ? f32_ord(lo) : INT_MIN;
+            tw = max(tw, __shfl_xor_sync(0xffffffffu, tw, 8));
+            tw = max(tw, __shfl_xor_sync(0xffffffffu, tw, 16));
+            int T = 0;
+            if (lane == 0) T = max(atomicMax(st, tw), tw);
+            T = __shfl_sync(0xffffffffu, T, 0);
+            if (mine && finite && f32_ord(hi) >= T) {
+                const int k = atomicAdd(st + 1, 1);
+                if (k < HQ_CAP) cl[k] = make_int2(r + i0 + j, f32_ord(hi));
+            }
+        }
+        __syncwarp();
+        if (lane == 0) { mbar_arrive(&ring.empty[slotA]); if (pair) mbar_arrive(&ring.empty[slotB]); }
+        r += R; q += pair ? 2 : 1;
+    }
+    cons_sync();
+    const int T = st[0], n = st[1];
+    const bool full = n > HQ_CAP || st[2] != 0;
+    const int cnt = full ? s.r1 - s.r0 : n;
+    int done = 0;
+    for (int k = warp; k < cnt; k += NCONS_WARPS) {
+        int row = s.r0 + k;
+        if (!full) { const int2 e = cl[k]; if (e.y < T) continue; row = e.x; }
+        const float v = row_dot<K>(reinterpret_cast<const uint4*>(s.W + (size_t)row * K), xr, lane);
+        if (v > best_v || (v == best_v && row < best_i)) { best_v = v; best_i = row; }
+        ++done;
+    }
+    if (lane == 0) atomicAdd(st + 3, done);
 }
 
 // transposed warp reduction of 8 per-lane partials: returns, in every lane, the warp total of value index (lane >> 2)
@@ -573,6 +722,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     float* part = reinterpret_cast<float*>(ired + 64);                 // [2][8 warps][8 rows] K-split partials (consume_ksplit)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const bool is_producer = warp == NCONS_WARPS;
+    constexpr bool HEADQ = !LOGPROB && !TOPK && !SAMPLE && !REP;   // greedy: the lm_head streams from its int8 copy
 
     if (__ldcg(p.done) != 0) return;            // sequence finished: nothing to do this step
 
@@ -667,7 +817,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
                 issue_slice(make_slice(w.wgu, 2 * I, H, 2));
                 issue_slice(make_slice(w.wdown, H, I, 1));
             }
-            issue_slice(make_slice(p.lm_head, p.V, H, 1));
+            if constexpr (HEADQ) {
+                const Slice sl = make_slice(nullptr, p.V, H, 1);
+                constexpr int RQ = SLOT_BYTES / H;
+                for (int r = sl.r0; r < sl.r1; r += RQ) issue(p.lm_head_q + (size_t)r * H, (uint32_t)min(RQ, sl.r1 - r) * H);
+            } else {
+                issue_slice(make_slice(p.lm_head, p.V, H, 1));
+            }
         }
         return;
     }
@@ -1000,8 +1156,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
     Draw dr{};
     float smx = -INFINITY, ssel = 0.f;                 // SLP: this lane's raw maximum logit, raw logit of its best-key row
     if constexpr (SAMPLE) dr = make_draw(p.smp, __ldcg(p.n_out), p.row);   // n_out changes only after every CTA's ticket
-    consume<H, ME_ARGMAX, LOGPROB, TOPK, SAMPLE, REP>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v, best_i,
-                                                      best_s, pbuf + (p.L & 1) * PARAM_FLOATS, nrf, nullptr, &tk, &dr, &smx, &ssel, &rb);
+    if constexpr (HEADQ) {
+        Slice sl = make_slice(p.lm_head, p.V, H, 1);
+        sl.rpc = SLOT_BYTES / H;                       // rows per slot of the int8 copy
+        consume_head_q<H>(sl, ring, q, xs, p.lm_head_sc, best_v, best_i, pbuf + (p.L & 1) * PARAM_FLOATS, nrf);
+    } else {
+        consume<H, ME_ARGMAX, LOGPROB, TOPK, SAMPLE, REP>(make_slice(p.lm_head, p.V, H, 1), ring, q, xs, nullptr, 0u, nullptr, best_v,
+                                                          best_i, best_s, pbuf + (p.L & 1) * PARAM_FLOATS, nrf, nullptr, &tk, &dr, &smx,
+                                                          &ssel, &rb);
+    }
     MEGA_MARK();
     // candidates live in lanes 0, 8, 16, 24 of every warp (the four rows of a turn; lanes 0 / 16 in the two-row form):
     // merge them, lane 0 publishes the warp's best
@@ -1044,6 +1207,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
         if constexpr (TOPK) {                // the CTA's TK_MAX best of its warps' lists
             for (int wq = 1; wq < NCONS_WARPS; ++wq) tk_merge_from(tk, tkv + wq * TK_MAX, tki + wq * TK_MAX, false);
             tk_store(tk, p.tk_part_val + (size_t)blockIdx.x * TK_MAX, p.tk_part_idx + (size_t)blockIdx.x * TK_MAX);
+        }
+        if constexpr (HEADQ) {               // candidate list header of consume_head_q (still in xs)
+            const int* st = reinterpret_cast<const int*>(xs);
+            atomicAdd(p.hq_stats, (unsigned long long)st[3]);
+            if (st[1] > HQ_CAP || st[2] != 0) atomicAdd(p.hq_stats + 3, 1ull);
         }
         __threadfence();
         unsigned t = atomicAdd(p.bar, 1u);
@@ -1120,6 +1288,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) decode_step_kernel(const Params p
             if (tok == 151643 || tok == 151645 || n >= p.max_new) { *p.done = 1; *p.next_id = -1; tok = -1; }
             else { p.ids_out[n] = tok; *p.n_out = n + 1; *p.pos = pos + 1; *p.next_id = tok; }
             tok_s = tok;
+            if constexpr (HEADQ) {               // every CTA has added its recomputed rows before its ticket
+                const unsigned long long nr = __ldcg(p.hq_stats);
+                p.hq_stats[0] = 0; p.hq_stats[1] = __ldcg(p.hq_stats + 1) + nr;
+                if (nr > __ldcg(p.hq_stats + 2)) p.hq_stats[2] = nr;
+            }
             p.bar[0] = 0;                        // every CTA has taken its ticket: reset for the next launch
             p.bar[1] = p.bar[1] + 1;             // new epoch: words published by this step can never match again
             p.bar[3] = p.bar[3] + 1;             // executed launches of this kernel: the next one uses the other set
@@ -1164,6 +1337,9 @@ bool decode_mega_supported(const Model& m, int B, int ctx) {
     if (c.num_hidden_layers > 32) return false;                  // 5-bit layer field
     if ((max_ctx + mega::KV_KEYS - 1) / mega::KV_KEYS > mega::MAX_SPLITS) return false;                           // merge loop bound (SB)
     if (((max_ctx + mega::KV_KEYS - 1) / mega::KV_KEYS) * c.num_key_value_heads > m.ctx->sm_count) return false;   // one CTA per (kv head, 64-key split)
+    return decode_mega_dims(c);
+}
+bool decode_mega_dims(const asrb_dims& c) {
     return dims_match<1024, 2048, 3072>(c) || dims_match<2048, 2048, 6144>(c) || dims_match<256, 512, 512>(c);
 }
 
@@ -1201,6 +1377,8 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
                              cudaStream_t st, int64_t* launches) {
     ASRB_REQUIRE(decode_mega_supported(m, B, ctx_now), ASRB_ERR_STATE, "fused decode step not supported for this model/batch/context");
     ASRB_REQUIRE(m.d_dec_layers && mb.bar && mb.part && mb.sx_seq, ASRB_ERR_STATE, "fused decode step buffers missing");
+    const bool greedy = !b.logprobs && !b.topk && !b.sample && !b.rep;      // the instantiation that reads the int8 copy
+    ASRB_REQUIRE(!greedy || (m.lm_head_q && m.lm_head_sc && mb.hq_stats), ASRB_ERR_STATE, "fused decode step: int8 lm_head copy missing");
     const asrb_dims& c = m.d.c;
     const int G = m.ctx->sm_count;
     const int group = c.num_attention_heads / c.num_key_value_heads;
@@ -1243,6 +1421,7 @@ void launch_decode_step_mega(const Model& m, const DecodeBufs& b, int B, float* 
             if (b.logprobs) { p.part_max = b.part_max; p.part_sel = b.part_sel; }
         }
         if (b.rep) { p.rep_bits = b.rep_mask; p.rep_words = rep_cta_words(c, G); p.rep = b.rep_params; }
+        p.lm_head_q = m.lm_head_q; p.lm_head_sc = m.lm_head_sc; p.hq_stats = mb.hq_stats;
         // tags must stay monotonic for red.max publication: long before the 24-bit epoch wraps, wipe the tagged exchange
         // buffers (the self-validating words live elsewhere and are left alone: to them 0 would be a published 0.0)
         if (mb.steps_issued && ++*mb.steps_issued >= 0xFFFF00u) {

@@ -81,6 +81,10 @@ struct Model {
     // (row & 7) -- bank-conflict-free ldmatrix on bulk-copied rows -- and plain norm vectors; null for unsupported dims
     DecLayerW* d_dec_layers_b = nullptr;
     bf16* lm_head_b = nullptr;
+    // greedy fused single-sequence step (decode_mega.cu consume_head_q): int8 copy of the lm_head and per row {scale s_r,
+    // bound constant C_r}; null for dims without that instantiation
+    int8_t* lm_head_q = nullptr;
+    float2* lm_head_sc = nullptr;
     float *rope_cos = nullptr, *rope_sin = nullptr;   // [rope_max_pos][head_dim/2]
     int rope_max_pos = 0;
 
@@ -235,8 +239,10 @@ size_t dec_attn_smem_bytes(const Model& m, int max_ctx);
 // also performs the greedy bookkeeping of src/inference.rs:161-170 (EOS check, append, embed)
 struct MegaBufs { unsigned* bar = nullptr; float* part = nullptr; long long* dbg = nullptr; size_t part_bytes = 0; unsigned* steps_issued = nullptr;
                   uint32_t* sx = nullptr; size_t sx_bytes = 0; int* sx_nb = nullptr;   // sx: decode_batch.cu's self-validating words   // per-session state of the fused step
-                  uint32_t* sx_seq = nullptr; };   // decode_mega.cu's self-validating words (outside `part`: never wiped to 0)
+                  uint32_t* sx_seq = nullptr;   // decode_mega.cu's self-validating words (outside `part`: never wiped to 0)
+                  unsigned long long* hq_stats = nullptr; };   // [4] int8 lm_head counters of the greedy single-sequence step
 size_t decode_mega_part_floats(const Model& m);
+bool decode_mega_dims(const asrb_dims& c);   // (hidden, q_dim, intermediate) the single-sequence fused step is compiled for
 size_t decode_mega_sx_bytes(const Model& m);
 size_t decode_batch_part_floats(const Model& m);
 size_t decode_batch_sx_bytes(const Model& m);   // decode_batch.cu: NB sequences per fused launch

@@ -162,6 +162,37 @@ static bf16* swizzled_rows_copy(Model* m, const bf16* src, size_t n_rows, int K)
     return dst;
 }
 
+// int8 copy of the lm_head for the greedy single-sequence fused step (decode_mega.cu consume_head_q; derivation in
+// DESIGN.md section 4.1), one warp per row: s_r = absmax / 127 (fp32), q_r = round(w_r / s_r), and in fp64
+//   C_r = |w_r - s_r q_r|_2 + gamma_n |w_r|_2 + gamma_(n+1) s_r |q_r|_2,   n = K / 64 + 6,  gamma_k = k u / (1 - k u),
+// enlarged by a relative 1e-9 (the fp64 sums' own rounding) and rounded up to fp32.  |x|_2 C_r bounds the distance between
+// the kernel's fp32 logit of the bf16 row and its fp32 approximation s_r * sum_i q_ri x_i.
+__global__ void quantize_head_kernel(const bf16* __restrict__ w, int8_t* __restrict__ q, float2* __restrict__ sc, int V, int K,
+                                     double gn, double gn1) {
+    const int lane = threadIdx.x & 31, row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= V) return;
+    const bf16* wr = w + (size_t)row * K;
+    float amax = 0.f;
+    for (int k = lane; k < K; k += 32) amax = fmaxf(amax, fabsf(__bfloat162float(wr[k])));
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const float s = amax / 127.f;
+    double r2 = 0.0, w2 = 0.0, q2 = 0.0;
+    for (int k = lane; k < K; k += 32) {
+        const float v = __bfloat162float(wr[k]);
+        const float qf = s > 0.f ? fminf(fmaxf(rintf(v / s), -127.f), 127.f) : 0.f;
+        q[(size_t)row * K + k] = (int8_t)qf;
+        const double d = (double)v - (double)s * (double)qf;
+        r2 += d * d; w2 += (double)v * (double)v; q2 += (double)qf * (double)qf;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        r2 += __shfl_xor_sync(0xffffffffu, r2, o); w2 += __shfl_xor_sync(0xffffffffu, w2, o); q2 += __shfl_xor_sync(0xffffffffu, q2, o);
+    }
+    if (lane == 0) {
+        const double C = (sqrt(r2) + gn * sqrt(w2) + gn1 * (double)s * sqrt(q2)) * (1.0 + 1e-9);
+        sc[row] = make_float2(s, __double2float_ru(C));
+    }
+}
+
 // Copy of an fp32 vector in the activation layout of the fused decode step (decode_mega.cu, xs_swz): 16-byte group k
 // is stored at k ^ ((k >> 3) & 1), which makes the per-lane 32-byte register loads of the GEMV bank-conflict free.
 static float* swizzled_copy(Model* m, const float* dev_src, int n) {
@@ -400,6 +431,15 @@ void model_finalize(Model* m) {
         m->lm_head_b = swizzled_rows_copy(m, m->lm_head, (size_t)V, (int)H);
         m->d_dec_layers_b = dev_alloc<DecLayerW>(m, tab.size());
         ASRB_CUDA_CHECK(cudaMemcpy(m->d_dec_layers_b, tab.data(), tab.size() * sizeof(DecLayerW), cudaMemcpyHostToDevice));
+    }
+    if (decode_mega_dims(c)) {                                  // int8 lm_head copy for the single-sequence fused step
+        const int n = (int)H / 64 + 6;                       // roundings on a term's path in row_dot4 / row_dot (and row_dot4_q)
+        const double u = std::ldexp(1.0, -24);
+        auto gamma = [&](int k) { return k * u / (1.0 - k * u); };
+        m->lm_head_q = dev_alloc<int8_t>(m, (size_t)V * H);
+        m->lm_head_sc = dev_alloc<float2>(m, (size_t)V);
+        quantize_head_kernel<<<(unsigned)((V + 7) / 8), 256>>>(m->lm_head, m->lm_head_q, m->lm_head_sc, (int)V, (int)H, gamma(n), gamma(n + 1));
+        ASRB_CUDA_CHECK(cudaGetLastError());
     }
     build_mel_tables(m);
     build_pos_tables(m);

@@ -258,6 +258,7 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
             s->mega.sx_seq = (uint32_t*)salloc<uint8_t>(s, bytes);
             ASRB_CUDA_CHECK(cudaMemset(s->mega.sx_seq, 0xFF, bytes));
         }
+        s->mega.hq_stats = salloc<unsigned long long>(s, 4, true);
         if (getenv("ASRB_MEGA_DEBUG")) s->mega.dbg = salloc<long long>(s, decode_mega_dbg_slots(), true);
         ASRB_CUDA_CHECK(cudaMallocHost(&s->h_done, Bm * sizeof(int)));
         ASRB_CUDA_CHECK(cudaMallocHost(&s->h_nout, Bm * sizeof(int)));
@@ -1055,8 +1056,15 @@ void session_last_top_logprobs(Session* s, int max_new_tokens, int k, int32_t* i
 }
 
 void session_stats(Session* s, int64_t* out, int n) {
-    const int64_t v[5] = {s->n_batch_steps, s->n_mega_steps, s->n_phase_steps, g_gemm_simt_fallbacks.load(), g_gemm_tc_launches.load()};
-    for (int i = 0; i < n && i < 5; ++i) out[i] = v[i];
+    unsigned long long hq[4] = {0, 0, 0, 0};
+    if (n > 5 && s->mega.hq_stats) {
+        ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+        ASRB_CUDA_CHECK(cudaMemcpyAsync(hq, s->mega.hq_stats, sizeof(hq), cudaMemcpyDeviceToHost, s->st));
+        ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    }
+    const int64_t v[8] = {s->n_batch_steps, s->n_mega_steps, s->n_phase_steps, g_gemm_simt_fallbacks.load(), g_gemm_tc_launches.load(),
+                          (int64_t)hq[1], (int64_t)hq[2], (int64_t)hq[3]};
+    for (int i = 0; i < n && i < 8; ++i) out[i] = v[i];
 }
 
 // ranked hypotheses of the last beam run: ids [batch][k][max_new_tokens] (-1 beyond the length), lens / sums / scores /

@@ -400,12 +400,13 @@ class AsrInference:
 
     def stats(self) -> Dict[str, int]:
         """Decoder-forward / GEMM path counters (asrb_session_stats): fallbacks are visible, never silent."""
-        out = (C.c_int64 * 5)()
+        out = (C.c_int64 * 8)()
         if self._session is None:
             return {}
-        _lib.check(self._lib.asrb_session_stats(self._session, out, 5))
+        _lib.check(self._lib.asrb_session_stats(self._session, out, 8))
         return dict(zip(("decode_batch_steps", "decode_fused_steps", "decode_phase_steps", "gemm_simt_fallbacks",
-                         "gemm_tc_launches"), [int(v) for v in out]))
+                         "gemm_tc_launches", "lmhead_rows_recomputed", "lmhead_step_max_recomputed",
+                         "lmhead_full_fallbacks"), [int(v) for v in out]))
 
     def _ensure_session(self, batch: int, max_samples: int, max_lang: int, max_new: int, max_context: int = 0):
         cap = self._cap
