@@ -323,6 +323,33 @@ ASRB_API int asrb_session_set_context(asrb_session* s, int n_rows, const int64_t
  * [2] KV bytes fanned out to followers; writes min(n, 3) values. */
 ASRB_API int asrb_last_prefill_stats(asrb_session* s, int64_t* out, int n);
 
+/* Teacher-forced scoring of caller-given continuations.  Utterance b (prompt S_b ids exactly as asrb_transcribe_ids
+ * builds it: context and lang_ids included) has n_cand[b] >= 1 candidates; candidate c (flattened over utterances in
+ * order) is cand_len[c] ids cand_ids[c][0..len).  Id i of candidate c sits at position S_b + i.
+ *   logprob_out  [n_total][max_new_tokens]  log p(ids[i] | prompt, ids[0..i)) = l - logsumexp(l) under the model's raw fp32
+ *                                          logits; NaN at and beyond cand_len[c]
+ *   top_ids_out / top_lp_out  [n_total][max_new_tokens][k] or NULL: with option "top_logprobs" = k >= 1, the k best ids
+ *                                          of that position under (logit descending, id ascending) and their
+ *                                          log-probabilities; -1 / NaN beyond the length
+ * Independent of the decode options: temperature, seed, beam_size, length_penalty, no_repeat_ngram_size and
+ * repetition_penalty are not consulted, and the results are bitwise equal whatever they are set to.  Bitwise
+ * deterministic for a given call.  Each candidate takes one KV slot; the first candidate of an utterance computes its
+ * prompt, the others take the prompt's K/V from it (asrb_last_prefill_stats: rows computed = sum_b S_b +
+ * sum_c (len_c - 1), rows shared = sum_b (n_cand[b] - 1) * S_b, KV bytes fanned out = rows shared x the K/V bytes of one
+ * position).  asrb_last_timings: [3] the decoder layers of the prefill, [4] the score head, [5] the whole call.
+ * ASRB_ERR_INVALID before any work: n_total = sum n_cand > max_batch, n_cand[b] < 1, cand_len[c] outside
+ * [1, max_new_tokens], an id outside [0, vocab), a hidden size the wgmma score head cannot take (not a multiple of 64),
+ * plus everything asrb_transcribe_ids refuses.  A scoring call ends any pending run: asrb_generate / asrb_decode_step /
+ * asrb_last_logprobs / _top_logprobs / _nbest return ASRB_ERR_STATE until the next prefill. */
+ASRB_API int asrb_score_ids(asrb_session* s, const float* const* samples, const int64_t* n_samples, int batch,
+                            const int64_t* const* lang_ids, const int32_t* n_lang_ids,
+                            const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
+                            int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out);
+/* the same on the utterances of the last asrb_ingest_pcm */
+ASRB_API int asrb_score_ingested(asrb_session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids,
+                                 const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
+                                 int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out);
+
 /* debug (ASRB_MEGA_DEBUG=1): clock64 timeline of the last fused decode step, CTA 0 then CTA G-1;
  * returns the number of slots per CTA (0 if disabled) */
 ASRB_API int asrb_debug_mega_timeline(long long* out, int cap);

@@ -16,7 +16,7 @@ import sys
 
 USAGE = ("Usage: python -m qwen3_asr_rs_b200 <model_dir> <audio_file> [language] [--logprobs] [--top-logprobs N] "
          "[--temperature T[,T...]] [--seed N] [--beam-size N] [--length-penalty A] [--context TEXT | --context-file PATH] "
-         "[--no-repeat-ngram N] [--repetition-penalty P] [--max-segment S]")
+         "[--no-repeat-ngram N] [--repetition-penalty P] [--max-segment S] [--score TEXT | --detect-language]")
 
 
 def parse_args(argv):
@@ -153,6 +153,19 @@ def split_context(argv):
     return f[0], text
 
 
+def split_score(argv):
+    """Remove `--score TEXT` and `--detect-language` from argv -> (remaining argv, text to score or None, detect), or
+    None when the text is missing or both are given."""
+    c = _take_flag(argv, "--score")
+    if c is None:
+        return None
+    rest = [a for a in c[0] if a != "--detect-language"]
+    detect = len(rest) != len(c[0])
+    if detect and c[1] is not None:
+        return None
+    return rest, c[1], detect
+
+
 def split_max_segment(argv):
     """Remove `--max-segment S` from argv -> (remaining argv, S in seconds; None when absent), or None when the value is
     missing or not a valid segment length (a whole number of 10 ms, at least 5 s)."""
@@ -187,6 +200,11 @@ def main(argv=None) -> int:
         print(USAGE, file=sys.stderr)
         return 1
     argv, max_segment = seg
+    sc = split_score(argv)
+    if sc is None:
+        print(USAGE, file=sys.stderr)
+        return 1
+    argv, score_text, detect = sc
     rep = split_repetition(argv)
     ctx = split_context(rep[0]) if rep is not None else None
     beam = split_beam(ctx[0]) if ctx is not None else None
@@ -206,6 +224,23 @@ def main(argv=None) -> int:
         return 1
     from . import AsrInference
     eng = AsrInference.load(model_dir, device=0)
+    if (score_text is not None or detect) and eng.tokenizer is None:
+        eng.close()
+        print(f"--score / --detect-language need tokenizer.json in {model_dir}", file=sys.stderr)
+        return 1
+    if score_text is not None or detect:
+        try:
+            if detect:
+                for name, p in eng.detect_language(audio)[:5]:
+                    print(f"{name}\t{p:.4f}")
+            else:
+                r = eng.score(audio, [score_text], language=language, context=ctx[1] or None)[0]
+                for t, lp in zip(r.ids, r.logprobs):
+                    print(f"{t}\t{lp:.6f}")
+                print(f"sum\t{r.sum_logprob:.6f}")
+        finally:
+            eng.close()
+        return 0
     try:
         _, temperature, seed = sampling
         kw = {} if temperature is None else dict(temperature=temperature, seed=seed)

@@ -19,6 +19,7 @@ SYMBOLS = [
     "asrb_last_logprobs", "asrb_last_top_logprobs", "asrb_last_nbest", "asrb_last_beam_stats",
     "asrb_session_create_ex", "asrb_session_set_context", "asrb_last_prefill_stats",
     "asrb_ingest_long", "asrb_long_read", "asrb_segment_long", "asrb_transcribe_segments",
+    "asrb_score_ids", "asrb_score_ingested",
 ]
 
 
@@ -93,6 +94,9 @@ def load_library() -> C.CDLL:
         "asrb_long_read": [vp, C.c_int, P(C.c_float)],
         "asrb_segment_long": [vp, i64, i64, C.c_int, P(i32), P(i64), P(i64)],
         "asrb_transcribe_segments": [vp, C.c_int, P(i32), P(i64), P(i64), P(P(i64)), P(i32), C.c_int, P(i32), P(i32)],
+        "asrb_score_ids": [vp, P(P(C.c_float)), P(i64), C.c_int, P(P(i64)), P(i32), P(i32), P(P(i64)), P(i32), C.c_int,
+                           P(C.c_float), P(i32), P(C.c_float)],
+        "asrb_score_ingested": [vp, P(P(i64)), P(i32), P(i32), P(P(i64)), P(i32), C.c_int, P(C.c_float), P(i32), P(C.c_float)],
     }
     for name, args in sig.items():
         fn = getattr(lib, name)

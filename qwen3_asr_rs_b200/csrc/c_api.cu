@@ -44,6 +44,9 @@ void session_last_nbest(Session* s, int max_new_tokens, int k, int32_t* ids_out,
 void session_last_beam_stats(Session* s, int64_t* out, int n);
 void session_set_context(Session* s, int n_rows, const int64_t* const* ids, const int32_t* n_ids);
 void session_last_prefill_stats(Session* s, int64_t* out, int n);
+void session_score_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* const* lang_ids,
+                       const int32_t* n_lang_ids, const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
+                       int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out);
 int decode_mega_debug_timeline(long long* out, int cap);
 int decode_batch_debug_timeline(long long* out, int cap);
 }  // namespace asrb
@@ -251,6 +254,21 @@ int asrb_last_nbest(asrb_session* s, int max_new_tokens, int k, int32_t* ids_out
 }
 int asrb_last_beam_stats(asrb_session* s, int64_t* out, int n) {
     return guarded([&] { NONNULL(s); NONNULL(out); session_last_beam_stats(s->s, out, n); });
+}
+int asrb_score_ids(asrb_session* s, const float* const* samples, const int64_t* n_samples, int batch,
+                   const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int32_t* n_cand,
+                   const int64_t* const* cand_ids, const int32_t* cand_len, int max_new_tokens, float* logprob_out,
+                   int32_t* top_ids_out, float* top_lp_out) {
+    return guarded([&] { NONNULL(s); NONNULL(samples); NONNULL(n_samples);
+                         session_score_ids(s->s, samples, n_samples, batch, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len,
+                                           max_new_tokens, logprob_out, top_ids_out, top_lp_out); });
+}
+int asrb_score_ingested(asrb_session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int32_t* n_cand,
+                        const int64_t* const* cand_ids, const int32_t* cand_len, int max_new_tokens, float* logprob_out,
+                        int32_t* top_ids_out, float* top_lp_out) {
+    return guarded([&] { NONNULL(s);
+                         session_score_ids(s->s, nullptr, nullptr, 0, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len,
+                                           max_new_tokens, logprob_out, top_ids_out, top_lp_out); });
 }
 
 int asrb_debug_mega_timeline(long long* out, int cap) {

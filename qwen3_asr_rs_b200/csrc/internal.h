@@ -252,6 +252,19 @@ void launch_greedy(const Model& m, const DecodeBufs& b, int B, cudaStream_t st, 
 void launch_lmhead_argmax(const Model& m, const float* x_rows, const int* d_row_idx, int B,
                           const DecodeBufs& b, bool write_logits, cudaStream_t st, int64_t* launches);
 
+// score.cu -- teacher-forced scoring head (asrb_score_ids, DESIGN.md 4.8)
+constexpr int SCORE_SLICES = 64;    // column slices per row: the partial workspace is rows x SCORE_SLICES, whatever the vocab
+struct ScorePart {                  // one (row, column slice): max logit, sum of exp(l - max), target logit (-inf: not here)
+    float m, s, t;
+    float tv[TK_MAX]; int ti[TK_MAX];   // TOPK: the slice's best (logit, id), best first
+};
+int score_slices(const Model& m);
+void check_score_head(const Model& m);   // throws ASRB_ERR_INVALID for a shape the wgmma head cannot take
+// rows r of hid[d_src[r]] -> final norm -> lm_head; lp_out[r] = log p(d_target[r]), with topk the 8 best of each row
+void launch_score_head(const Model& m, const float* hid, const int* d_src, const int* d_target, int rows, float* gathered,
+                       bf16* planes, size_t plane_stride, int nplanes, ScorePart* part, bool topk, float* lp_out,
+                       int* tk_ids, float* tk_lp, cudaStream_t st, int64_t* launches);
+
 // beam.cu -- beam search over the TOPK records (session option "beam_size"); the spec is in include/asr_b200.h
 constexpr int BEAM_MAX = 6;
 struct BeamUtt {                   // device state of one utterance's search

@@ -111,6 +111,15 @@ struct Session {
     std::vector<int64_t> long_n, long_off;
     double* d_seg_blk = nullptr; size_t seg_blk_cap = 0;      // asrb_segment_long scratch: 160-sample block energies
     int64_t* d_seg_i64 = nullptr; size_t seg_i64_cap = 0;     // ... its plan, cut counts and cuts
+    size_t act_rows = 0;                // rows the decoder activations hold (hid, dqkv, qrot, dh, dattn, dact)
+    // teacher-forced scoring (asrb_score_ids): allocated, and grown, by the scoring calls that need them; a scoring call
+    // whose prefill has more rows than act_rows (the candidates' own rows beside the prompts) widens the activations
+    struct ScoreBufs {
+        int rows_cap = 0;                       // score rows the head's scratch holds
+        float* gathered = nullptr; bf16* planes = nullptr; ScorePart* part = nullptr;
+        float* lp = nullptr; int* tk_ids = nullptr; float* tk_lp = nullptr;
+        int* h_int = nullptr; int* d_int = nullptr; size_t int_cap = 0;   // row plan | per-slot arrays | score rows
+    } sc;
     ~Session();
 };
 
@@ -128,6 +137,7 @@ Session::~Session() {
     if (h_ids) cudaFreeHost(h_ids);
     if (h_nout) cudaFreeHost(h_nout);
     if (h_next) cudaFreeHost(h_next);
+    if (sc.h_int) cudaFreeHost(sc.h_int);
     if (ingest) ingest_state_free(ingest);
     if (st) cudaStreamDestroy(st);
 }
@@ -201,6 +211,7 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
         s->dqkv = salloc<float>(s, totS * d.qkv_dim);
         s->qrot = salloc<float>(s, totS * d.q_dim);
         s->dh_ps = totS * c.hidden_size; s->dattn_ps = totS * d.q_dim; s->dact_ps = totS * c.intermediate_size;
+        s->act_rows = totS;
         s->dh = salloc<bf16>(s, 3 * s->dh_ps);
         s->dattn = salloc<bf16>(s, 3 * s->dattn_ps);
         s->dact = salloc<bf16>(s, 3 * s->dact_ps);
@@ -622,13 +633,65 @@ void session_last_prefill_stats(Session* s, int64_t* out, int n) {
     for (int i = 0; i < n && i < 3; ++i) out[i] = v[i];
 }
 
+// utterance b's whole prompt, position by position (s->S[b] positions): ids, and the audio row of each audio position
+// (-1 elsewhere)
+static void build_prompt(const Session* s, int b, const int64_t* const* lang_ids, std::vector<int>& pid, std::vector<int>& parow) {
+    const std::vector<int>& cb = context_of(s, b);
+    pid.clear(); parow.clear();
+    for (int i = 0; i < 3; ++i) { pid.push_back(kPromptHead[i]); parow.push_back(-1); }
+    for (int id : cb) { pid.push_back(id); parow.push_back(-1); }
+    for (int i = 3; i < 9; ++i) { pid.push_back(kPromptHead[i]); parow.push_back(-1); }
+    for (int t = 0; t < s->T[b]; ++t) { pid.push_back(kAudioPad); parow.push_back(s->toff[b] + t); }
+    for (int i = 0; i < 6; ++i) { pid.push_back(kPromptTail[i]); parow.push_back(-1); }
+    for (int i = 0, nl = s->S[b] - (int)pid.size(); i < nl; ++i) { pid.push_back((int)lang_ids[b][i]); parow.push_back(-1); }
+}
+
+// embed + inject and the decoder layers over the planned rows (s->d_ids ..., totS rows; sequence q's rows are its
+// segment of the attention, in KV slot q)
+static void prefill_layers(Session* s, int totS, int nseq, int maxrows, const FanOut* fan, const int* d_qpos0) {
+    Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
+    cudaStream_t st = s->st; const int np = s->nplanes;
+    launch_embed_inject(m.embed, c.hidden_size, s->d_ids, s->d_audio_row, s->audio, totS, s->hid, st);
+    s->launches += 1;
+    const int H = c.hidden_size; const float eps = (float)c.rms_norm_eps;
+    for (int l = 0; l < c.num_hidden_layers; ++l) {
+        const DecLayerW& w = m.dec[l];
+        float* kc = s->kcache + (size_t)l * s->cache_layer_stride;
+        float* vc = s->vcache + (size_t)l * s->cache_layer_stride;
+        launch_rmsnorm_s3(s->hid, w.ln_in, totS, H, eps, s->dh, s->dh_ps, st);
+        { GemmA A = plainA(s->dh, s->dh_ps, totS, H, np);
+          GemmEpi E; E.out_f32 = s->dqkv; E.ldo = d.qkv_dim;
+          launch_gemm(A, w.wqkv, d.qkv_dim, E, s->gemm_impl, st); }
+        launch_qk_norm_rope(s->dqkv, totS, s->d_row_seq, s->d_row_pos, w.qnorm, w.knorm, eps, m.rope_cos, m.rope_sin,
+                            c.num_attention_heads, c.num_key_value_heads, c.head_dim, s->qrot, kc, vc, s->cache_seq_stride,
+                            s->max_ctx, st, fan);
+        { AttnParams p{}; p.q = s->qrot; p.ldq = d.q_dim; p.k = kc; p.v = vc; p.seg_stride = s->cache_seq_stride;
+          p.head_stride = (size_t)s->max_ctx * c.head_dim; p.ldk = c.head_dim; p.keys_in_rows = 0;
+          p.seg_q0 = s->d_seq_q0; p.seg_len = s->d_seq_len; p.nseg = nseq; p.nheads = c.num_attention_heads;
+          p.group = c.num_attention_heads / c.num_key_value_heads; p.causal = 1; p.max_len = maxrows; p.seg_pos0 = d_qpos0;
+          p.out_s3 = s->dattn; p.plane_stride = s->dattn_ps; p.ldo = d.q_dim;
+          launch_attention(p, c.head_dim, st); }
+        { GemmA A = plainA(s->dattn, s->dattn_ps, totS, d.q_dim, np);
+          GemmEpi E; E.residual = s->hid; E.ldr = H; E.out_f32 = s->hid; E.ldo = H; E.splitk_ws = s->splitk_ws; E.extra_launches = &s->launches;
+          launch_gemm(A, w.wo, H, E, s->gemm_impl, st); }
+        launch_rmsnorm_s3(s->hid, w.ln_post, totS, H, eps, s->dh, s->dh_ps, st);
+        { GemmA A = plainA(s->dh, s->dh_ps, totS, H, np);
+          GemmEpi E; E.mode = EPI_SWIGLU; E.out_s3 = s->dact; E.s3_plane_stride = s->dact_ps; E.lds = c.intermediate_size;
+          launch_gemm(A, w.wgu, 2 * c.intermediate_size, E, s->gemm_impl, st); }
+        { GemmA A = plainA(s->dact, s->dact_ps, totS, c.intermediate_size, np);
+          GemmEpi E; E.residual = s->hid; E.ldr = H; E.out_f32 = s->hid; E.ldo = H; E.splitk_ws = s->splitk_ws; E.extra_launches = &s->launches;
+          launch_gemm(A, w.wdown, H, E, s->gemm_impl, st); }
+        s->launches += 8;
+    }
+}
+
 void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, int64_t* seq_lens_out,
                      float* last_logits) {
     ASRB_REQUIRE(s->stage >= 2, ASRB_ERR_STATE, "prefill called before encode");
     check_sampling_options(s, s->B);
     check_context(s, s->B);
-    Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
-    const int B = s->B; cudaStream_t st = s->st; const int np = s->nplanes;
+    Model& m = *s->m; const asrb_dims& c = m.d.c;
+    const int B = s->B; cudaStream_t st = s->st;
     for (int b = 0; b < B; ++b) {
         int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
         ASRB_REQUIRE(nl >= 0 && nl <= s->max_lang, ASRB_ERR_INVALID, "language prompt exceeds session capacity");
@@ -665,14 +728,7 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     int64_t shared = 0;
     std::vector<int> pid, parow;
     for (int b = 0; b < B; ++b) {
-        const std::vector<int>& cb = context_of(s, b);
-        pid.clear(); parow.clear();                                    // the whole prompt, position by position
-        for (int i = 0; i < 3; ++i) { pid.push_back(kPromptHead[i]); parow.push_back(-1); }
-        for (int id : cb) { pid.push_back(id); parow.push_back(-1); }
-        for (int i = 3; i < 9; ++i) { pid.push_back(kPromptHead[i]); parow.push_back(-1); }
-        for (int t = 0; t < s->T[b]; ++t) { pid.push_back(kAudioPad); parow.push_back(s->toff[b] + t); }
-        for (int i = 0; i < 6; ++i) { pid.push_back(kPromptTail[i]); parow.push_back(-1); }
-        for (int i = 0, nl = s->S[b] - (int)pid.size(); i < nl; ++i) { pid.push_back((int)lang_ids[b][i]); parow.push_back(-1); }
+        build_prompt(s, b, lang_ids, pid, parow);
         // rows from position skip[b] on (build_position_ids :259-266: position = index in the prompt)
         for (int i = skip[b], r = s->srow0[b]; i < s->S[b]; ++i, ++r) { ids[r] = pid[i]; arow[r] = parow[i]; rseq[r] = b; rpos[r] = i; }
         const int rows = s->S[b] - skip[b];
@@ -719,38 +775,7 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
         ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.tk_eos_lp, 0xFF, (size_t)B * TK_MAX * sizeof(float), st));
     }
 
-    launch_embed_inject(m.embed, c.hidden_size, s->d_ids, s->d_audio_row, s->audio, totS, s->hid, st);
-    s->launches += 1;
-    const int H = c.hidden_size; const float eps = (float)c.rms_norm_eps;
-    for (int l = 0; l < c.num_hidden_layers; ++l) {
-        const DecLayerW& w = m.dec[l];
-        float* kc = s->kcache + (size_t)l * s->cache_layer_stride;
-        float* vc = s->vcache + (size_t)l * s->cache_layer_stride;
-        launch_rmsnorm_s3(s->hid, w.ln_in, totS, H, eps, s->dh, s->dh_ps, st);
-        { GemmA A = plainA(s->dh, s->dh_ps, totS, H, np);
-          GemmEpi E; E.out_f32 = s->dqkv; E.ldo = d.qkv_dim;
-          launch_gemm(A, w.wqkv, d.qkv_dim, E, s->gemm_impl, st); }
-        launch_qk_norm_rope(s->dqkv, totS, s->d_row_seq, s->d_row_pos, w.qnorm, w.knorm, eps, m.rope_cos, m.rope_sin,
-                            c.num_attention_heads, c.num_key_value_heads, c.head_dim, s->qrot, kc, vc, s->cache_seq_stride,
-                            s->max_ctx, st, fan ? &fan_plan : nullptr);
-        { AttnParams p{}; p.q = s->qrot; p.ldq = d.q_dim; p.k = kc; p.v = vc; p.seg_stride = s->cache_seq_stride;
-          p.head_stride = (size_t)s->max_ctx * c.head_dim; p.ldk = c.head_dim; p.keys_in_rows = 0;
-          p.seg_q0 = s->d_seq_q0; p.seg_len = s->d_seq_len; p.nseg = B; p.nheads = c.num_attention_heads;
-          p.group = c.num_attention_heads / c.num_key_value_heads; p.causal = 1; p.max_len = maxrows; p.seg_pos0 = d_qpos0;
-          p.out_s3 = s->dattn; p.plane_stride = s->dattn_ps; p.ldo = d.q_dim;
-          launch_attention(p, c.head_dim, st); }
-        { GemmA A = plainA(s->dattn, s->dattn_ps, totS, d.q_dim, np);
-          GemmEpi E; E.residual = s->hid; E.ldr = H; E.out_f32 = s->hid; E.ldo = H; E.splitk_ws = s->splitk_ws; E.extra_launches = &s->launches;
-          launch_gemm(A, w.wo, H, E, s->gemm_impl, st); }
-        launch_rmsnorm_s3(s->hid, w.ln_post, totS, H, eps, s->dh, s->dh_ps, st);
-        { GemmA A = plainA(s->dh, s->dh_ps, totS, H, np);
-          GemmEpi E; E.mode = EPI_SWIGLU; E.out_s3 = s->dact; E.s3_plane_stride = s->dact_ps; E.lds = c.intermediate_size;
-          launch_gemm(A, w.wgu, 2 * c.intermediate_size, E, s->gemm_impl, st); }
-        { GemmA A = plainA(s->dact, s->dact_ps, totS, c.intermediate_size, np);
-          GemmEpi E; E.residual = s->hid; E.ldr = H; E.out_f32 = s->hid; E.ldo = H; E.splitk_ws = s->splitk_ws; E.extra_launches = &s->launches;
-          launch_gemm(A, w.wdown, H, E, s->gemm_impl, st); }
-        s->launches += 8;
-    }
+    prefill_layers(s, totS, B, maxrows, fan ? &fan_plan : nullptr, d_qpos0);
     // final norm + lm_head on the last row of each utterance only (the reference computes all S rows,
     // text_decoder.rs:111-112, and uses row S-1, inference.rs:156)
     launch_lmhead_argmax(m, s->hid, s->d_lastrow, B, s->db, last_logits != nullptr, st, &s->launches);
@@ -987,6 +1012,218 @@ void session_transcribe_segments(Session* s, int n, const int32_t* file, const i
         off[i] = s->long_off[f] + start[i];
     }
     transcribe_impl(s, nullptr, len.data(), n, off.data(), lang_ids, n_lang_ids, max_new_tokens, ids_out, lens_out);
+}
+
+// -------------------------------------------------------------------------------------------------
+// teacher-forced scoring (asrb_score_ids, DESIGN.md 4.8): one prefill over every candidate, flat candidates sharing
+// their utterance's prompt through the K/V fan-out, then the score head over the rows that predict the given ids
+// -------------------------------------------------------------------------------------------------
+// device buffers taken all or none: a failed cudaMalloc frees the ones already taken and throws, and nothing of the
+// session has changed; commit() hands them to the session
+struct AllocAll {
+    std::vector<void*> got;
+    ~AllocAll() { for (void* p : got) cudaFree(p); }
+    template <typename T> T* take(size_t n) {
+        void* p = nullptr;
+        ASRB_CUDA_CHECK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)));
+        got.push_back(p);
+        return static_cast<T*>(p);
+    }
+    void commit(Session* s) { for (void* p : got) s->owned.push_back(p); got.clear(); }
+};
+static void release_owned(Session* s, void* p) {
+    auto it = std::find(s->owned.begin(), s->owned.end(), p);
+    if (it != s->owned.end()) { cudaFree(p); s->owned.erase(it); }
+}
+
+// a scoring call's prefill of `rows` rows, `score_rows` head rows and a plan of `plan_ints` ints: every buffer is grown
+// to fit first, then the old ones are released, so a failed allocation leaves the session as it was
+static void ensure_score_bufs(Session* s, size_t rows, int score_rows, size_t plan_ints) {
+    const Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
+    Session::ScoreBufs& b = s->sc;
+    const bool act = rows > s->act_rows, head = score_rows > b.rows_cap, plan = plan_ints > b.int_cap;
+    if (!act && !head && !plan) return;
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));      // the old buffers may still be read
+    AllocAll a;
+    float *hid = nullptr, *dqkv = nullptr, *qrot = nullptr; bf16 *dh = nullptr, *dattn = nullptr, *dact = nullptr;
+    if (act) {
+        hid = a.take<float>(rows * c.hidden_size); dqkv = a.take<float>(rows * d.qkv_dim); qrot = a.take<float>(rows * d.q_dim);
+        dh = a.take<bf16>(3 * rows * c.hidden_size); dattn = a.take<bf16>(3 * rows * d.q_dim);
+        dact = a.take<bf16>(3 * rows * c.intermediate_size);
+    }
+    const size_t R = std::max(score_rows, b.rows_cap);
+    float *gathered = nullptr, *lp = nullptr, *tk_lp = nullptr; bf16* planes = nullptr; ScorePart* part = nullptr; int* tk_ids = nullptr;
+    if (head) {
+        gathered = a.take<float>(R * c.hidden_size); planes = a.take<bf16>(3 * R * c.hidden_size);
+        part = a.take<ScorePart>(R * score_slices(m)); lp = a.take<float>(R);
+        tk_ids = a.take<int>(R * TK_MAX); tk_lp = a.take<float>(R * TK_MAX);
+    }
+    int *d_int = nullptr, *h_int = nullptr;
+    if (plan) {
+        d_int = a.take<int>(plan_ints);
+        ASRB_CUDA_CHECK(cudaMallocHost(&h_int, plan_ints * sizeof(int)));
+    }
+    // every allocation succeeded: swap in, release the old buffers
+    a.commit(s);
+    if (act) {
+        for (void* p : {(void*)s->hid, (void*)s->dqkv, (void*)s->qrot, (void*)s->dh, (void*)s->dattn, (void*)s->dact}) release_owned(s, p);
+        s->hid = hid; s->dqkv = dqkv; s->qrot = qrot; s->dh = dh; s->dattn = dattn; s->dact = dact;
+        s->dh_ps = rows * c.hidden_size; s->dattn_ps = rows * d.q_dim; s->dact_ps = rows * c.intermediate_size;
+        s->act_rows = rows;
+    }
+    if (head) {
+        for (void* p : {(void*)b.gathered, (void*)b.planes, (void*)b.part, (void*)b.lp, (void*)b.tk_ids, (void*)b.tk_lp}) release_owned(s, p);
+        b.gathered = gathered; b.planes = planes; b.part = part; b.lp = lp; b.tk_ids = tk_ids; b.tk_lp = tk_lp;
+        b.rows_cap = (int)R;
+    }
+    if (plan) {
+        release_owned(s, b.d_int);
+        if (b.h_int) cudaFreeHost(b.h_int);
+        b.d_int = d_int; b.h_int = h_int; b.int_cap = plan_ints;
+    }
+}
+
+static void score_impl(Session* s, const float* const* samples, const int64_t* n_samples, int batch,
+                       const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int32_t* n_cand,
+                       const int64_t* const* cand_ids, const int32_t* cand_len, int max_new_tokens, float* logprob_out,
+                       int32_t* top_ids_out, float* top_lp_out) {
+    ASRB_REQUIRE(logprob_out && n_cand && cand_ids && cand_len, ASRB_ERR_INVALID, "score: null argument");
+    if (samples == nullptr) {
+        batch = (int)s->ingested_n.size();          // asrb_score_ingested
+        ASRB_REQUIRE(batch >= 1, ASRB_ERR_STATE, "score_ingested: no ingested audio");
+    }
+    Model& m = *s->m; const asrb_dims& c = m.d.c;
+    // ---- every argument checked before any work ----
+    ASRB_REQUIRE(batch >= 1 && batch <= s->max_batch, ASRB_ERR_INVALID, "score: batch exceeds session capacity");
+    ASRB_REQUIRE(max_new_tokens >= 1 && max_new_tokens <= s->max_new, ASRB_ERR_INVALID, "max_new_tokens exceeds session capacity");
+    check_context(s, batch);
+    check_score_head(m);
+    int64_t n_total = 0;
+    for (int b = 0; b < batch; ++b) {
+        ASRB_REQUIRE(n_cand[b] >= 1, ASRB_ERR_INVALID, "score: every utterance needs at least one candidate");
+        n_total += n_cand[b];
+        const int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
+        ASRB_REQUIRE(nl >= 0 && nl <= s->max_lang, ASRB_ERR_INVALID, "language prompt exceeds session capacity");
+        for (int i = 0; i < nl; ++i)
+            ASRB_REQUIRE(lang_ids[b][i] >= 0 && lang_ids[b][i] < c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
+    }
+    ASRB_REQUIRE(n_total <= s->max_batch, ASRB_ERR_INVALID,
+                 "score: " + std::to_string(n_total) + " candidates exceed the session's max_batch (one KV slot each)");
+    const int N = (int)n_total;
+    for (int q = 0; q < N; ++q) {
+        ASRB_REQUIRE(cand_len[q] >= 1 && cand_len[q] <= max_new_tokens, ASRB_ERR_INVALID, "score: candidate length outside [1, max_new_tokens]");
+        ASRB_REQUIRE(cand_ids[q], ASRB_ERR_INVALID, "score: null candidate");
+        for (int i = 0; i < cand_len[q]; ++i)
+            ASRB_REQUIRE(cand_ids[q][i] >= 0 && cand_ids[q][i] < c.vocab_size, ASRB_ERR_INVALID, "score: candidate id out of vocabulary");
+    }
+    const int k = s->top_k;
+    const bool topk = k >= 1 && top_ids_out && top_lp_out;
+    ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
+    cudaStream_t st = s->st;
+    s->launches = 0; s->decode_steps = 0;
+    s->nbest_valid = false; s->lp_valid = false; s->tk_valid = 0;
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
+    s->timing = true;
+    try { mel_impl(s, samples, n_samples, batch, nullptr, nullptr); } catch (...) { s->timing = false; throw; }
+    s->timing = false;
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
+    session_encode(s, nullptr);
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[3], st));
+    s->stage = 2;                                     // the KV slots are overwritten: no run to continue after this call
+    // ---- plan: slot q = candidate q; the first candidate of an utterance leads (its prompt and its ids but the last),
+    // the others (followers) compute their ids but the last from position S_b on, their prompt K/V fanned out ----
+    const int B = batch;
+    s->S.assign(B, 0);
+    std::vector<int> utt(N), lead(N), srow0(N), rows(N), coff(N + 1, 0);
+    int totS = 0, maxrows = 0, R = 0;
+    int64_t shared = 0;
+    for (int b = 0, q = 0; b < B; ++b) {
+        const int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
+        s->S[b] = 9 + (int)context_of(s, b).size() + s->T[b] + 6 + nl;
+        for (int j = 0; j < n_cand[b]; ++j, ++q) {
+            utt[q] = b; lead[q] = q - j;
+            rows[q] = (j == 0 ? s->S[b] : 0) + cand_len[q] - 1;
+            srow0[q] = totS; totS += rows[q]; maxrows = std::max(maxrows, rows[q]);
+            coff[q] = R; R += cand_len[q];
+        }
+        shared += (int64_t)(n_cand[b] - 1) * s->S[b];
+    }
+    coff[N] = R;
+    Session::ScoreBufs& sb = s->sc;
+    ensure_score_bufs(s, (size_t)totS, R, 4 * (size_t)totS + 8 * (size_t)N + 2 * (size_t)R + 16);
+    int* hi = sb.h_int;
+    int* ids = hi; int* arow = ids + totS; int* rseq = arow + totS; int* rpos = rseq + totS;
+    int* sq0 = rpos + totS; int* slen = sq0 + N; int* qpos0 = slen + N;
+    int* fan_n = qpos0 + N; int* fan_off = fan_n + N; int* fan_P = fan_off + N; int* fan_slots = fan_P + N;
+    int* src = fan_slots + std::max(N, 1); int* tgt = src + R;
+    const size_t nint = (size_t)(tgt + R - hi);
+    ASRB_REQUIRE(nint <= sb.int_cap && R <= sb.rows_cap, ASRB_ERR_INVALID, "score: plan exceeds session capacity");
+    std::vector<int> pid, parow;
+    int nf = 0;
+    for (int q = 0; q < N; ++q) {
+        const int b = utt[q], Sb = s->S[b];
+        const bool leader = lead[q] == q;
+        int r = srow0[q];
+        if (leader) {
+            build_prompt(s, b, lang_ids, pid, parow);
+            for (int i = 0; i < Sb; ++i, ++r) { ids[r] = pid[i]; arow[r] = parow[i]; rseq[r] = q; rpos[r] = i; }
+        }
+        for (int i = 0; i + 1 < cand_len[q]; ++i, ++r) { ids[r] = (int)cand_ids[q][i]; arow[r] = -1; rseq[r] = q; rpos[r] = Sb + i; }
+        sq0[q] = srow0[q]; slen[q] = rows[q]; qpos0[q] = leader ? 0 : Sb;
+        fan_off[q] = nf; fan_n[q] = 0; fan_P[q] = 0;
+        if (leader) {
+            fan_P[q] = Sb;
+            for (int f = q + 1; f < N && lead[f] == q; ++f) { fan_slots[nf++] = f; ++fan_n[q]; }
+        }
+        // row map: id 0 from the leader's last prompt row, id i from this candidate's row at position S_b + i - 1
+        const int own0 = leader ? srow0[q] + Sb : srow0[q];
+        for (int i = 0; i < cand_len[q]; ++i) {
+            src[coff[q] + i] = i == 0 ? srow0[lead[q]] + Sb - 1 : own0 + i - 1;
+            tgt[coff[q] + i] = (int)cand_ids[q][i];
+        }
+    }
+    s->pf_rows = totS; s->pf_shared_rows = shared;
+    s->pf_fan_bytes = shared * 2LL * c.num_hidden_layers * c.num_key_value_heads * c.head_dim * (int64_t)sizeof(float);
+    int* di = sb.d_int;
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(di, hi, nint * sizeof(int), cudaMemcpyHostToDevice, st));
+    s->d_ids = di; s->d_audio_row = di + (arow - hi); s->d_row_seq = di + (rseq - hi);
+    s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
+    const FanOut fan_plan{di + (fan_n - hi), di + (fan_off - hi), di + (fan_P - hi), di + (fan_slots - hi)};
+    const bool fan = nf > 0;
+    prefill_layers(s, totS, N, maxrows, fan ? &fan_plan : nullptr, fan ? di + (qpos0 - hi) : nullptr);
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
+    launch_score_head(m, s->hid, di + (src - hi), di + (tgt - hi), R, sb.gathered, sb.planes, (size_t)sb.rows_cap * c.hidden_size,
+                      s->nplanes, sb.part, topk, sb.lp, sb.tk_ids, sb.tk_lp, st, &s->launches);
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
+    std::vector<float> lp((size_t)R), tlp(topk ? (size_t)R * TK_MAX : 0);
+    std::vector<int> tid(tlp.size());
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(lp.data(), sb.lp, lp.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (topk) {
+        ASRB_CUDA_CHECK(cudaMemcpyAsync(tid.data(), sb.tk_ids, tid.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+        ASRB_CUDA_CHECK(cudaMemcpyAsync(tlp.data(), sb.tk_lp, tlp.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
+    }
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int i = 0; i < 5; ++i) ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[i], s->ev[i], s->ev[i + 1]));
+    ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[5], s->ev[0], s->ev[5]));
+    const float nan = std::numeric_limits<float>::quiet_NaN();
+    for (int q = 0; q < N; ++q)
+        for (int i = 0; i < max_new_tokens; ++i) {
+            const bool in = i < cand_len[q];
+            const size_t o = (size_t)q * max_new_tokens + i, r = (size_t)coff[q] + i;
+            logprob_out[o] = in ? lp[r] : nan;
+            if (topk)
+                for (int j = 0; j < k; ++j) {
+                    top_ids_out[o * k + j] = in ? tid[r * TK_MAX + j] : -1;
+                    top_lp_out[o * k + j] = in ? tlp[r * TK_MAX + j] : nan;
+                }
+        }
+}
+
+void session_score_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* const* lang_ids,
+                       const int32_t* n_lang_ids, const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
+                       int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out) {
+    score_impl(s, samples, n_samples, batch, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len, max_new_tokens, logprob_out,
+               top_ids_out, top_lp_out);
 }
 
 void session_last_timings(Session* s, float* ms6, int64_t* kernels, int64_t* steps) {

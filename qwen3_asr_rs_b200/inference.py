@@ -23,6 +23,8 @@ from .config import AsrConfig
 
 EOS_TOKEN_IDS = (151643, 151645)      # inference.rs:154
 MAX_NEW_TOKENS = 4096                 # inference.rs:153
+SCORE_SLOTS = 32                      # candidates (KV slots) per scoring call; more run in waves of whole utterances
+EOS_ID = 151645                       # <|im_end|>
 MEL_SAMPLE_RATE = 16000               # inference.rs:16
 
 _DT = {"float32": 0, "bfloat16": 1, "float16": 2}
@@ -303,6 +305,52 @@ class TranscribeIds:
     # beam_size=K > 1: per utterance, its K hypotheses ranked as (ids, sum_logprob, score, eos_id; -1 = stopped by the
     # cap); entry 0 is `ids` (None for an attempt that sampled)
     nbest: Optional[List[Optional[List[Tuple[List[int], float, float, int]]]]] = None
+
+
+@dataclass
+class ScoredCandidate:
+    """One scored continuation: `logprobs[i]` = log p(ids[i] | prompt, ids[:i]); with top_logprobs = k, the k best
+    (id, log p) of every position and `greedy_prefix`, the number of leading ids that are the top-1 of their position."""
+    ids: List[int]
+    logprobs: List[float]
+    sum_logprob: float
+    top_logprobs: Optional[List[List[Tuple[int, float]]]] = None
+    greedy_prefix: Optional[int] = None
+
+
+def check_candidates(candidates, batch: int, vocab: int) -> List[List[List[int]]]:
+    """candidates[b]: a non-empty list of non-empty id lists per utterance, every id in [0, vocab)."""
+    if len(candidates) != batch:
+        raise ValueError(f"need one candidate list per utterance: {len(candidates)} for {batch}")
+    out = []
+    for b, cands in enumerate(candidates):
+        if not cands:
+            raise ValueError(f"utterance {b} has no candidate")
+        rows = []
+        for c in cands:
+            ids = [int(i) for i in c]
+            if not ids:
+                raise ValueError(f"utterance {b}: an empty candidate")
+            if any(i < 0 or i >= vocab for i in ids):
+                raise ValueError(f"utterance {b}: candidate id out of [0, {vocab})")
+            rows.append(ids)
+        out.append(rows)
+    return out
+
+
+def score_waves(n_cand: Sequence[int], slots: int) -> List[List[int]]:
+    """Utterance indices per call: whole utterances in order, at most max(slots, the largest n_cand) candidates each."""
+    cap = max([slots] + list(n_cand))
+    waves, cur, used = [], [], 0
+    for b, n in enumerate(n_cand):
+        if cur and used + n > cap:
+            waves.append(cur)
+            cur, used = [], 0
+        cur.append(b)
+        used += n
+    if cur:
+        waves.append(cur)
+    return waves
 
 
 class AsrInference:
@@ -716,6 +764,130 @@ class AsrInference:
                 self._record_logprobs(s, False)
             if top_logprobs:
                 self._record_top_logprobs(s, top_logprobs, False)
+
+    # ---- teacher-forced scoring (asrb_score_ids) --------------------------------------------------------------------
+    def score_ids(self, clips: Sequence[np.ndarray], candidates: Sequence[Sequence[Sequence[int]]],
+                  language_ids: Optional[Sequence] = None, context_ids: Optional[Sequence] = None,
+                  top_logprobs: int = 0) -> List[List[ScoredCandidate]]:
+        """Log-probability of every id of every candidate continuation, from one teacher-forced prefill per call:
+        `candidates[b]` lists id sequences for clip b, each scored after the prompt transcribe_ids builds (language ids
+        and context included).  The candidates of a clip share its prompt's prefill.  With `top_logprobs` = k in 1..8,
+        also the k best ids of every position and the greedy prefix.  More candidates than SCORE_SLOTS run in several
+        calls of whole utterances."""
+        B = len(clips)
+        cands = check_candidates(candidates, B, self.config.text.vocab_size)
+        k = check_top_logprobs(top_logprobs)
+        ctx = check_context_ids(context_ids, B, self.config.text.vocab_size)
+        out: List[List[ScoredCandidate]] = [None] * B
+        for wave in score_waves([len(c) for c in cands], SCORE_SLOTS):
+            sub = [clips[b] for b in wave]
+            arrs, ptrs, lens = self._pack_samples(sub)
+            lang = None if language_ids is None else [language_ids[b] for b in wave]
+            keep, lptrs, llens, mx = self._pack_lang(lang, len(wave))
+            wc = [cands[b] for b in wave]
+            n_total = sum(len(c) for c in wc)
+            max_new = max(len(c) for cs in wc for c in cs)
+            wctx = None if ctx is None else [ctx[b] for b in wave]
+            s = self._ensure_session(n_total, max(a.shape[0] for a in arrs), mx, max_new, _max_len(wctx))
+            res = self._score(s, wc, max_new, k, wctx, lambda *a: self._lib.asrb_score_ids(s, ptrs, lens, len(wave), lptrs, llens, *a))
+            for b, r in zip(wave, res):
+                out[b] = r
+        return out
+
+    def score_pcm(self, pcms: Sequence, rates: Sequence[int], candidates: Sequence[Sequence[Sequence[int]]],
+                  language_ids: Optional[Sequence] = None, context_ids: Optional[Sequence] = None,
+                  top_logprobs: int = 0) -> List[List[ScoredCandidate]]:
+        """score_ids with step 1 on the GPU: raw PCM in (as transcribe_pcm)."""
+        B = len(pcms)
+        cands = check_candidates(candidates, B, self.config.text.vocab_size)
+        k = check_top_logprobs(top_logprobs)
+        ctx = check_context_ids(context_ids, B, self.config.text.vocab_size)
+        out: List[List[ScoredCandidate]] = [None] * B
+        for wave in score_waves([len(c) for c in cands], SCORE_SLOTS):
+            lang = None if language_ids is None else [language_ids[b] for b in wave]
+            keep, lptrs, llens, mx = self._pack_lang(lang, len(wave))
+            wc = [cands[b] for b in wave]
+            max_new = max(len(c) for cs in wc for c in cs)
+            wctx = None if ctx is None else [ctx[b] for b in wave]
+            s, _arrs, _n = self._ingest([pcms[b] for b in wave], [rates[b] for b in wave], mx, max_new,
+                                        slots=sum(len(c) for c in wc), max_context=_max_len(wctx))
+            res = self._score(s, wc, max_new, k, wctx, lambda *a: self._lib.asrb_score_ingested(s, lptrs, llens, *a))
+            for b, r in zip(wave, res):
+                out[b] = r
+        return out
+
+    def _score(self, s, cands: List[List[List[int]]], max_new: int, k: int, context_ids, call) -> List[List[ScoredCandidate]]:
+        flat = [c for cs in cands for c in cs]
+        N = len(flat)
+        n_cand = (C.c_int32 * len(cands))(*[len(cs) for cs in cands])
+        arrs = [np.ascontiguousarray(c, dtype=np.int64) for c in flat]
+        cptrs = (C.POINTER(C.c_int64) * N)(*[a.ctypes.data_as(C.POINTER(C.c_int64)) for a in arrs])
+        clens = (C.c_int32 * N)(*[len(c) for c in flat])
+        lp = np.empty((N, max_new), dtype=np.float32)
+        tid = np.empty((N, max_new, max(k, 1)), dtype=np.int32)
+        tlp = np.empty((N, max_new, max(k, 1)), dtype=np.float32)
+        if k:
+            self._record_top_logprobs(s, k, True)
+        try:
+            if context_ids is not None:
+                self._set_context(s, context_ids)
+            _lib.check(call(n_cand, cptrs, clens, int(max_new), lp.ctypes.data_as(C.POINTER(C.c_float)),
+                            tid.ctypes.data_as(C.POINTER(C.c_int32)) if k else None,
+                            tlp.ctypes.data_as(C.POINTER(C.c_float)) if k else None))
+        finally:
+            if context_ids is not None:
+                self._set_context(s, None)
+            if k:
+                self._record_top_logprobs(s, k, False)
+        res, q = [], 0
+        for cs in cands:
+            row = []
+            for c in cs:
+                n = len(c)
+                lps = [float(v) for v in lp[q, :n]]
+                sc = ScoredCandidate(ids=list(c), logprobs=lps, sum_logprob=float(np.sum(np.asarray(lps, np.float64))))
+                if k:
+                    sc.top_logprobs = [[(int(tid[q, i, j]), float(tlp[q, i, j])) for j in range(k)] for i in range(n)]
+                    g = 0
+                    while g < n and sc.top_logprobs[g][0][0] == c[g]:
+                        g += 1
+                    sc.greedy_prefix = g
+                row.append(sc)
+                q += 1
+            res.append(row)
+        return res
+
+    def score(self, audio_path: str, texts: Sequence[str], language: Optional[str] = None, context: Optional[str] = None,
+              eos: bool = True, top_logprobs: int = 0) -> List[ScoredCandidate]:
+        """Score transcripts of one WAV file: each text is tokenised (tokenizer.json) and, with `eos`, followed by
+        <|im_end|>, so that its log-probability includes ending there.  `language` / `context`: the prompt of
+        transcribe(language=..., context=...)."""
+        from .audio import read_wav_pcm
+        from .text import context_prompt_ids, language_prompt_ids
+        if self.tokenizer is None:
+            raise ValueError("scoring text needs tokenizer.json")
+        lang_ids = language_prompt_ids(self.tokenizer, language)
+        ctx_ids = context_prompt_ids(self.tokenizer, context)
+        cands = [self.tokenizer.encode(t) + ([EOS_ID] if eos else []) for t in texts]
+        pcm, rate = read_wav_pcm(audio_path)
+        return self.score_pcm([pcm], [rate], [cands], language_ids=[lang_ids] if lang_ids is not None else None,
+                              context_ids=[ctx_ids] if ctx_ids else None, top_logprobs=top_logprobs)[0]
+
+    def detect_language(self, audio_path: str, languages: Sequence[str] = None) -> List[Tuple[str, float]]:
+        """Language identification over a closed set: every `language_prompt_ids(tok, name)` continuation ("language
+        Xxx") is one candidate of the one utterance, all sharing its prompt's prefill.  Returns (name, probability)
+        best first, the probabilities a softmax over the candidates' summed log-probabilities.  The sums are
+        comparable without a terminator token only because no name of the set is a prefix of another (true of
+        text.LANGUAGES): a name that prefixed another would score its own ids and not its ending."""
+        from .audio import read_wav_pcm
+        from .text import LANGUAGES, language_probabilities, language_prompt_ids
+        names = list(LANGUAGES if languages is None else languages)
+        if self.tokenizer is None:
+            raise ValueError("language identification needs tokenizer.json")
+        cands = [language_prompt_ids(self.tokenizer, n) for n in names]
+        pcm, rate = read_wav_pcm(audio_path)
+        r = self.score_pcm([pcm], [rate], [cands])[0]
+        return language_probabilities(names, [c.sum_logprob for c in r])
 
     # ---- GPU-side audio ingest (step 1, src/audio.rs:162-245) -------------------------------------------
     _PCM_FMT = {"int16": 0, "float32": 1, "int32": 2}

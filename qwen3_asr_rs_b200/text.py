@@ -5,6 +5,7 @@ HF `tokenizers` runtime like /root/reference/src/tokenizer.rs:4-50.  SURVEY.md s
 """
 from __future__ import annotations
 
+import math
 import os
 from typing import List, Optional, Tuple
 
@@ -91,3 +92,22 @@ def context_prompt_ids(tokenizer: Optional[AsrTokenizer], context: Optional[str]
     if tokenizer is None:
         raise ValueError("a context needs tokenizer.json (to encode the text)")
     return tokenizer.encode(context)
+
+
+# the languages of the Qwen3-ASR model card, as the model writes them after "language "; no name is a prefix of another
+LANGUAGES = ("Chinese", "English", "Cantonese", "Arabic", "German", "French", "Spanish", "Portuguese", "Indonesian",
+             "Italian", "Korean", "Russian", "Thai", "Vietnamese", "Japanese", "Turkish", "Hindi", "Malay", "Dutch",
+             "Swedish", "Danish", "Finnish", "Polish", "Czech", "Filipino", "Persian", "Greek", "Hungarian",
+             "Macedonian", "Romanian")
+
+
+def language_probabilities(names: List[str], sum_logprobs: List[float]) -> List[Tuple[str, float]]:
+    """(name, probability) sorted by probability (then by the order given): a softmax over the candidates' summed
+    log-probabilities, in float64."""
+    if len(names) != len(sum_logprobs) or not names:
+        raise ValueError("need one summed log-probability per language")
+    m = max(sum_logprobs)
+    w = [math.exp(x - m) for x in sum_logprobs]
+    z = sum(w)
+    order = sorted(range(len(names)), key=lambda i: -w[i])
+    return [(names[i], w[i] / z) for i in order]
