@@ -2,6 +2,7 @@
 // entry point returns a status int and records a thread-local message (idiom of the reference's
 // own FFI layer, /root/reference/src/backend/mlx/ffi.rs:60-110).
 #include <cstring>
+#include <functional>
 #include "internal.h"
 
 namespace asrb {
@@ -78,6 +79,11 @@ template <typename F> static int guarded(F&& f) {
     catch (...) { g_last_error = "unknown error"; return ASRB_ERR_INVALID; }
 }
 #define NONNULL(p) ASRB_REQUIRE((p) != nullptr, ASRB_ERR_INVALID, "null pointer: " #p)
+
+namespace asrb {
+// the same status / message convention for the test probes (probe.cu)
+int run_guarded(const std::function<void()>& f) { return guarded(f); }
+}  // namespace asrb
 
 struct asrb_ctx { Ctx c; };
 struct asrb_model { Model m; };

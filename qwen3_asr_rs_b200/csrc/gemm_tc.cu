@@ -237,6 +237,36 @@ const CUtensorMap& tc_cached_map(const void* base, int rank, const cuuint64_t* d
     return tc::cached_map(base, rank, dims, strides_bytes, box);
 }
 
+GemmPlan plan_gemm_tc(const GemmA& A, int N, const GemmEpi& E, int sms) {
+    using namespace tc;
+    GemmPlan p;
+    if (A.K % BK != 0 || A.M <= 0 || N <= 0 || N % 8 != 0) return p;
+    if (A.nplanes < 1 || A.nplanes > 3) return p;
+    if (A.mode == A_PLAIN) {
+        if (A.plane_stride % 8 != 0 && A.nplanes > 1) return p;
+        if (E.mode != EPI_PLAIN && E.mode != EPI_SWIGLU && E.mode != EPI_CONVOUT) return p;
+        p.tiles_n = (N + BN - 1) / BN; p.tiles_m = (A.M + BM - 1) / BM;
+        // Split-K for plain GEMMs that cannot fill the GPU (e.g. prefill o_proj / down_proj: 32 tiles, K = 2048 / 3072;
+        // encoder fc2: 28 tiles, K = 3584): such a CTA is bound by its own TMA load rate (64 KB of operands per k-block),
+        // so 2-4 CTAs per tile finish 2-4x sooner; a second pass sums the partial tiles (fixed order) and applies the
+        // epilogue.  Deterministic; costs one extra fp32 round trip of the tile through L2.
+        const int tiles = p.tiles_n * p.tiles_m, kblocks = A.K / BK;
+        if ((E.mode == EPI_PLAIN || E.mode == EPI_CONVOUT) && E.splitk_ws && tiles <= 64 && (size_t)4 * A.M * N <= SPLITK_WS_FLOATS) {
+            for (int sp = 4; sp >= 2; --sp)
+                if (kblocks % sp == 0 && kblocks / sp >= 6 && tiles * sp <= sms + sms / 12) { p.splits = sp; break; }   // at most ~1.1 waves
+        }
+    } else {
+        if (A.cpad % BK != 0 || A.OW > BM || A.OW <= 0 || A.OH <= 0) return p;
+        if (E.mode != EPI_CONV_PARITY && E.mode != EPI_CONV_FEAT) return p;
+        p.box_h = std::min(A.OH, BM / A.OW);
+        p.tiles_n = (N + BN - 1) / BN;
+        p.tiles_m = (A.M / (A.OH * A.OW)) * ((A.OH + p.box_h - 1) / p.box_h);
+    }
+    p.grid = std::min(p.tiles_m * p.tiles_n * p.splits, sms);
+    p.tc = p.grid > 0;
+    return p;
+}
+
 bool launch_gemm_tc(const GemmA& A, const bf16* W, int N, const GemmEpi& Ein, cudaStream_t st) {
     using namespace tc;
     const GemmEpi& E = Ein;
@@ -255,8 +285,8 @@ bool launch_gemm_tc(const GemmA& A, const bf16* W, int N, const GemmEpi& Ein, cu
             cudaEventDestroy(e0); cudaEventDestroy(e1);
         }
     } timer(time_all, A.M, N, A.K, E.mode, st);
-    if (A.K % BK != 0 || A.M <= 0 || N <= 0) return false;
-    if (A.nplanes < 1 || A.nplanes > 3) return false;
+    const GemmPlan pl = plan_gemm_tc(A, N, E, sm_count());
+    if (!pl.tc) return false;
     if ((reinterpret_cast<uintptr_t>(A.a) & 15) || (reinterpret_cast<uintptr_t>(W) & 15)) return false;
     // B: [N][K] row-major bf16
     cuuint64_t bd[2] = {(cuuint64_t)A.K, (cuuint64_t)N};
@@ -265,34 +295,21 @@ bool launch_gemm_tc(const GemmA& A, const bf16* W, int N, const GemmEpi& Ein, cu
     const CUtensorMap mapB = cached_map(W, 2, bd, bs, bb);
     ConvGeom cg{};
     const size_t smem = smem_bytes();
-    if (N % 8 != 0) return false;
+    const int tiles_m = pl.tiles_m, tiles_n = pl.tiles_n;
     if (A.mode == A_PLAIN) {
-        if (A.plane_stride % 8 != 0 && A.nplanes > 1) return false;
         cuuint64_t ad[3] = {(cuuint64_t)A.K, (cuuint64_t)A.M, (cuuint64_t)3};
         cuuint64_t as[2] = {(cuuint64_t)A.lda * 2, (cuuint64_t)A.plane_stride * 2};
         cuuint32_t ab[3] = {(cuuint32_t)BK, (cuuint32_t)BM, 1};
         const CUtensorMap mapA = cached_map(A.a, 3, ad, as, ab);
-        const int tiles_n = (N + BN - 1) / BN, tiles_m = (A.M + BM - 1) / BM;
-        const int sms = sm_count();
-        // Split-K for plain GEMMs that cannot fill the GPU (e.g. prefill o_proj / down_proj: 32 tiles, K = 2048 / 3072;
-        // encoder fc2: 28 tiles, K = 3584): such a CTA is bound by its own TMA load rate (64 KB of operands per k-block),
-        // so 2-4 CTAs per tile finish 2-4x sooner; a second pass sums the partial tiles (fixed order) and applies the
-        // epilogue.  Deterministic; costs one extra fp32 round trip of the tile through L2.
-        const int tiles = tiles_n * tiles_m, kblocks = A.K / BK;
-        int splits = 1;
-        if ((E.mode == EPI_PLAIN || E.mode == EPI_CONVOUT) && E.splitk_ws && tiles <= 64 && N % 8 == 0 && (size_t)4 * A.M * N <= SPLITK_WS_FLOATS) {
-            for (int sp = 4; sp >= 2; --sp)
-                if (kblocks % sp == 0 && kblocks / sp >= 6 && tiles * sp <= sms + sms / 12) { splits = sp; break; }   // at most ~1.1 waves
-        }
-        if (splits > 1) {
+        if (pl.splits > 1) {
             GemmEpi P;                               // partial tiles: plain fp32 rows [split][M][N]
             P.out_f32 = E.splitk_ws; P.ldo = N;
             // (the attribute is per device: set on every launch, a process may hold contexts on several GPUs)
             ASRB_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<0, EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            gemm_tc_kernel<0, EPI_PLAIN><<<std::min(tiles * splits, sms), NTHREADS, smem, st>>>(mapA, mapB, A.M, N, A.K, A.nplanes, tiles_m, tiles_n, splits, cg, P);
+            gemm_tc_kernel<0, EPI_PLAIN><<<pl.grid, NTHREADS, smem, st>>>(mapA, mapB, A.M, N, A.K, A.nplanes, tiles_m, tiles_n, pl.splits, cg, P);
             const int work = A.M * (N / 8);
-            if (E.mode == EPI_PLAIN) splitk_reduce_kernel<EPI_PLAIN><<<(work + 255) / 256, 256, 0, st>>>(E.splitk_ws, splits, A.M, N, E);
-            else splitk_reduce_kernel<EPI_CONVOUT><<<(work + 255) / 256, 256, 0, st>>>(E.splitk_ws, splits, A.M, N, E);
+            if (E.mode == EPI_PLAIN) splitk_reduce_kernel<EPI_PLAIN><<<(work + 255) / 256, 256, 0, st>>>(E.splitk_ws, pl.splits, A.M, N, E);
+            else splitk_reduce_kernel<EPI_CONVOUT><<<(work + 255) / 256, 256, 0, st>>>(E.splitk_ws, pl.splits, A.M, N, E);
             ASRB_CUDA_CHECK(cudaGetLastError());
             if (E.extra_launches) *E.extra_launches += 1;
             return true;
@@ -300,17 +317,14 @@ bool launch_gemm_tc(const GemmA& A, const bf16* W, int N, const GemmEpi& Ein, cu
 #define ASRB_TC_LAUNCH(AM, EM)                                                                                         \
     {                                                                                                                  \
         ASRB_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<AM, EM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        gemm_tc_kernel<AM, EM><<<std::min(tiles_m * tiles_n, sms), NTHREADS, smem, st>>>(mapA, mapB, A.M, N, A.K, A.nplanes, tiles_m, tiles_n, 1, cg, E); \
+        gemm_tc_kernel<AM, EM><<<pl.grid, NTHREADS, smem, st>>>(mapA, mapB, A.M, N, A.K, A.nplanes, tiles_m, tiles_n, 1, cg, E); \
     }
         if (E.mode == EPI_PLAIN) ASRB_TC_LAUNCH(0, EPI_PLAIN)
         else if (E.mode == EPI_SWIGLU) ASRB_TC_LAUNCH(0, EPI_SWIGLU)
-        else if (E.mode == EPI_CONVOUT) ASRB_TC_LAUNCH(0, EPI_CONVOUT)
-        else return false;
+        else ASRB_TC_LAUNCH(0, EPI_CONVOUT)
     } else {
-        if (A.cpad % BK != 0 || A.OW > BM) return false;
-        const int per = A.OH * A.OW;
-        const int chunks = A.M / per;
-        cg.OH = A.OH; cg.OW = A.OW; cg.box_h = std::min(A.OH, BM / A.OW);
+        const int chunks = A.M / (A.OH * A.OW);
+        cg.OH = A.OH; cg.OW = A.OW; cg.box_h = pl.box_h;
         cg.tiles_per_chunk = (A.OH + cg.box_h - 1) / cg.box_h; cg.kblk_per_tap = A.cpad / BK;
         cg.a_box_bytes = A.OW * cg.box_h * BK * 2;
         // [plane][chunk*4 + ph*2 + pw][Hh][Wh][cpad]
@@ -319,11 +333,8 @@ bool launch_gemm_tc(const GemmA& A, const bf16* W, int N, const GemmEpi& Ein, cu
                             (cuuint64_t)A.plane_stride * 2};
         cuuint32_t ab[5] = {(cuuint32_t)BK, (cuuint32_t)A.OW, (cuuint32_t)cg.box_h, 1, 1};
         const CUtensorMap mapA = cached_map(A.a, 5, ad, as, ab);
-        const int tiles_n = (N + BN - 1) / BN, tiles_m = chunks * cg.tiles_per_chunk;
-        const int sms = sm_count();
         if (E.mode == EPI_CONV_PARITY) ASRB_TC_LAUNCH(1, EPI_CONV_PARITY)
-        else if (E.mode == EPI_CONV_FEAT) ASRB_TC_LAUNCH(1, EPI_CONV_FEAT)
-        else return false;
+        else ASRB_TC_LAUNCH(1, EPI_CONV_FEAT)
 #undef ASRB_TC_LAUNCH
     }
     ASRB_CUDA_CHECK(cudaGetLastError());

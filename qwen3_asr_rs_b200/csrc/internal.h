@@ -134,6 +134,11 @@ extern std::atomic<int64_t> g_gemm_simt_fallbacks, g_gemm_tc_launches;   // gemm
 void launch_gemm(const GemmA& A, const bf16* W, int N, const GemmEpi& E, int impl, cudaStream_t st);
 // wgmma implementation (gemm_tc.cu); returns false when the shape is unsupported
 bool launch_gemm_tc(const GemmA& A, const bf16* W, int N, const GemmEpi& E, cudaStream_t st);
+// What launch_gemm_tc launches for a shape on a GPU of `sms` SMs (host only, no device call): tc = false when the
+// wgmma kernel cannot take the shape or epilogue (launch_gemm then runs the SIMT GEMM); otherwise the k-split factor,
+// the output tiles and the persistent grid (work items = tiles_m * tiles_n * splits, dealt round-robin over the grid)
+struct GemmPlan { bool tc = false; int splits = 1, tiles_m = 0, tiles_n = 0, grid = 0, box_h = 0; };
+GemmPlan plan_gemm_tc(const GemmA& A, int N, const GemmEpi& E, int sms);
 void launch_gemm_simt(const GemmA& A, const bf16* W, int N, const GemmEpi& E, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------
