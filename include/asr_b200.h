@@ -350,6 +350,55 @@ ASRB_API int asrb_score_ingested(asrb_session* s, const int64_t* const* lang_ids
                                  const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
                                  int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out);
 
+/* ---- streaming transcription (DESIGN.md 4.9) ----
+ * A streaming run uses an ordinary session (asrb_session_create_ex).  Stream b lives in KV slot b,
+ * 0 <= b < n_streams <= max_batch.  It owns its 16 kHz f32 samples x[0..n), its forced prefix p (ids, empty at the
+ * start) and a push counter k.  Push k on stream b with new samples, and optionally `final`:
+ *   1. appends the samples; n may not exceed max_samples;
+ *   2. computes the hypothesis h = p + g, where g is the greedy (or sampled, per the session options) continuation of
+ *      the prompt asrb_transcribe_ids builds for x[0..n) with lang_ids = the push's language ids + p.  The context of
+ *      asrb_session_set_context is latched when the stream starts (asrb_stream_open / asrb_stream_reset).  g stops at
+ *      EOS or at the push's max_new_tokens;
+ *   3. sets the next prefix p' = h[0 .. max(0, |h| - R)) when k + 1 >= U, else empty; R = rollback_ids (default 5),
+ *      U = unfixed_pushes (default 2).  |p'| is returned as the hypothesis' fixed length;
+ *   4. on a final push every frame counts as final and there is no rollback (p' = h); the stream is then closed and a
+ *      later push on it returns ASRB_ERR_STATE until asrb_stream_reset.
+ * A stream that gets no samples (and is not final) in a push is idle: it is not prefilled or decoded and its
+ * hypothesis is unchanged.  k counts the pushes that gave the stream samples.
+ * Equivalence: the stream's mel after any push is bitwise asrb_mel(x[0..n)); its encoder output, prefill and decode
+ * records follow the project's float64 rule against the oracle on x[0..n) with the same prompt; its g equals
+ * asrb_transcribe_ids(x[0..n), lang + p) on clips whose decisions have a margin; for a given push schedule, samples and
+ * options the results are bitwise reproducible.  They are NOT promised bitwise equal to an offline call: windows and K/V
+ * reused from earlier pushes were computed under other GEMM shapes (split-K choice).
+ * Reuse: a finished encoder window (all frames final: frame f is final once 160 f + 200 <= n) is not encoded again when
+ * its clamped mel cannot have changed; the decoder keeps the K/V of positions < P_b = 9 + L_b + (tokens of the windows
+ * before the first re-encoded one), and P_b = 0 on a stream's first push after open / reset.
+ * Any non-stream call that starts a run (asrb_transcribe*, asrb_score*, asrb_mel, asrb_prefill) or asrb_stream_open
+ * ends all streams: asrb_stream_push then returns ASRB_ERR_STATE.
+ * Refused with ASRB_ERR_INVALID before any work, leaving all stream state intact: beam_size > 1 (streams own their
+ * slots), n_streams > max_batch, samples past max_samples, |lang| + |p| > max_lang_ids, a stream's first push with
+ * <= 160 samples, max_ids < |p| + max_new_tokens, and the option conflicts asrb_transcribe_ids refuses. */
+ASRB_API int asrb_stream_open(asrb_session* s, int n_streams, int rollback_ids, int unfixed_pushes);
+/* stream b back to its start (no samples, empty prefix, k = 0, open), the context re-latched */
+ASRB_API int asrb_stream_reset(asrb_session* s, int stream);
+/* one push on all n_streams streams (n_streams as opened):
+ *   samples[b] / n_samples[b]  new samples of stream b (n_samples[b] = 0: none)
+ *   is_final[b]                NULL or nonzero: stream b's last push
+ *   lang_ids[b] / n_lang_ids   as asrb_transcribe_ids
+ *   hyp_out [n_streams][max_ids], hyp_len_out / fixed_len_out [n_streams]: every stream's hypothesis after the push
+ * asrb_last_logprobs / _top_logprobs / asrb_last_timings / asrb_session_stats describe the push's run, one row per
+ * stream (idle streams: no ids). */
+ASRB_API int asrb_stream_push(asrb_session* s, int n_streams, const float* const* samples, const int64_t* n_samples,
+                              const int32_t* is_final, const int64_t* const* lang_ids, const int32_t* n_lang_ids,
+                              int max_new_tokens, int max_ids, int32_t* hyp_out, int32_t* hyp_len_out,
+                              int32_t* fixed_len_out);
+/* stream b's mel [128][F] (F = ceil(n / 160)) and encoder output [T][output_dim] after its last push */
+ASRB_API int asrb_stream_mel_read(asrb_session* s, int stream, float* out);
+ASRB_API int asrb_stream_encode_read(asrb_session* s, int stream, float* out);
+/* counters of the last push, summed over its streams: [0] windows encoded  [1] windows reused  [2] windows re-encoded
+ * because the mel floor moved  [3] prompt rows computed  [4] prompt rows kept from earlier pushes */
+ASRB_API int asrb_last_stream_stats(asrb_session* s, int64_t* out, int n);
+
 /* debug (ASRB_MEGA_DEBUG=1): clock64 timeline of the last fused decode step, CTA 0 then CTA G-1;
  * returns the number of slots per CTA (0 if disabled) */
 ASRB_API int asrb_debug_mega_timeline(long long* out, int cap);

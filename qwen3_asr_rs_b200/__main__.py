@@ -11,12 +11,14 @@ recognition towards its words (names, jargon, a keyword list).
 `--no-repeat-ngram N` (N in 0..16) bans every token that would repeat an N-gram of the tokens generated so far, and
 `--repetition-penalty P` (P in [1, 10]) penalises the logits of tokens generated so far; both anywhere on the line.
 `--max-segment S` (seconds, anywhere on the line) cuts the recording at quiet points into segments of at most S seconds,
-decodes them as batches and prints a `Segments:` block of `[start - end] text` lines."""
+decodes them as batches and prints a `Segments:` block of `[start - end] text` lines.
+`--stream S` (seconds, anywhere on the line) replays the file as a live stream in pushes of S seconds and prints each
+push's fixed and unfixed text (`[t] fixed | unfixed`), then the final transcript."""
 import sys
 
 USAGE = ("Usage: python -m qwen3_asr_rs_b200 <model_dir> <audio_file> [language] [--logprobs] [--top-logprobs N] "
          "[--temperature T[,T...]] [--seed N] [--beam-size N] [--length-penalty A] [--context TEXT | --context-file PATH] "
-         "[--no-repeat-ngram N] [--repetition-penalty P] [--max-segment S] [--score TEXT | --detect-language]")
+         "[--no-repeat-ngram N] [--repetition-penalty P] [--max-segment S | --stream S] [--score TEXT | --detect-language]")
 
 
 def parse_args(argv):
@@ -183,6 +185,38 @@ def split_max_segment(argv):
     return m[0], s
 
 
+def split_stream(argv):
+    """Remove `--stream S` from argv -> (remaining argv, S in seconds; None when absent), or None when the value is
+    missing or not a push length in whole 10 ms from 0.1 s to 30 s."""
+    m = _take_flag(argv, "--stream")
+    if m is None:
+        return None
+    if m[1] is None:
+        return m[0], None
+    try:
+        s = float(m[1])
+    except ValueError:
+        return None
+    if not (0.1 <= s <= 30.0) or abs(s * 100 - round(s * 100)) > 1e-6:
+        return None
+    return m[0], s
+
+
+STREAM_PART_S = 30.0          # a recording is streamed in parts of at most this long, each a stream of its own
+
+
+def stream_pushes(n_samples: int, push_s: float):
+    """(start, end, final) sample ranges of the pushes replaying n_samples in pushes of push_s seconds.  A part's last
+    push is final: the stream ends there, and the next part is a new stream."""
+    step = int(round(push_s * 16000))
+    per_part = max(1, int(STREAM_PART_S * 16000) // step)
+    out = []
+    for k, a in enumerate(range(0, n_samples, step)):
+        b = min(a + step, n_samples)
+        out.append((a, b, b == n_samples or (k + 1) % per_part == 0))
+    return out
+
+
 def format_segment(start_s: float, end_s: float, text: str) -> str:
     """One line of the `Segments:` block."""
     return f"  [{start_s:.2f} - {end_s:.2f}] {text}"
@@ -200,6 +234,11 @@ def main(argv=None) -> int:
         print(USAGE, file=sys.stderr)
         return 1
     argv, max_segment = seg
+    sm = split_stream(argv)
+    if sm is None or (sm[1] is not None and max_segment is not None):
+        print(USAGE, file=sys.stderr)
+        return 1
+    argv, stream_s = sm
     sc = split_score(argv)
     if sc is None:
         print(USAGE, file=sys.stderr)
@@ -218,6 +257,12 @@ def main(argv=None) -> int:
     top = split[1]
     _, beam_size, length_penalty = beam
     temperature = sampling[1]
+    if stream_s is not None and (score_text is not None or detect or logprobs or top or beam_size > 1
+                                 or isinstance(temperature, tuple)):
+        print("--stream cannot be combined with --score, --detect-language, --logprobs, --top-logprobs, --beam-size or "
+              "a temperature schedule", file=sys.stderr)
+        print(USAGE, file=sys.stderr)
+        return 1
     if beam_size > 1 and (top or (temperature is not None and not isinstance(temperature, tuple) and temperature > 0)):
         print("--beam-size > 1 cannot be combined with --top-logprobs or a temperature > 0", file=sys.stderr)
         print(USAGE, file=sys.stderr)
@@ -228,6 +273,11 @@ def main(argv=None) -> int:
         eng.close()
         print(f"--score / --detect-language need tokenizer.json in {model_dir}", file=sys.stderr)
         return 1
+    if stream_s is not None:
+        try:
+            return _stream_file(eng, audio, language, stream_s, ctx[1] or None, rep, sampling)
+        finally:
+            eng.close()
     if score_text is not None or detect:
         try:
             if detect:
@@ -276,6 +326,34 @@ def main(argv=None) -> int:
         print("Segments:")
         for start_s, end_s, text in r.segments:
             print(format_segment(start_s, end_s, text))
+    return 0
+
+
+def _stream_file(eng, audio: str, language, push_s: float, context, rep, sampling) -> int:
+    """--stream: the file's 16 kHz samples (GPU ingest) pushed as live streams of at most STREAM_PART_S each."""
+    from .audio import read_wav_pcm
+    from .text import join_segment_texts
+    _, temperature, seed = sampling
+    pcm, rate = read_wav_pcm(audio)
+    x = eng.ingest_pcm([pcm], [rate])[0]
+    decode = eng.tokenizer.decode if eng.tokenizer is not None else (lambda ids: " ".join(str(i) for i in ids))
+    ss, start, texts = None, 0, []
+    for a, b, final in stream_pushes(len(x), push_s):
+        if ss is None:
+            ss = eng.open_streams(1, STREAM_PART_S + 0.02, language=language, context=context, temperature=temperature or 0.0,
+                                  seed=seed or 0, no_repeat_ngram_size=rep[1], repetition_penalty=rep[2])
+        if final and b < len(x) and len(x) - b <= 160:      # a stream needs > 160 samples: the last bit joins this part
+            b = len(x)
+        h = ss.push([x[a:b]], final=final)[0]
+        fixed = h.fixed_text if h.fixed_text is not None else decode(h.ids[: h.fixed])
+        text = h.text if h.text is not None else decode(h.ids)
+        print(f"[{b / 16000.0:.2f}] {fixed} | {text[len(fixed):] if text.startswith(fixed) else text}")
+        if final:
+            texts.append(text)
+            ss = None
+        if b == len(x):
+            break
+    print(f"Text: {join_segment_texts(texts, language)}")
     return 0
 
 

@@ -48,6 +48,14 @@ void session_last_prefill_stats(Session* s, int64_t* out, int n);
 void session_score_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* const* lang_ids,
                        const int32_t* n_lang_ids, const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
                        int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out);
+void session_stream_open(Session* s, int n_streams, int rollback, int unfixed);
+void session_stream_reset(Session* s, int b);
+void session_stream_push(Session* s, int nst, const float* const* samples, const int64_t* n_samples, const int32_t* is_final,
+                         const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens, int max_ids,
+                         int32_t* hyp_out, int32_t* hyp_len_out, int32_t* fixed_len_out);
+void session_stream_mel_read(Session* s, int b, float* out);
+void session_stream_encode_read(Session* s, int b, float* out);
+void session_last_stream_stats(Session* s, int64_t* out, int n);
 int decode_mega_debug_timeline(long long* out, int cap);
 int decode_batch_debug_timeline(long long* out, int cap);
 }  // namespace asrb
@@ -275,6 +283,27 @@ int asrb_score_ingested(asrb_session* s, const int64_t* const* lang_ids, const i
     return guarded([&] { NONNULL(s);
                          session_score_ids(s->s, nullptr, nullptr, 0, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len,
                                            max_new_tokens, logprob_out, top_ids_out, top_lp_out); });
+}
+
+int asrb_stream_open(asrb_session* s, int n_streams, int rollback_ids, int unfixed_pushes) {
+    return guarded([&] { NONNULL(s); session_stream_open(s->s, n_streams, rollback_ids, unfixed_pushes); });
+}
+int asrb_stream_reset(asrb_session* s, int stream) { return guarded([&] { NONNULL(s); session_stream_reset(s->s, stream); }); }
+int asrb_stream_push(asrb_session* s, int n_streams, const float* const* samples, const int64_t* n_samples, const int32_t* is_final,
+                     const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens, int max_ids,
+                     int32_t* hyp_out, int32_t* hyp_len_out, int32_t* fixed_len_out) {
+    return guarded([&] { NONNULL(s); NONNULL(n_samples); NONNULL(hyp_out); NONNULL(hyp_len_out); NONNULL(fixed_len_out);
+                         session_stream_push(s->s, n_streams, samples, n_samples, is_final, lang_ids, n_lang_ids, max_new_tokens,
+                                             max_ids, hyp_out, hyp_len_out, fixed_len_out); });
+}
+int asrb_stream_mel_read(asrb_session* s, int stream, float* out) {
+    return guarded([&] { NONNULL(s); NONNULL(out); session_stream_mel_read(s->s, stream, out); });
+}
+int asrb_stream_encode_read(asrb_session* s, int stream, float* out) {
+    return guarded([&] { NONNULL(s); NONNULL(out); session_stream_encode_read(s->s, stream, out); });
+}
+int asrb_last_stream_stats(asrb_session* s, int64_t* out, int n) {
+    return guarded([&] { NONNULL(s); NONNULL(out); session_last_stream_stats(s->s, out, n); });
 }
 
 int asrb_debug_mega_timeline(long long* out, int cap) {

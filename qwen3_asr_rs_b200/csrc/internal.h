@@ -148,6 +148,14 @@ void launch_gemm_simt(const GemmA& A, const bf16* W, int N, const GemmEpi& E, cu
 void launch_mel(const Model& m, const float* samples, const int64_t* d_soff, const int64_t* d_n,
                 const int64_t* d_npad, const int64_t* d_foff, int batch, int max_frames,
                 float* mel_out, int* d_maxkey, cudaStream_t st);
+// streaming (DESIGN.md 4.9): frames [ffirst[b], F_b) of stream b into its raw log-mel rows (raw + b * n_mels * ldo), then
+// the fold of the frames that became final (d_fold[b] = {f_old, f_new, F, active}) into stats row b
+void launch_mel_stream(const Model& m, const float* samples, const int64_t* d_soff, const int64_t* d_n, const int64_t* d_npad,
+                       const int64_t* d_foff, const int* d_ffirst, int n_streams, int max_new_frames, int ldo, float* raw,
+                       const int4* d_fold, int win_frames, float* stats, int stats_ld, cudaStream_t st);
+// the re-encoded windows as clamped, scaled pseudo-utterances (d_plan[u] = {slot, first frame, frames, phi bits})
+void launch_mel_stream_stage(const Model& m, const float* raw, const int4* d_plan, const int64_t* d_foff, int n_utt, int ldo,
+                             float* mel_out, cudaStream_t st);
 // segment.cu: window energies and cut points of the long-audio files (DESIGN.md section 4.6)
 void launch_segment(const float* d_long, const int64_t* d_plan, int n_files, int64_t total_blocks, int64_t max_seg,
                     int64_t search, double* d_blk, int64_t* d_cuts, int64_t* d_ncuts, int sm_count, cudaStream_t st);

@@ -22,13 +22,18 @@ namespace asrb {
 
 static constexpr int NFFT = 400, HOP = 160, NBIN = 201, KP = 208, FT = 16, MEL_THREADS = 224;
 
+// STREAM: utterance b's frames [ffirst[b], F) only, rows of ldo floats, no running max (the streams' raw log-mel store,
+// folded by mel_stream_fold_kernel).  A frame's arithmetic does not depend on the 16-frame block it falls in, so a frame
+// computed here is bitwise the offline one.  The offline instantiation passes neither and compiles to the same SASS.
+template <bool STREAM>
 __global__ void __launch_bounds__(MEL_THREADS)
 mel_power_kernel(const float* __restrict__ samples, const int64_t* __restrict__ soff,
                  const int64_t* __restrict__ n_true, const int64_t* __restrict__ n_pad,
                  const int64_t* __restrict__ foff, const float* __restrict__ hann,
                  const float2* __restrict__ tw,
                  const float* __restrict__ fb, const int* __restrict__ krange, int n_mels,
-                 float* __restrict__ mel_out, int* __restrict__ maxkey) {
+                 float* __restrict__ mel_out, int* __restrict__ maxkey,
+                 const int* __restrict__ ffirst = nullptr, int ldo = 0) {
     constexpr int NH = NFFT / 2;                           // 200
     __shared__ __align__(16) float buf[(2 * NH + 1) * FT];
     float (*xe)[FT] = reinterpret_cast<float (*)[FT]>(buf);                   // xe[n] = x[n] + x[400-n] (n = 1..199); xe[0] = x[0]; xe[200] = x[200]
@@ -40,7 +45,7 @@ mel_power_kernel(const float* __restrict__ samples, const int64_t* __restrict__ 
     const int b = blockIdx.y;
     const int64_t npad = n_pad[b], ntrue = n_true[b];
     const int F = (int)(npad / HOP);
-    const int f0 = blockIdx.x * FT;
+    const int f0 = (STREAM ? ffirst[b] : 0) + blockIdx.x * FT;
     if (f0 >= F) return;
     const float* x = samples + soff[b];
     for (int i = threadIdx.x; i < NFFT; i += MEL_THREADS) tws[i] = tw[i];
@@ -97,12 +102,14 @@ mel_power_kernel(const float* __restrict__ samples, const int64_t* __restrict__ 
         for (int kk = k0; kk < k1; ++kk) acc = fmaf(fb[m * NBIN + kk], pw[fi][kk], acc);
         float v = log10f(fmaxf(acc, 1e-10f));                     // clamp_min(1e-10).log10()
         if (f < F) {
-            out[(size_t)m * F + f] = v;
+            out[(size_t)m * (STREAM ? ldo : F) + f] = v;
             lmax = fmaxf(lmax, v);
         }
     }
-    lmax = block_max(lmax, red);
-    if (threadIdx.x == 0) atomicMax(&maxkey[b], float_to_ordered(lmax));
+    if constexpr (!STREAM) {
+        lmax = block_max(lmax, red);
+        if (threadIdx.x == 0) atomicMax(&maxkey[b], float_to_ordered(lmax));
+    }
 }
 
 __global__ void mel_finalize_kernel(float* __restrict__ mel, const int64_t* __restrict__ foff,
@@ -129,11 +136,83 @@ void launch_mel(const Model& m, const float* samples, const int64_t* d_soff, con
                 float* mel_out, int* d_maxkey, cudaStream_t st) {
     mel_init_max_kernel<<<(batch + 127) / 128, 128, 0, st>>>(d_maxkey, batch);
     dim3 grid((max_frames + FT - 1) / FT, batch);
-    mel_power_kernel<<<grid, MEL_THREADS, 0, st>>>(samples, d_soff, d_n, d_npad, d_foff, m.hann,
+    mel_power_kernel<false><<<grid, MEL_THREADS, 0, st>>>(samples, d_soff, d_n, d_npad, d_foff, m.hann,
                                                    reinterpret_cast<const float2*>(m.dft_tw), m.mel_fb, m.mel_krange,
                                                    m.d.c.num_mel_bins, mel_out, d_maxkey);
     dim3 g2(132, batch);                                          // one CTA per H100 SM per clip
     mel_finalize_kernel<<<g2, 256, 0, st>>>(mel_out, d_foff, d_npad, m.d.c.num_mel_bins, d_maxkey);
+    ASRB_CUDA_CHECK(cudaGetLastError());
+}
+
+// ---- streaming (DESIGN.md 4.9) ----
+// one CTA per stream: frames [f_old, f_new) became final this push -- fold them into the stream's final maximum and into
+// the minima of their encoder windows (win_frames frames each); the maximum over the provisional frames [f_new, F) is
+// written beside them.  stats row b: [0] final max  [1] provisional max (-inf: none)  [2 + w] minimum of window w.
+// max / min are exact in any order, so the values do not depend on the reduction order.
+__global__ void mel_stream_fold_kernel(const float* __restrict__ raw, const int4* __restrict__ plan, int n_mels, int ldo,
+                                       int win_frames, float* __restrict__ stats, int stats_ld) {
+    __shared__ float red[32];
+    const int b = blockIdx.x;
+    const int4 q = plan[b];                                     // {f_old, f_new, F, active}
+    if (!q.w) return;
+    const float* r = raw + (size_t)b * n_mels * ldo;
+    float* out = stats + (size_t)b * stats_ld;
+    auto range_max = [&](int f0, int f1, float sign) {          // max of sign * v over frames [f0, f1) of every mel row
+        float v = -INFINITY;
+        const int nf = f1 - f0;
+        for (int i = threadIdx.x; i < n_mels * nf; i += blockDim.x) {
+            const int m = i / nf, f = f0 + (i - m * nf);
+            v = fmaxf(v, sign * r[(size_t)m * ldo + f]);
+        }
+        return block_max(v, red);
+    };
+    if (q.y > q.x) {
+        const float fm = range_max(q.x, q.y, 1.f);
+        if (threadIdx.x == 0) out[0] = fmaxf(out[0], fm);
+        for (int w = q.x / win_frames; w * win_frames < q.y; ++w) {
+            const float mn = -range_max(max(q.x, w * win_frames), min(q.y, (w + 1) * win_frames), -1.f);
+            if (threadIdx.x == 0) out[2 + w] = fminf(out[2 + w], mn);
+        }
+    }
+    const float tm = q.z > q.y ? range_max(q.y, q.z, 1.f) : -INFINITY;
+    if (threadIdx.x == 0) out[1] = tm;
+}
+
+// the re-encoded windows of a push as pseudo-utterances for the encoder: utterance u = frames [fs, fs + Fu) of stream
+// slot's raw log-mel, clamped at the stream's floor phi and scaled as mel_finalize_kernel does, written [n_mels][Fu] at
+// frame offset foff[u] of mel_out.  plan row u: {slot, fs, Fu, float bits of phi}
+__global__ void mel_stream_stage_kernel(const float* __restrict__ raw, const int4* __restrict__ plan,
+                                        const int64_t* __restrict__ foff, int n_mels, int ldo, float* __restrict__ mel_out) {
+    const int u = blockIdx.y;
+    const int4 q = plan[u];
+    const float floor_v = __int_as_float(q.w);
+    const float* r = raw + (size_t)q.x * n_mels * ldo + q.y;
+    float* p = mel_out + (size_t)n_mels * foff[u];
+    const int64_t total = (int64_t)n_mels * q.z;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int m = (int)(i / q.z), f = (int)(i - (int64_t)m * q.z);
+        const float v = fmaxf(r[(size_t)m * ldo + f], floor_v);
+        p[i] = (v + 4.0f) / 4.0f;
+    }
+}
+
+void launch_mel_stream(const Model& m, const float* samples, const int64_t* d_soff, const int64_t* d_n, const int64_t* d_npad,
+                       const int64_t* d_foff, const int* d_ffirst, int n_streams, int max_new_frames, int ldo, float* raw,
+                       const int4* d_fold, int win_frames, float* stats, int stats_ld, cudaStream_t st) {
+    if (max_new_frames > 0) {
+        dim3 grid((max_new_frames + FT - 1) / FT, n_streams);
+        mel_power_kernel<true><<<grid, MEL_THREADS, 0, st>>>(samples, d_soff, d_n, d_npad, d_foff, m.hann,
+                                                             reinterpret_cast<const float2*>(m.dft_tw), m.mel_fb, m.mel_krange,
+                                                             m.d.c.num_mel_bins, raw, nullptr, d_ffirst, ldo);
+    }
+    mel_stream_fold_kernel<<<n_streams, 256, 0, st>>>(raw, d_fold, m.d.c.num_mel_bins, ldo, win_frames, stats, stats_ld);
+    ASRB_CUDA_CHECK(cudaGetLastError());
+}
+
+void launch_mel_stream_stage(const Model& m, const float* raw, const int4* d_plan, const int64_t* d_foff, int n_utt, int ldo,
+                             float* mel_out, cudaStream_t st) {
+    dim3 grid(32, n_utt);
+    mel_stream_stage_kernel<<<grid, 256, 0, st>>>(raw, d_plan, d_foff, m.d.c.num_mel_bins, ldo, mel_out);
     ASRB_CUDA_CHECK(cudaGetLastError());
 }
 

@@ -120,6 +120,31 @@ struct Session {
         float* lp = nullptr; int* tk_ids = nullptr; float* tk_lp = nullptr;
         int* h_int = nullptr; int* d_int = nullptr; size_t int_cap = 0;   // row plan | per-slot arrays | score rows
     } sc;
+    // streaming (asrb_stream_*, DESIGN.md 4.9): stream b lives in KV slot b; its buffers are allocated by the first open
+    struct Stream {
+        int64_t n = 0;                  // samples received, in str_samples row b
+        int k = 0;                      // pushes that gave it samples
+        bool closed = false;            // its final push is done
+        std::vector<int> p, hyp, ctx;   // forced prefix, last hypothesis, context latched when the stream started
+        int fixed = 0;                  // fixed length of hyp (= |p|)
+        int Ffin = 0;                   // final mel frames, folded into stats row b
+        float phi = 0.f;                // mel floor of the last push
+        int T = 0;                      // audio tokens in token-store row b
+        int kv_valid = 0;               // prompt positions whose K/V in slot b are those of the stream's current audio
+        std::vector<float> win_phi;     // per encoder window: the floor it was last encoded under
+        std::vector<char> win_final;    //   and whether all its frames were final then
+    };
+    std::vector<Stream> streams;
+    bool streams_open = false;
+    bool stream_run = false;            // the last run was a push: the stage-level reads describe no offline batch
+    int str_rollback = 5, str_unfixed = 2, str_maxW = 0, str_stats_ld = 0;
+    float* str_samples = nullptr;       // [max_batch][max_npad] 16 kHz samples
+    float* str_raw = nullptr;           // [max_batch][n_mels][maxF] raw (pre-floor) log-mel
+    float* str_tok = nullptr;           // [max_batch][maxT][output_dim] encoder output
+    float* str_stats = nullptr;         // [max_batch][2 + maxW] fold results (mel_stream_fold_kernel)
+    float* h_str_stats = nullptr;
+    int *str_int = nullptr, *h_str_int = nullptr; size_t str_int_cap = 0;   // fold plan | first frames | staging plan
+    int64_t str_counts[5] = {0, 0, 0, 0, 0};   // last push: windows encoded / reused / re-encoded for the floor, rows computed / kept
     ~Session();
 };
 
@@ -138,6 +163,8 @@ Session::~Session() {
     if (h_nout) cudaFreeHost(h_nout);
     if (h_next) cudaFreeHost(h_next);
     if (sc.h_int) cudaFreeHost(sc.h_int);
+    if (h_str_stats) cudaFreeHost(h_str_stats);
+    if (h_str_int) cudaFreeHost(h_str_int);
     if (ingest) ingest_state_free(ingest);
     if (st) cudaStreamDestroy(st);
 }
@@ -295,6 +322,7 @@ static void mel_impl(Session* s, const float* const* samples, const int64_t* n_s
     const bool ingested = (samples == nullptr) && !views;   // samples already in HBM, written by asrb_ingest_pcm
     if (ingested) ASRB_REQUIRE((int)s->ingested_n.size() == batch, ASRB_ERR_STATE, "no ingested audio for this batch");
     s->B = batch; s->stage = 0;
+    s->streams_open = false; s->stream_run = false;     // every call that starts from audio ends the streams
     s->n.assign(batch, 0); s->npad.assign(batch, 0); s->F.assign(batch, 0); s->foff.assign(batch, 0); s->soff.assign(batch, 0);
     int64_t so = 0, fo = 0; int maxF = 0;
     for (int b = 0; b < batch; ++b) {
@@ -425,7 +453,7 @@ void session_segment_long(Session* s, int64_t max_seg, int64_t search, int max_s
 }
 
 void session_mel_read(Session* s, int b, float* out) {
-    ASRB_REQUIRE(s->stage >= 1 && b >= 0 && b < s->B, ASRB_ERR_STATE, "mel_read: no mel for this index");
+    ASRB_REQUIRE(s->stage >= 1 && !s->stream_run && b >= 0 && b < s->B, ASRB_ERR_STATE, "mel_read: no mel for this index");
     ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
     const int nm = s->m->d.c.num_mel_bins;
     ASRB_CUDA_CHECK(cudaMemcpy(out, s->d_mel + (size_t)nm * s->foff[b], (size_t)nm * s->F[b] * sizeof(float), cudaMemcpyDeviceToHost));
@@ -439,7 +467,7 @@ static GemmA plainA(const bf16* a, size_t ps, int M, int K, int nplanes) {
 }
 
 void session_encode(Session* s, int64_t* n_tokens_out) {
-    ASRB_REQUIRE(s->stage >= 1, ASRB_ERR_STATE, "encode called before mel");
+    ASRB_REQUIRE(s->stage >= 1 && !s->stream_run, ASRB_ERR_STATE, "encode called before mel");
     Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
     const int B = s->B, tpc = d.tok_per_chunk, cf = d.chunk_frames;
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
@@ -542,7 +570,7 @@ void session_encode(Session* s, int64_t* n_tokens_out) {
 }
 
 void session_encode_read(Session* s, int b, float* out) {
-    ASRB_REQUIRE(s->stage >= 2 && b >= 0 && b < s->B, ASRB_ERR_STATE, "encode_read: nothing encoded for this index");
+    ASRB_REQUIRE(s->stage >= 2 && !s->stream_run && b >= 0 && b < s->B, ASRB_ERR_STATE, "encode_read: nothing encoded for this index");
     ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
     const int od = s->m->d.c.output_dim;
     ASRB_CUDA_CHECK(cudaMemcpy(out, s->audio + (size_t)s->toff[b] * od, (size_t)s->T[b] * od * sizeof(float), cudaMemcpyDeviceToHost));
@@ -633,25 +661,41 @@ void session_last_prefill_stats(Session* s, int64_t* out, int n) {
     for (int i = 0; i < n && i < 3; ++i) out[i] = v[i];
 }
 
-// utterance b's whole prompt, position by position (s->S[b] positions): ids, and the audio row of each audio position
-// (-1 elsewhere)
-static void build_prompt(const Session* s, int b, const int64_t* const* lang_ids, std::vector<int>& pid, std::vector<int>& parow) {
-    const std::vector<int>& cb = context_of(s, b);
+// a whole prompt, position by position: ids, and the audio row of each audio position (-1 elsewhere).  Head, context,
+// end of the system turn and start of the user turn, T audio pads reading rows arow0 .. arow0 + T - 1, the tail, the nl
+// language ids, then the forced prefix of a stream
+static void build_prompt(const std::vector<int>& ctx, int T, int arow0, const int64_t* lang, int nl, const std::vector<int>& forced,
+                         std::vector<int>& pid, std::vector<int>& parow) {
     pid.clear(); parow.clear();
     for (int i = 0; i < 3; ++i) { pid.push_back(kPromptHead[i]); parow.push_back(-1); }
-    for (int id : cb) { pid.push_back(id); parow.push_back(-1); }
+    for (int id : ctx) { pid.push_back(id); parow.push_back(-1); }
     for (int i = 3; i < 9; ++i) { pid.push_back(kPromptHead[i]); parow.push_back(-1); }
-    for (int t = 0; t < s->T[b]; ++t) { pid.push_back(kAudioPad); parow.push_back(s->toff[b] + t); }
+    for (int t = 0; t < T; ++t) { pid.push_back(kAudioPad); parow.push_back(arow0 + t); }
     for (int i = 0; i < 6; ++i) { pid.push_back(kPromptTail[i]); parow.push_back(-1); }
-    for (int i = 0, nl = s->S[b] - (int)pid.size(); i < nl; ++i) { pid.push_back((int)lang_ids[b][i]); parow.push_back(-1); }
+    for (int i = 0; i < nl; ++i) { pid.push_back((int)lang[i]); parow.push_back(-1); }
+    for (int id : forced) { pid.push_back(id); parow.push_back(-1); }
+}
+// utterance b's prompt of the current offline batch (s->S[b] positions)
+static void build_prompt(const Session* s, int b, const int64_t* const* lang_ids, std::vector<int>& pid, std::vector<int>& parow) {
+    const std::vector<int>& cb = context_of(s, b);
+    const int nl = s->S[b] - (15 + (int)cb.size() + s->T[b]);
+    build_prompt(cb, s->T[b], s->toff[b], nl > 0 ? lang_ids[b] : nullptr, nl, {}, pid, parow);
+}
+// positions [from, |pid|) of a prompt into the row plan from row r0, as rows of sequence (KV slot) q; returns the next row
+static int plan_prompt_rows(const std::vector<int>& pid, const std::vector<int>& parow, int from, int r0, int q, int* ids,
+                            int* arow, int* rseq, int* rpos) {
+    int r = r0;
+    for (int i = from; i < (int)pid.size(); ++i, ++r) { ids[r] = pid[i]; arow[r] = parow[i]; rseq[r] = q; rpos[r] = i; }
+    return r;
 }
 
 // embed + inject and the decoder layers over the planned rows (s->d_ids ..., totS rows; sequence q's rows are its
-// segment of the attention, in KV slot q)
-static void prefill_layers(Session* s, int totS, int nseq, int maxrows, const FanOut* fan, const int* d_qpos0) {
+// segment of the attention, in KV slot q); audio rows are read from `audio`
+static void prefill_layers(Session* s, int totS, int nseq, int maxrows, const FanOut* fan, const int* d_qpos0,
+                           const float* audio) {
     Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
     cudaStream_t st = s->st; const int np = s->nplanes;
-    launch_embed_inject(m.embed, c.hidden_size, s->d_ids, s->d_audio_row, s->audio, totS, s->hid, st);
+    launch_embed_inject(m.embed, c.hidden_size, s->d_ids, s->d_audio_row, audio, totS, s->hid, st);
     s->launches += 1;
     const int H = c.hidden_size; const float eps = (float)c.rms_norm_eps;
     for (int l = 0; l < c.num_hidden_layers; ++l) {
@@ -685,10 +729,14 @@ static void prefill_layers(Session* s, int totS, int nseq, int maxrows, const Fa
     }
 }
 
+static void begin_run(Session* s, int B, const int* d_done0);
+static void first_token(Session* s, int B, bool write_logits, const int* pos0);
+
 void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, int64_t* seq_lens_out,
                      float* last_logits) {
-    ASRB_REQUIRE(s->stage >= 2, ASRB_ERR_STATE, "prefill called before encode");
+    ASRB_REQUIRE(s->stage >= 2 && !s->stream_run, ASRB_ERR_STATE, "prefill called before encode");
     check_sampling_options(s, s->B);
+    s->streams_open = false;                        // the prefill overwrites the streams' K/V slots
     check_context(s, s->B);
     Model& m = *s->m; const asrb_dims& c = m.d.c;
     const int B = s->B; cudaStream_t st = s->st;
@@ -730,7 +778,7 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     for (int b = 0; b < B; ++b) {
         build_prompt(s, b, lang_ids, pid, parow);
         // rows from position skip[b] on (build_position_ids :259-266: position = index in the prompt)
-        for (int i = skip[b], r = s->srow0[b]; i < s->S[b]; ++i, ++r) { ids[r] = pid[i]; arow[r] = parow[i]; rseq[r] = b; rpos[r] = i; }
+        plan_prompt_rows(pid, parow, skip[b], s->srow0[b], b, ids, arow, rseq, rpos);
         const int rows = s->S[b] - skip[b];
         sq0[b] = s->srow0[b]; slen[b] = rows; lastrow[b] = s->srow0[b] + rows - 1; pos0[b] = s->S[b] - 1; qpos0[b] = skip[b];
         shared += skip[b];
@@ -752,7 +800,23 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     const int* d_qpos0 = fan ? di + (qpos0 - hi) : nullptr;   // no follower: the plan and kernels of a call without contexts
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_lastrow, di + (lastrow - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
     ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.pos, di + (pos0 - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.done, 0, B * sizeof(int), st));
+    begin_run(s, B, nullptr);
+    prefill_layers(s, totS, B, maxrows, fan ? &fan_plan : nullptr, d_qpos0, s->audio);
+    first_token(s, B, last_logits != nullptr, di + (pos0 - hi));
+    if (seq_lens_out) for (int b = 0; b < B; ++b) seq_lens_out[b] = s->S[b];
+    if (last_logits) {
+        ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
+        ASRB_CUDA_CHECK(cudaMemcpy(last_logits, s->db.logits, (size_t)B * c.vocab_size * sizeof(float), cudaMemcpyDeviceToHost));
+    }
+    s->stage = 3;
+}
+
+// the result rows of the run's B sequences reset (done from d_done0 when given, else 0) and its record, sampling and
+// top-k options latched; before the prefill
+static void begin_run(Session* s, int B, const int* d_done0) {
+    cudaStream_t st = s->st;
+    if (d_done0) ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.done, d_done0, B * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    else ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.done, 0, B * sizeof(int), st));
     ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.n_out, 0, B * sizeof(int), st));
     s->lp_valid = s->opt_logprobs || s->top_k > 0;   // latched here: a run records log-probabilities only if it starts with the option on
     if (s->db.logprobs) {                  // all NaN (0xFFFFFFFF): no EOS seen, nothing appended
@@ -774,15 +838,19 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
         ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.tk_eos_ids, 0xFF, (size_t)B * TK_MAX * sizeof(int), st));
         ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.tk_eos_lp, 0xFF, (size_t)B * TK_MAX * sizeof(float), st));
     }
+}
 
-    prefill_layers(s, totS, B, maxrows, fan ? &fan_plan : nullptr, d_qpos0);
+// token 0 of every sequence from its last prefill row (s->d_lastrow), then the repetition rule latched for the steps;
+// pos0: the prompt lengths minus one, for the beam run's token-0 walk
+static void first_token(Session* s, int B, bool write_logits, const int* pos0) {
+    Model& m = *s->m; cudaStream_t st = s->st;
     // final norm + lm_head on the last row of each utterance only (the reference computes all S rows,
     // text_decoder.rs:111-112, and uses row S-1, inference.rs:156)
-    launch_lmhead_argmax(m, s->hid, s->d_lastrow, B, s->db, last_logits != nullptr, st, &s->launches);
+    launch_lmhead_argmax(m, s->hid, s->d_lastrow, B, s->db, write_logits, st, &s->launches);
     // greedy bookkeeping for token 0 (inference.rs:161-170): argmax, EOS check, append, embed
     launch_greedy(m, s->db, B, st, &s->launches);
     // beam search: the token-0 walk on each utterance's record, then its prompt KV copied into its other K - 1 slots
-    if (s->run_k > 1) launch_beam_step(beam_args(s), true, di + (pos0 - hi), st, &s->launches);
+    if (s->run_k > 1) launch_beam_step(beam_args(s), true, pos0, st, &s->launches);
     s->greedy_done = 1;
     s->db.rep = s->ngram > 0 || s->rep_penalty != 1.0;   // latched: every decode step of the run applies this run's rule
     if (s->db.rep) {
@@ -790,14 +858,8 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
         ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_rep, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
         if (!s->db.rep_mask)                // per-phase: [max_batch][2][vocab words]; fused steps: [G][up to 16][2][CTA words]
             s->db.rep_mask = salloc<uint32_t>(s, std::max((size_t)s->max_batch * 2 * s->db.rep_words,
-                                                          (size_t)m.ctx->sm_count * 16 * 2 * rep_cta_words(c, m.ctx->sm_count)));
+                                                          (size_t)m.ctx->sm_count * 16 * 2 * rep_cta_words(m.d.c, m.ctx->sm_count)));
     }
-    if (seq_lens_out) for (int b = 0; b < B; ++b) seq_lens_out[b] = s->S[b];
-    if (last_logits) {
-        ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
-        ASRB_CUDA_CHECK(cudaMemcpy(last_logits, s->db.logits, (size_t)B * c.vocab_size * sizeof(float), cudaMemcpyDeviceToHost));
-    }
-    s->stage = 3;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1166,7 +1228,7 @@ static void score_impl(Session* s, const float* const* samples, const int64_t* n
         int r = srow0[q];
         if (leader) {
             build_prompt(s, b, lang_ids, pid, parow);
-            for (int i = 0; i < Sb; ++i, ++r) { ids[r] = pid[i]; arow[r] = parow[i]; rseq[r] = q; rpos[r] = i; }
+            r = plan_prompt_rows(pid, parow, 0, r, q, ids, arow, rseq, rpos);
         }
         for (int i = 0; i + 1 < cand_len[q]; ++i, ++r) { ids[r] = (int)cand_ids[q][i]; arow[r] = -1; rseq[r] = q; rpos[r] = Sb + i; }
         sq0[q] = srow0[q]; slen[q] = rows[q]; qpos0[q] = leader ? 0 : Sb;
@@ -1190,7 +1252,7 @@ static void score_impl(Session* s, const float* const* samples, const int64_t* n
     s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
     const FanOut fan_plan{di + (fan_n - hi), di + (fan_off - hi), di + (fan_P - hi), di + (fan_slots - hi)};
     const bool fan = nf > 0;
-    prefill_layers(s, totS, N, maxrows, fan ? &fan_plan : nullptr, fan ? di + (qpos0 - hi) : nullptr);
+    prefill_layers(s, totS, N, maxrows, fan ? &fan_plan : nullptr, fan ? di + (qpos0 - hi) : nullptr, s->audio);
     ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
     launch_score_head(m, s->hid, di + (src - hi), di + (tgt - hi), R, sb.gathered, sb.planes, (size_t)sb.rows_cap * c.hidden_size,
                       s->nplanes, sb.part, topk, sb.lp, sb.tk_ids, sb.tk_lp, st, &s->launches);
@@ -1224,6 +1286,310 @@ void session_score_ids(Session* s, const float* const* samples, const int64_t* n
                        int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out) {
     score_impl(s, samples, n_samples, batch, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len, max_new_tokens, logprob_out,
                top_ids_out, top_lp_out);
+}
+
+// -------------------------------------------------------------------------------------------------
+// streaming (asrb_stream_*, DESIGN.md 4.9): stream b in KV slot b; per push the mel of its new frames, the encoder over
+// the windows whose clamped mel may have changed, and the prefill from the first position those change
+// -------------------------------------------------------------------------------------------------
+static int stream_win_frames(const Session* s) {     // frames of one encoder window (the whole stream without windows)
+    const Dims& d = s->m->d;
+    return d.chunks_per_window > 0 ? d.chunk_frames * d.chunks_per_window : s->maxF;
+}
+
+static void stream_clear(Session* s, int b) {
+    Session::Stream& x = s->streams[b];
+    x = Session::Stream();
+    x.ctx = context_of(s, b);                        // latched when the stream starts
+    x.win_phi.assign(s->str_maxW, 0.f); x.win_final.assign(s->str_maxW, 0);
+    float* row = s->h_str_stats + (size_t)b * s->str_stats_ld;
+    row[0] = -INFINITY; row[1] = -INFINITY;
+    for (int w = 0; w < s->str_maxW; ++w) row[2 + w] = INFINITY;
+    ASRB_CUDA_CHECK(cudaMemcpy(s->str_stats + (size_t)b * s->str_stats_ld, row, s->str_stats_ld * sizeof(float), cudaMemcpyHostToDevice));
+}
+
+void session_stream_open(Session* s, int n_streams, int rollback, int unfixed) {
+    ASRB_REQUIRE(n_streams >= 1 && n_streams <= s->max_batch, ASRB_ERR_INVALID, "stream_open: n_streams must be in [1, max_batch]");
+    ASRB_REQUIRE(rollback >= 0 && unfixed >= 0, ASRB_ERR_INVALID, "stream_open: rollback_ids and unfixed_pushes must be >= 0");
+    check_context(s, n_streams);
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    s->streams_open = false;
+    if (!s->str_samples) {
+        const Dims& d = s->m->d; const size_t Bm = s->max_batch;
+        const int cpw = d.chunks_per_window;
+        s->str_maxW = cpw > 0 ? (s->maxC + cpw - 1) / cpw : 1;
+        s->str_stats_ld = 2 + s->str_maxW;
+        s->str_int_cap = 8 * Bm + 4 * Bm * s->str_maxW + 16;
+        AllocAll a;
+        float* smp = a.take<float>(Bm * s->max_npad);
+        float* raw = a.take<float>(Bm * d.c.num_mel_bins * s->maxF);
+        float* tok = a.take<float>(Bm * s->maxT * d.c.output_dim);
+        float* stats = a.take<float>(Bm * s->str_stats_ld);
+        int* pi = a.take<int>(s->str_int_cap);
+        float* hs = nullptr; int* hi = nullptr;
+        ASRB_CUDA_CHECK(cudaMallocHost(&hs, Bm * s->str_stats_ld * sizeof(float)));
+        if (cudaMallocHost(&hi, s->str_int_cap * sizeof(int)) != cudaSuccess) { cudaFreeHost(hs); throw Error(ASRB_ERR_CUDA, "stream_open: out of host memory"); }
+        a.commit(s);
+        s->str_samples = smp; s->str_raw = raw; s->str_tok = tok; s->str_stats = stats; s->str_int = pi;
+        s->h_str_stats = hs; s->h_str_int = hi;
+    }
+    s->str_rollback = rollback; s->str_unfixed = unfixed;
+    s->streams.assign(n_streams, Session::Stream());
+    for (int b = 0; b < n_streams; ++b) stream_clear(s, b);
+    for (auto& v : s->str_counts) v = 0;
+    s->streams_open = true;
+}
+
+void session_stream_reset(Session* s, int b) {
+    ASRB_REQUIRE(s->streams_open, ASRB_ERR_STATE, "stream_reset: no open streams");
+    ASRB_REQUIRE(b >= 0 && b < (int)s->streams.size(), ASRB_ERR_INVALID, "stream_reset: no such stream");
+    check_context(s, (int)s->streams.size());
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    stream_clear(s, b);
+}
+
+void session_stream_push(Session* s, int nst, const float* const* samples, const int64_t* n_samples, const int32_t* is_final,
+                         const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens, int max_ids,
+                         int32_t* hyp_out, int32_t* hyp_len_out, int32_t* fixed_len_out) {
+    ASRB_REQUIRE(s->streams_open, ASRB_ERR_STATE, "stream_push: no open streams (a non-stream call ends them)");
+    ASRB_REQUIRE(nst == (int)s->streams.size(), ASRB_ERR_INVALID, "stream_push: n_streams differs from asrb_stream_open's");
+    ASRB_REQUIRE(n_samples && hyp_out && hyp_len_out && fixed_len_out, ASRB_ERR_INVALID, "stream_push: null argument");
+    ASRB_REQUIRE(s->beam_k == 1, ASRB_ERR_INVALID, "stream_push: beam_size > 1 is not available on streams (streams own their slots)");
+    check_sampling_options(s, nst);
+    ASRB_REQUIRE(max_new_tokens >= 1 && max_new_tokens <= s->max_new, ASRB_ERR_INVALID, "max_new_tokens exceeds session capacity");
+    Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
+    const int cf = d.chunk_frames, cpw = d.chunks_per_window, od = c.output_dim;
+    const int Wf = stream_win_frames(s), Bm = s->max_batch;
+    // ---- every argument checked before any work ----
+    std::vector<char> act((size_t)nst, 0), fin((size_t)nst, 0);
+    std::vector<int> nl((size_t)nst, 0);
+    int n_act = 0;
+    for (int b = 0; b < nst; ++b) {
+        const Session::Stream& x = s->streams[b];
+        const int64_t nb = n_samples[b];
+        fin[b] = is_final && is_final[b];
+        act[b] = nb > 0 || fin[b];
+        ASRB_REQUIRE(nb >= 0 && (nb == 0 || (samples && samples[b])), ASRB_ERR_INVALID, "stream_push: bad samples");
+        ASRB_REQUIRE((int)x.hyp.size() <= max_ids, ASRB_ERR_INVALID, "stream_push: max_ids is below a stream's hypothesis");
+        if (!act[b]) continue;
+        ++n_act;
+        ASRB_REQUIRE(!x.closed, ASRB_ERR_STATE, "stream_push: stream " + std::to_string(b) + " is closed (asrb_stream_reset reopens it)");
+        ASRB_REQUIRE(x.n + nb <= s->max_samples, ASRB_ERR_INVALID, "stream_push: samples past the session's max_samples");
+        ASRB_REQUIRE(((x.n + nb + 159) / 160) * 160 > 200, ASRB_ERR_INVALID, "stream_push: a stream needs > 160 samples before its first push");
+        nl[b] = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
+        ASRB_REQUIRE(nl[b] >= 0 && nl[b] + (int)x.p.size() <= s->max_lang, ASRB_ERR_INVALID,
+                     "stream_push: language ids + forced prefix exceed the session's max_lang_ids");
+        for (int i = 0; i < nl[b]; ++i)
+            ASRB_REQUIRE(lang_ids[b][i] >= 0 && lang_ids[b][i] < c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
+        ASRB_REQUIRE((int)x.p.size() + max_new_tokens <= max_ids, ASRB_ERR_INVALID, "stream_push: max_ids < forced prefix + max_new_tokens");
+    }
+    ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
+    cudaStream_t st = s->st;
+    for (auto& v : s->str_counts) v = 0;
+    auto write_out = [&]() {
+        for (int b = 0; b < nst; ++b) {
+            const Session::Stream& x = s->streams[b];
+            for (size_t i = 0; i < x.hyp.size(); ++i) hyp_out[(size_t)b * max_ids + i] = x.hyp[i];
+            hyp_len_out[b] = (int32_t)x.hyp.size(); fixed_len_out[b] = x.fixed;
+        }
+    };
+    if (n_act == 0) { write_out(); return; }
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(st));     // the pinned plan buffers below may still feed an earlier copy
+    s->launches = 0; s->decode_steps = 0; s->stream_run = false; s->nbest_valid = false;
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
+    // ---- samples, then the mel of frames [Ffin, F) and the fold of the frames that became final ----
+    std::vector<int> F((size_t)nst, 0), Ffin((size_t)nst, 0);
+    int4* fold = reinterpret_cast<int4*>(s->h_str_int);
+    int* ffirst = s->h_str_int + 4 * Bm;
+    int64_t* h = s->h_i64;
+    int max_new_frames = 0;
+    for (int b = 0; b < nst; ++b) {
+        Session::Stream& x = s->streams[b];
+        const int64_t n = x.n + n_samples[b], np = ((n + 159) / 160) * 160;
+        if (n_samples[b] > 0)
+            ASRB_CUDA_CHECK(cudaMemcpyAsync(s->str_samples + (size_t)b * s->max_npad + x.n, samples[b], n_samples[b] * sizeof(float),
+                                            cudaMemcpyHostToDevice, st));
+        F[b] = act[b] ? (int)(np / 160) : 0;
+        // frame f reads samples [160 f - 200, 160 f + 200): final once 160 f + 200 <= n, whatever arrives later
+        Ffin[b] = !act[b] ? 0 : fin[b] ? F[b] : (int)std::min<int64_t>(F[b], n >= 200 ? (n - 200) / 160 + 1 : 0);
+        h[b] = (int64_t)b * s->max_npad; h[Bm + b] = act[b] ? n : 0; h[2 * Bm + b] = act[b] ? np : 0; h[3 * Bm + b] = (int64_t)b * s->maxF;
+        ffirst[b] = act[b] ? x.Ffin : 0;
+        fold[b] = make_int4(x.Ffin, Ffin[b], F[b], act[b]);
+        if (act[b]) { x.n = n; max_new_frames = std::max(max_new_frames, F[b] - x.Ffin); }
+    }
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_i64, h, 4 * Bm * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->str_int, s->h_str_int, 5 * Bm * sizeof(int), cudaMemcpyHostToDevice, st));
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[1], st));
+    launch_mel_stream(m, s->str_samples, s->d_i64, s->d_i64 + Bm, s->d_i64 + 2 * Bm, s->d_i64 + 3 * Bm, s->str_int + 4 * Bm, nst,
+                      max_new_frames, s->maxF, s->str_raw, reinterpret_cast<const int4*>(s->str_int), Wf, s->str_stats,
+                      s->str_stats_ld, st);
+    s->launches += max_new_frames > 0 ? 2 : 1;
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->h_str_stats, s->str_stats, (size_t)nst * s->str_stats_ld * sizeof(float), cudaMemcpyDeviceToHost, st));
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
+    // ---- the reuse rule: which windows are encoded again, and from which prompt position the decoder recomputes ----
+    struct Utt { int slot, w, f0, frames, tok0; float phi; };
+    std::vector<Utt> utts;
+    std::vector<int> P((size_t)nst, 0), T((size_t)nst, 0);
+    for (int b = 0; b < nst; ++b) {
+        if (!act[b]) continue;
+        Session::Stream& x = s->streams[b];
+        const float* row = s->h_str_stats + (size_t)b * s->str_stats_ld;
+        const float phi = fmaxf(row[0], row[1]) - 8.0f;       // = mel_finalize_kernel's floor of the offline mel of x[0..n)
+        const int C = (F[b] + cf - 1) / cf, W = cpw > 0 ? (C + cpw - 1) / cpw : 1;
+        int first_re = W, tok = 0, tok_re = -1;   // tok_re: first token of the first re-encoded window
+        for (int w = 0; w < W; ++w) {
+            const int f0 = w * Wf, f1 = std::min(F[b], (w + 1) * Wf);
+            int wt = 0;
+            for (int k = f0 / cf; k * cf < f1; ++k) wt += conv_out_len(conv_out_len(conv_out_len(std::min(cf, F[b] - k * cf))));
+            const bool finished = f1 <= Ffin[b];
+            const bool was_final = x.win_final[w];
+            const bool floor_ok = phi == x.win_phi[w] || row[2 + w] >= fmaxf(phi, x.win_phi[w]);
+            if (finished && was_final && floor_ok) s->str_counts[1] += 1;
+            else {
+                if (finished && was_final) s->str_counts[2] += 1;
+                utts.push_back({b, w, f0, f1 - f0, tok, phi});
+                x.win_phi[w] = phi; x.win_final[w] = finished;
+                first_re = std::min(first_re, w);
+            }
+            if (w == first_re && tok_re < 0) tok_re = tok;
+            tok += wt;
+        }
+        T[b] = tok;
+        x.phi = phi; x.Ffin = Ffin[b]; x.T = tok;
+        // P_b: head, context and the pads of the windows before the first re-encoded one (0 before the first prefill)
+        P[b] = std::min(9 + (int)x.ctx.size() + (tok_re < 0 ? tok : tok_re), x.kv_valid);
+    }
+    s->str_counts[0] = (int64_t)utts.size();
+    // ---- encoder: the re-encoded windows as pseudo-utterances of at most one window each, in waves of max_batch ----
+    int4* stage = reinterpret_cast<int4*>(s->h_str_int + 8 * Bm);
+    for (size_t u = 0; u < utts.size(); ++u) {
+        int phi_bits; memcpy(&phi_bits, &utts[u].phi, sizeof(phi_bits));
+        stage[u] = make_int4(utts[u].slot, utts[u].f0, utts[u].frames, phi_bits);
+    }
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->str_int + 8 * Bm, stage, utts.size() * sizeof(int4), cudaMemcpyHostToDevice, st));
+    for (size_t w0 = 0; w0 < utts.size(); w0 += Bm) {
+        const int nu = (int)std::min<size_t>(Bm, utts.size() - w0);
+        if (w0 > 0) ASRB_CUDA_CHECK(cudaStreamSynchronize(st));      // the pinned plans of the previous wave
+        s->B = nu;
+        s->F.assign(nu, 0); s->foff.assign(nu, 0);
+        int64_t fo = 0;
+        for (int u = 0; u < nu; ++u) {
+            s->F[u] = utts[w0 + u].frames; s->foff[u] = fo; fo += s->F[u];
+            h[3 * Bm + u] = s->foff[u]; h[4 * Bm + u] = s->F[u];
+        }
+        ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_i64, h, 5 * Bm * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+        launch_mel_stream_stage(m, s->str_raw, reinterpret_cast<const int4*>(s->str_int + 8 * Bm) + w0, s->d_i64 + 3 * Bm, nu,
+                                s->maxF, s->d_mel, st);
+        s->launches += 1;
+        s->stage = 1;
+        session_encode(s, nullptr);
+        for (int u = 0; u < nu; ++u) {
+            const Utt& q = utts[w0 + u];
+            ASRB_CUDA_CHECK(cudaMemcpyAsync(s->str_tok + ((size_t)q.slot * s->maxT + q.tok0) * od, s->audio + (size_t)s->toff[u] * od,
+                                            (size_t)s->T[u] * od * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        }
+    }
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[3], st));
+    // ---- prefill: stream b's rows from position P_b on, attending to the K/V its slot keeps below P_b ----
+    const int B = nst;
+    s->B = B; s->run_k = 1; s->run_alpha = -1.0; s->nslots = B;
+    s->S.assign(B, 0); s->srow0.assign(B, 0);
+    int totS = 0, maxlen = 0, maxrows = 0;
+    for (int b = 0; b < B; ++b) {
+        const Session::Stream& x = s->streams[b];
+        maxlen = std::max(maxlen, x.kv_valid + 1);     // an idle row's decode position (below)
+        if (!act[b]) continue;
+        s->srow0[b] = totS; s->S[b] = 9 + (int)x.ctx.size() + T[b] + 6 + nl[b] + (int)x.p.size();
+        totS += s->S[b] - P[b];
+        maxlen = std::max(maxlen, s->S[b]); maxrows = std::max(maxrows, s->S[b] - P[b]);
+    }
+    s->totS = totS; s->maxlenS = maxlen;
+    int* hi = s->h_int + s->enc_int_cap;
+    int* di = s->d_int + s->enc_int_cap;
+    int* ids = hi; int* arow = ids + totS; int* rseq = arow + totS; int* rpos = rseq + totS;
+    int* sq0 = rpos + totS; int* slen = sq0 + B; int* lastrow = slen + B; int* pos0 = lastrow + B; int* qpos0 = pos0 + B;
+    int* done0 = qpos0 + B;
+    const size_t nint = (size_t)(done0 + B - hi);
+    ASRB_REQUIRE(s->enc_int_cap + nint <= s->int_cap, ASRB_ERR_INVALID, "plan exceeds session capacity");
+    int64_t kept = 0;
+    for (int b = 0; b < B; ++b) {
+        const Session::Stream& x = s->streams[b];
+        // idle: no rows, done.  The batched decode step still writes a done row's K/V at its position: kv_valid, the
+        // first position the stream's next prefill recomputes
+        sq0[b] = 0; slen[b] = 0; lastrow[b] = 0; pos0[b] = x.kv_valid; qpos0[b] = 0; done0[b] = 1;
+        if (!act[b]) continue;
+        std::vector<int> pid, parow;
+        build_prompt(x.ctx, T[b], b * s->maxT, nl[b] > 0 ? lang_ids[b] : nullptr, nl[b], x.p, pid, parow);
+        plan_prompt_rows(pid, parow, P[b], s->srow0[b], b, ids, arow, rseq, rpos);
+        const int rows = s->S[b] - P[b];
+        sq0[b] = s->srow0[b]; slen[b] = rows; lastrow[b] = s->srow0[b] + rows - 1; pos0[b] = s->S[b] - 1; qpos0[b] = P[b]; done0[b] = 0;
+        kept += P[b];
+    }
+    s->str_counts[3] = totS; s->str_counts[4] = kept;
+    s->pf_rows = totS; s->pf_shared_rows = 0; s->pf_fan_bytes = 0;
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(di, hi, nint * sizeof(int), cudaMemcpyHostToDevice, st));
+    s->d_ids = di; s->d_audio_row = di + (arow - hi); s->d_row_seq = di + (rseq - hi);
+    s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_lastrow, di + (lastrow - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.pos, di + (pos0 - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    begin_run(s, B, di + (done0 - hi));
+    prefill_layers(s, totS, B, maxrows, nullptr, di + (qpos0 - hi), s->str_tok);
+    first_token(s, B, false, nullptr);
+    s->stage = 3;
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
+    // ---- decode: the offline batch's paths; idle streams are done from the start ----
+    std::vector<int32_t> g((size_t)B * max_new_tokens), glen((size_t)B);
+    session_generate(s, max_new_tokens, g.data(), glen.data());
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
+    ASRB_CUDA_CHECK(cudaEventSynchronize(s->ev[5]));
+    for (int i = 0; i < 5; ++i) ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[i], s->ev[i], s->ev[i + 1]));
+    ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[5], s->ev[0], s->ev[5]));
+    s->stream_run = true;
+    // ---- hypotheses and the next forced prefixes ----
+    for (int b = 0; b < B; ++b) {
+        if (!act[b]) continue;
+        Session::Stream& x = s->streams[b];
+        x.kv_valid = 9 + (int)x.ctx.size() + T[b];
+        std::vector<int> hyp = x.p;
+        hyp.insert(hyp.end(), g.begin() + (size_t)b * max_new_tokens, g.begin() + (size_t)b * max_new_tokens + glen[b]);
+        if (fin[b]) { x.p = hyp; x.closed = true; }
+        else if (x.k + 1 >= s->str_unfixed) x.p.assign(hyp.begin(), hyp.begin() + std::max(0, (int)hyp.size() - s->str_rollback));
+        else x.p.clear();
+        x.fixed = (int)x.p.size(); x.hyp = std::move(hyp); x.k += 1;
+    }
+    write_out();
+}
+
+// the stream's mel after its last push: bitwise asrb_mel of its samples ([n_mels][F])
+void session_stream_mel_read(Session* s, int b, float* out) {
+    ASRB_REQUIRE(s->streams_open && b >= 0 && b < (int)s->streams.size() && s->streams[b].n > 0, ASRB_ERR_STATE,
+                 "stream_mel_read: no pushed audio on this stream");
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    const Session::Stream& x = s->streams[b];
+    const int nm = s->m->d.c.num_mel_bins, F = (int)((x.n + 159) / 160);
+    ASRB_CUDA_CHECK(cudaMemcpy2D(out, F * sizeof(float), s->str_raw + (size_t)b * nm * s->maxF, s->maxF * sizeof(float),
+                                 F * sizeof(float), nm, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < (size_t)nm * F; ++i) out[i] = (std::max(out[i], x.phi) + 4.0f) / 4.0f;   // mel_finalize_kernel
+}
+
+void session_stream_encode_read(Session* s, int b, float* out) {
+    ASRB_REQUIRE(s->streams_open && b >= 0 && b < (int)s->streams.size() && s->streams[b].n > 0, ASRB_ERR_STATE,
+                 "stream_encode_read: no pushed audio on this stream");
+    ASRB_CUDA_CHECK(cudaSetDevice(s->m->ctx->device));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    const int od = s->m->d.c.output_dim;
+    ASRB_CUDA_CHECK(cudaMemcpy(out, s->str_tok + (size_t)b * s->maxT * od, (size_t)s->streams[b].T * od * sizeof(float),
+                               cudaMemcpyDeviceToHost));
+}
+
+// [0] windows encoded  [1] windows reused  [2] windows re-encoded because the floor moved  [3] prompt rows computed
+// [4] prompt rows kept from earlier pushes; over the streams of the last push
+void session_last_stream_stats(Session* s, int64_t* out, int n) {
+    for (int i = 0; i < n && i < 5; ++i) out[i] = s->str_counts[i];
 }
 
 void session_last_timings(Session* s, float* ms6, int64_t* kernels, int64_t* steps) {

@@ -765,6 +765,28 @@ class AsrInference:
             if top_logprobs:
                 self._record_top_logprobs(s, top_logprobs, False)
 
+    # ---- streaming (asrb_stream_*) ------------------------------------------------------------------------------------
+    def open_streams(self, n: int, max_seconds: float, language: Optional[str] = None, context: Optional[str] = None,
+                     rollback: int = 5, unfixed_pushes: int = 2, max_new_tokens: int = 32, language_ids=None,
+                     context_ids=None, logprobs: bool = False, top_logprobs: int = 0, temperature: float = 0.0,
+                     seed: int = 0, no_repeat_ngram_size: int = 0, repetition_penalty: float = 1.0):
+        """n live streams of up to `max_seconds` each (stream.StreamSet): push(samples_per_stream, final=...) returns
+        every stream's hypothesis of the audio received so far, decoded with the previous hypothesis less its last
+        `rollback` ids forced as a prefix (after `unfixed_pushes` pushes); `max_new_tokens` per push.  `language` /
+        `context` need tokenizer.json; `language_ids` / `context_ids` give the ids directly.  The session's
+        max_lang_ids is the language ids plus a forced prefix of stream.PREFIX_IDS_PER_SECOND ids per second of
+        `max_seconds` plus max_new_tokens (stream.stream_max_lang_ids); a push whose language ids and prefix outgrow it
+        is refused (ASRB_ERR_INVALID, the streams intact: finish the stream and open the next).  Any other
+        call on this engine ends the streams."""
+        from .stream import StreamSet
+        from .text import context_prompt_ids, language_prompt_ids
+        if self._options.get("beam_size", "1") != "1":
+            raise ValueError("beam search is not available on streams (the engine's beam_size option is set)")
+        lang = language_ids if language_ids is not None else language_prompt_ids(self.tokenizer, language)
+        ctx = context_ids if context_ids is not None else context_prompt_ids(self.tokenizer, context)
+        return StreamSet(self, int(n), float(max_seconds), lang, ctx, int(rollback), int(unfixed_pushes), int(max_new_tokens),
+                         logprobs, top_logprobs, temperature, seed, no_repeat_ngram_size, repetition_penalty)
+
     # ---- teacher-forced scoring (asrb_score_ids) --------------------------------------------------------------------
     def score_ids(self, clips: Sequence[np.ndarray], candidates: Sequence[Sequence[Sequence[int]]],
                   language_ids: Optional[Sequence] = None, context_ids: Optional[Sequence] = None,

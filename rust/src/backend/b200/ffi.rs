@@ -85,5 +85,13 @@ extern "C" {
     pub fn asrb_last_nbest(s: *mut asrb_session, max_new_tokens: c_int, k: c_int, ids_out: *mut i32, lens_out: *mut i32,
                            sum_logprob_out: *mut f32, score_out: *mut f32, eos_id_out: *mut i32) -> c_int;
     pub fn asrb_last_beam_stats(s: *mut asrb_session, out: *mut i64, n: c_int) -> c_int;
+    pub fn asrb_stream_open(s: *mut asrb_session, n_streams: c_int, rollback_ids: c_int, unfixed_pushes: c_int) -> c_int;
+    pub fn asrb_stream_reset(s: *mut asrb_session, stream: c_int) -> c_int;
+    pub fn asrb_stream_push(s: *mut asrb_session, n_streams: c_int, samples: *const *const f32, n_samples: *const i64,
+                            is_final: *const i32, lang_ids: *const *const i64, n_lang_ids: *const i32, max_new_tokens: c_int,
+                            max_ids: c_int, hyp_out: *mut i32, hyp_len_out: *mut i32, fixed_len_out: *mut i32) -> c_int;
+    pub fn asrb_stream_mel_read(s: *mut asrb_session, stream: c_int, out: *mut f32) -> c_int;
+    pub fn asrb_stream_encode_read(s: *mut asrb_session, stream: c_int, out: *mut f32) -> c_int;
+    pub fn asrb_last_stream_stats(s: *mut asrb_session, out: *mut i64, n: c_int) -> c_int;
     pub fn asrb_debug_mega_timeline(out: *mut c_longlong, cap: c_int) -> c_int;
 }

@@ -252,6 +252,23 @@ impl B200Engine {
         run
     }
 
+    /// One live stream on a session of its own (dropped with the returned handle): push 16 kHz mono f32 audio as it
+    /// arrives and get the hypothesis of everything received so far (`asrb_stream_push`, one stream).  `max_samples`
+    /// bounds the stream's length; the forced prefix may hold up to 8 ids per second of audio plus `max_new_tokens`.
+    pub fn open_stream(&self, max_samples: usize, lang_ids: Option<&[i64]>, rollback_ids: usize, unfixed_pushes: usize)
+                       -> Result<B200Stream<'_>> {
+        let m = self.max_new_tokens;
+        let lang = lang_ids.map(|v| v.to_vec());
+        let max_lang = lang.as_ref().map_or(0, |v| v.len()) + (max_samples * 8 + 15_999) / 16_000 + m;
+        let mut session = ptr::null_mut();
+        check(unsafe {
+            ffi::asrb_session_create_ex(self.model.0, 1, max_samples.max(201) as i64, max_lang as i32, 0, m as i32, &mut session)
+        })?;
+        let session = Session(session);
+        check(unsafe { ffi::asrb_stream_open(session.0, 1, rollback_ids as i32, unfixed_pushes as i32) })?;
+        Ok(B200Stream { session, lang, max_ids: max_lang + m, max_new_tokens: m, _engine: self })
+    }
+
     /// Long recordings: 16 kHz mono f32 `samples` of any length are cut on the GPU at the quietest 100 ms window of
     /// the last `search_samples` before every `max_segment_samples` (`asrb_segment_long`; both multiples of 160,
     /// `max_segment_samples` >= 80000, 32000 <= `search_samples` <= `max_segment_samples` / 2), and the segments are
@@ -298,4 +315,33 @@ impl B200Engine {
         }
         Ok(out)
     }
+}
+
+/// A live stream from `B200Engine::open_stream`; its session is freed on drop.
+pub struct B200Stream<'a> {
+    session: Session,
+    lang: Option<Vec<i64>>,
+    max_ids: usize,
+    max_new_tokens: usize,
+    _engine: &'a B200Engine,
+}
+
+impl B200Stream<'_> {
+    /// Appends `samples` (the last push sets `is_final`) and returns (hypothesis ids, fixed length): the first `fixed`
+    /// ids are forced into every later hypothesis of the stream.
+    pub fn push(&mut self, samples: &[f32], is_final: bool) -> Result<(Vec<i64>, usize)> {
+        let (ptrs, n, fin) = ([samples.as_ptr()], [samples.len() as i64], [is_final as i32]);
+        let lp = [self.lang.as_ref().map_or(ptr::null(), |v| v.as_ptr())];
+        let ll = [self.lang.as_ref().map_or(0, |v| v.len() as i32)];
+        let mut hyp = vec![0i32; self.max_ids];
+        let (mut len, mut fixed) = (0i32, 0i32);
+        check(unsafe {
+            ffi::asrb_stream_push(self.session.0, 1, ptrs.as_ptr(), n.as_ptr(), fin.as_ptr(), lp.as_ptr(), ll.as_ptr(),
+                                  self.max_new_tokens as i32, self.max_ids as i32, hyp.as_mut_ptr(), &mut len, &mut fixed)
+        })?;
+        Ok((hyp[..len as usize].iter().map(|&t| t as i64).collect(), fixed as usize))
+    }
+
+    /// Back to an empty stream (after a final push, or to start over).
+    pub fn reset(&mut self) -> Result<()> { check(unsafe { ffi::asrb_stream_reset(self.session.0, 0) }) }
 }
