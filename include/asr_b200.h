@@ -350,6 +350,56 @@ ASRB_API int asrb_score_ingested(asrb_session* s, const int64_t* const* lang_ids
                                  const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
                                  int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out);
 
+/* ---- word timestamps: alignment from the decoder's audio attention (DESIGN.md 4.10) ----
+ * Utterance b has its prompt of S_b ids exactly as asrb_transcribe_ids builds it (context and lang_ids included), its
+ * T_b audio tokens at positions a_b .. a_b + T_b - 1 with a_b = 9 + L_b (L_b = its context length), caller-given ids
+ * x_0 .. x_{n_b - 1} = ids[b][0 .. n_ids[b]) (normally the decoded ids followed by EOS 151645), and f_b = text_from[b]:
+ * the ids before f_b (for example "language English<asr_text>") are context and are not aligned.
+ *   Rows: row i, f_b <= i < n_b, is the query at position S_b - 1 + i, the row that predicts x_i in one causal forward
+ *     over prompt + ids; N_b = n_b - f_b rows.
+ *   Heads: heads[k] = {layer, query head}, n_heads pairs; n_heads = 0 means every query head of the layers
+ *     num_hidden_layers / 2 .. num_hidden_layers - 1.  Query head h reads kv head h / (nq / nkv).
+ *   Weights: per head and row, P[i][j] = softmax_j(q_i . k_j / sqrt(head_dim)) over the audio keys only, 0 <= j < T_b,
+ *     in fp32.
+ *   Normalise: per head and column j, z[i][j] = (P[i][j] - mean) / std over the N_b rows, std the population std;
+ *     z = 0 where std = 0.
+ *   Filter: per head and row, the median of width 7 along j with mirror padding (x[-1] = x[1]); none when T_b <= 3.
+ *   Head mean: M[i][j] = the sum over the heads in (layer, head) ascending order, divided by their count.
+ *   DTW on X = -M: C is (N + 1) x (T + 1) fp32, C[0][0] = 0 and the rest of row 0 and column 0 +inf;
+ *     C[i][j] = X[i-1][j-1] + c, where the step is diagonal (c = C[i-1][j-1]) when C[i-1][j-1] is less than both other
+ *     predecessors, else up (c = C[i-1][j]) when C[i-1][j] is less than both, else left (c = C[i][j-1]).  The path is
+ *     traced back from (N, T) to (0, 0); start_tok[i] = the least j on the path in row i.
+ *   Frames (10 ms each): audio token j, at in-chunk index t of encoder chunk k, starts at frame k * 2 * n_window + 8 t.
+ *     start_frame_out[b][i] = the frame of start_tok of row i, end_frame_out[b][i] = the next row's start frame, the
+ *     last row's = F_b, the utterance's mel frame count.  Both are [batch][max_ids] by id position; -1 outside
+ *     [f_b, n_b).
+ * Bitwise deterministic for a given call, and independent of the decode options (temperature, seed, beam_size,
+ * length_penalty and the repetition controls are not consulted).  The context of asrb_session_set_context applies,
+ * latched as in scoring.  An alignment call ends any pending run, as a scoring call does.  asrb_last_timings: [3] the
+ * decoder layers up to the last listed one with the probability and fold kernels, [4] the DTW, [5] the whole call.
+ * ASRB_ERR_INVALID before any work, the session as it was: batch outside [1, max_batch], n_ids[b] < 1 or greater than
+ * max_ids or the session's max_new_tokens, an id outside [0, vocab), text_from[b] outside [0, n_ids[b] - 1], a head
+ * outside the model or listed twice, plus everything asrb_transcribe_ids refuses (language ids, context rows). */
+ASRB_API int asrb_align_ids(asrb_session* s, const float* const* samples, const int64_t* n_samples, int batch,
+                            const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int64_t* const* ids,
+                            const int32_t* n_ids, const int32_t* text_from, const int32_t* heads, int n_heads, int max_ids,
+                            int32_t* start_frame_out, int32_t* end_frame_out);
+/* the same on the utterances of the last asrb_ingest_pcm */
+ASRB_API int asrb_align_ingested(asrb_session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids,
+                                 const int64_t* const* ids, const int32_t* n_ids, const int32_t* text_from,
+                                 const int32_t* heads, int n_heads, int max_ids, int32_t* start_frame_out,
+                                 int32_t* end_frame_out);
+/* the same on n views [start, end) of the long-audio files, read in place and checked as asrb_transcribe_segments
+ * reads and checks them; frames count from each view's start */
+ASRB_API int asrb_align_segments(asrb_session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
+                                 const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int64_t* const* ids,
+                                 const int32_t* n_ids, const int32_t* text_from, const int32_t* heads, int n_heads,
+                                 int max_ids, int32_t* start_frame_out, int32_t* end_frame_out);
+/* N_b (rows) and T_b (audio tokens) of utterance b of the last alignment call (either pointer may be NULL), and its
+ * M [N_b][T_b]; ASRB_ERR_STATE when that call had no utterance b */
+ASRB_API int asrb_last_align_dims(asrb_session* s, int b, int32_t* n_rows_out, int32_t* n_tokens_out);
+ASRB_API int asrb_align_matrix_read(asrb_session* s, int b, float* out);
+
 /* ---- streaming transcription (DESIGN.md 4.9) ----
  * A streaming run uses an ordinary session (asrb_session_create_ex).  Stream b lives in KV slot b,
  * 0 <= b < n_streams <= max_batch.  It owns its 16 kHz f32 samples x[0..n), its forced prefix p (ids, empty at the

@@ -13,12 +13,15 @@ recognition towards its words (names, jargon, a keyword list).
 `--max-segment S` (seconds, anywhere on the line) cuts the recording at quiet points into segments of at most S seconds,
 decodes them as batches and prints a `Segments:` block of `[start - end] text` lines.
 `--stream S` (seconds, anywhere on the line) replays the file as a live stream in pushes of S seconds and prints each
-push's fixed and unfixed text (`[t] fixed | unfixed`), then the final transcript."""
+push's fixed and unfixed text (`[t] fixed | unfixed`), then the final transcript.
+`--word-timestamps` (anywhere on the line) also prints a `Words:` block of `[start - end] word` lines, from the
+decoder's attention over the audio (with `--max-segment` too); not with `--stream`, `--score` or `--detect-language`."""
 import sys
 
 USAGE = ("Usage: python -m qwen3_asr_rs_b200 <model_dir> <audio_file> [language] [--logprobs] [--top-logprobs N] "
          "[--temperature T[,T...]] [--seed N] [--beam-size N] [--length-penalty A] [--context TEXT | --context-file PATH] "
-         "[--no-repeat-ngram N] [--repetition-penalty P] [--max-segment S | --stream S] [--score TEXT | --detect-language]")
+         "[--no-repeat-ngram N] [--repetition-penalty P] [--max-segment S | --stream S] [--score TEXT | --detect-language] "
+         "[--word-timestamps]")
 
 
 def parse_args(argv):
@@ -217,6 +220,12 @@ def stream_pushes(n_samples: int, push_s: float):
     return out
 
 
+def split_word_timestamps(argv):
+    """Remove `--word-timestamps` from argv -> (remaining argv, whether it was there)."""
+    rest = [a for a in argv if a != "--word-timestamps"]
+    return rest, len(rest) != len(argv)
+
+
 def format_segment(start_s: float, end_s: float, text: str) -> str:
     """One line of the `Segments:` block."""
     return f"  [{start_s:.2f} - {end_s:.2f}] {text}"
@@ -229,6 +238,7 @@ def format_candidates(cands, decode) -> str:
 
 def main(argv=None) -> int:
     argv = list(sys.argv[1:] if argv is None else argv)
+    argv, words = split_word_timestamps(argv)
     seg = split_max_segment(argv)
     if seg is None:
         print(USAGE, file=sys.stderr)
@@ -261,6 +271,10 @@ def main(argv=None) -> int:
                                  or isinstance(temperature, tuple)):
         print("--stream cannot be combined with --score, --detect-language, --logprobs, --top-logprobs, --beam-size or "
               "a temperature schedule", file=sys.stderr)
+        print(USAGE, file=sys.stderr)
+        return 1
+    if words and (stream_s is not None or score_text is not None or detect):
+        print("--word-timestamps cannot be combined with --stream, --score or --detect-language", file=sys.stderr)
         print(USAGE, file=sys.stderr)
         return 1
     if beam_size > 1 and (top or (temperature is not None and not isinstance(temperature, tuple) and temperature > 0)):
@@ -302,6 +316,8 @@ def main(argv=None) -> int:
             kw.update(max_segment_s=max_segment)
         if rep[1] or rep[2] != 1.0:
             kw.update(no_repeat_ngram_size=rep[1], repetition_penalty=rep[2])
+        if words:
+            kw.update(word_timestamps=True)
         r = eng.transcribe(audio, language, logprobs=logprobs, top_logprobs=top, **kw)
         decode = eng.tokenizer.decode if eng.tokenizer is not None else (lambda ids: " ".join(str(i) for i in ids))
     finally:
@@ -326,6 +342,10 @@ def main(argv=None) -> int:
         print("Segments:")
         for start_s, end_s, text in r.segments:
             print(format_segment(start_s, end_s, text))
+    if r.words is not None:
+        print("Words:")
+        for w in r.words:
+            print(format_segment(w.start_s, w.end_s, w.text.strip()))
     return 0
 
 

@@ -20,6 +20,7 @@ SYMBOLS = [
     "asrb_session_create_ex", "asrb_session_set_context", "asrb_last_prefill_stats",
     "asrb_ingest_long", "asrb_long_read", "asrb_segment_long", "asrb_transcribe_segments",
     "asrb_score_ids", "asrb_score_ingested",
+    "asrb_align_ids", "asrb_align_ingested", "asrb_align_segments", "asrb_last_align_dims", "asrb_align_matrix_read",
     "asrb_stream_open", "asrb_stream_reset", "asrb_stream_push", "asrb_stream_mel_read", "asrb_stream_encode_read",
     "asrb_last_stream_stats",
 ]
@@ -99,6 +100,13 @@ def load_library() -> C.CDLL:
         "asrb_score_ids": [vp, P(P(C.c_float)), P(i64), C.c_int, P(P(i64)), P(i32), P(i32), P(P(i64)), P(i32), C.c_int,
                            P(C.c_float), P(i32), P(C.c_float)],
         "asrb_score_ingested": [vp, P(P(i64)), P(i32), P(i32), P(P(i64)), P(i32), C.c_int, P(C.c_float), P(i32), P(C.c_float)],
+        "asrb_align_ids": [vp, P(P(C.c_float)), P(i64), C.c_int, P(P(i64)), P(i32), P(P(i64)), P(i32), P(i32), P(i32),
+                           C.c_int, C.c_int, P(i32), P(i32)],
+        "asrb_align_ingested": [vp, P(P(i64)), P(i32), P(P(i64)), P(i32), P(i32), P(i32), C.c_int, C.c_int, P(i32), P(i32)],
+        "asrb_align_segments": [vp, C.c_int, P(i32), P(i64), P(i64), P(P(i64)), P(i32), P(P(i64)), P(i32), P(i32), P(i32),
+                                C.c_int, C.c_int, P(i32), P(i32)],
+        "asrb_last_align_dims": [vp, C.c_int, P(i32), P(i32)],
+        "asrb_align_matrix_read": [vp, C.c_int, P(C.c_float)],
         "asrb_stream_open": [vp, C.c_int, C.c_int, C.c_int],
         "asrb_stream_reset": [vp, C.c_int],
         "asrb_stream_push": [vp, C.c_int, P(P(C.c_float)), P(i64), P(i32), P(P(i64)), P(i32), C.c_int, C.c_int, P(i32), P(i32),

@@ -48,6 +48,15 @@ void session_last_prefill_stats(Session* s, int64_t* out, int n);
 void session_score_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* const* lang_ids,
                        const int32_t* n_lang_ids, const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
                        int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out);
+void session_align_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* const* lang_ids,
+                       const int32_t* n_lang_ids, const int64_t* const* ids, const int32_t* n_ids, const int32_t* text_from,
+                       const int32_t* heads, int n_heads, int max_ids, int32_t* start_out, int32_t* end_out);
+void session_align_segments(Session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
+                            const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int64_t* const* ids,
+                            const int32_t* n_ids, const int32_t* text_from, const int32_t* heads, int n_heads, int max_ids,
+                            int32_t* start_out, int32_t* end_out);
+void session_last_align_dims(Session* s, int b, int32_t* n_rows, int32_t* n_tokens);
+void session_align_matrix_read(Session* s, int b, float* out);
 void session_stream_open(Session* s, int n_streams, int rollback, int unfixed);
 void session_stream_reset(Session* s, int b);
 void session_stream_push(Session* s, int nst, const float* const* samples, const int64_t* n_samples, const int32_t* is_final,
@@ -283,6 +292,36 @@ int asrb_score_ingested(asrb_session* s, const int64_t* const* lang_ids, const i
     return guarded([&] { NONNULL(s);
                          session_score_ids(s->s, nullptr, nullptr, 0, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len,
                                            max_new_tokens, logprob_out, top_ids_out, top_lp_out); });
+}
+
+int asrb_align_ids(asrb_session* s, const float* const* samples, const int64_t* n_samples, int batch,
+                   const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int64_t* const* ids, const int32_t* n_ids,
+                   const int32_t* text_from, const int32_t* heads, int n_heads, int max_ids, int32_t* start_frame_out,
+                   int32_t* end_frame_out) {
+    return guarded([&] { NONNULL(s); NONNULL(samples); NONNULL(n_samples);
+                         session_align_ids(s->s, samples, n_samples, batch, lang_ids, n_lang_ids, ids, n_ids, text_from, heads,
+                                           n_heads, max_ids, start_frame_out, end_frame_out); });
+}
+int asrb_align_ingested(asrb_session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int64_t* const* ids,
+                        const int32_t* n_ids, const int32_t* text_from, const int32_t* heads, int n_heads, int max_ids,
+                        int32_t* start_frame_out, int32_t* end_frame_out) {
+    return guarded([&] { NONNULL(s);
+                         session_align_ids(s->s, nullptr, nullptr, 0, lang_ids, n_lang_ids, ids, n_ids, text_from, heads,
+                                           n_heads, max_ids, start_frame_out, end_frame_out); });
+}
+int asrb_align_segments(asrb_session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
+                        const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int64_t* const* ids,
+                        const int32_t* n_ids, const int32_t* text_from, const int32_t* heads, int n_heads, int max_ids,
+                        int32_t* start_frame_out, int32_t* end_frame_out) {
+    return guarded([&] { NONNULL(s); NONNULL(file); NONNULL(start); NONNULL(end);
+                         session_align_segments(s->s, n, file, start, end, lang_ids, n_lang_ids, ids, n_ids, text_from, heads,
+                                                n_heads, max_ids, start_frame_out, end_frame_out); });
+}
+int asrb_last_align_dims(asrb_session* s, int b, int32_t* n_rows_out, int32_t* n_tokens_out) {
+    return guarded([&] { NONNULL(s); session_last_align_dims(s->s, b, n_rows_out, n_tokens_out); });
+}
+int asrb_align_matrix_read(asrb_session* s, int b, float* out) {
+    return guarded([&] { NONNULL(s); NONNULL(out); session_align_matrix_read(s->s, b, out); });
 }
 
 int asrb_stream_open(asrb_session* s, int n_streams, int rollback_ids, int unfixed_pushes) {

@@ -278,6 +278,33 @@ void launch_score_head(const Model& m, const float* hid, const int* d_src, const
                        bf16* planes, size_t plane_stride, int nplanes, ScorePart* part, bool topk, float* lp_out,
                        int* tk_ids, float* tk_lp, cudaStream_t st, int64_t* launches);
 
+// align.cu -- word-timing alignment (asrb_align_ids, DESIGN.md 4.10); per-utterance device arrays indexed by b
+struct AlignProbArgs {
+    const float* q; int ldq;                   // post-RoPE q rows (s->qrot)
+    const float* k; size_t seg_stride, head_stride; int hd, group;   // the layer's K cache
+    const int *qrow0, *N, *T, *a0, *slot;      // first aligned row, rows, audio keys, first audio position, KV slot
+    const long long* moff;                     // offset of utterance b's [N][T] block in a plane
+    const int* heads; int nheads;              // query heads of the layer (device), in list order
+    float* P; size_t plane;                    // [nheads][plane] probabilities
+};
+struct AlignFoldArgs {
+    const int *N, *T; const long long* moff;
+    float* P; size_t plane; int nheads;        // z-scores in place
+    float* M;                                  // [sum N T] running head sum (the last listed layer: the mean)
+    int count;                                 // > 0 on the last listed layer: divide by it
+};
+struct AlignDtwArgs {
+    const int *N, *T; const long long* moff;
+    const float* M;
+    const int* smem_trace;                     // 1: trace in shared memory, else at trace + toff[b]
+    uint32_t* trace; const long long* toff;
+    int* start; const int* soff;               // start[soff[b] + i]: least column of the path in row i
+};
+void launch_align_probs(const AlignProbArgs& a, int B, int maxN, cudaStream_t st);
+void launch_align_fold(const AlignFoldArgs& a, int B, int maxT, int maxNT, cudaStream_t st);
+size_t align_dtw_smem(int N, int T, bool trace_in_smem);
+void launch_align_dtw(const AlignDtwArgs& a, int B, size_t smem, cudaStream_t st);
+
 // beam.cu -- beam search over the TOPK records (session option "beam_size"); the spec is in include/asr_b200.h
 constexpr int BEAM_MAX = 6;
 struct BeamUtt {                   // device state of one utterance's search

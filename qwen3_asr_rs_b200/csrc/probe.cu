@@ -219,4 +219,31 @@ int asrbt_attention(const asrbt_attn_args* a) {
     });
 }
 
+int asrbt_dtw(const float* M, int N, int T, int32_t* start_tok_out) {
+    return run_guarded([&] {
+        ASRB_REQUIRE(M && start_tok_out && N >= 1 && T >= 1, ASRB_ERR_INVALID, "asrbt_dtw: bad arguments");
+        int dev = 0;
+        ASRB_CUDA_CHECK(cudaGetDevice(&dev));
+        int optin = 0;
+        ASRB_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        const bool in_smem = align_dtw_smem(N, T, true) <= (size_t)optin;
+        const size_t smem = align_dtw_smem(N, T, in_smem);
+        ASRB_REQUIRE(smem <= (size_t)optin, ASRB_ERR_INVALID, "asrbt_dtw: N too large for the DTW kernel");
+        Scope s;
+        const int h_int[4] = {N, T, in_smem ? 1 : 0, 0};
+        const long long h_ll[2] = {0, 0};
+        const int* d_int = s.upload(h_int, 4);
+        const long long* d_ll = s.upload(h_ll, 2);
+        AlignDtwArgs a{};
+        a.N = d_int; a.T = d_int + 1; a.smem_trace = d_int + 2; a.soff = d_int + 3; a.moff = d_ll; a.toff = d_ll + 1;
+        a.M = s.upload(M, (size_t)N * T);
+        a.trace = s.alloc<uint32_t>(in_smem ? 1 : ((size_t)N * T + 15) / 16);
+        int* d_start = s.alloc<int>((size_t)N, 0xff);
+        a.start = d_start;
+        launch_align_dtw(a, 1, smem, s.st);
+        s.download(start_tok_out, d_start, (size_t)N);
+        s.sync();
+    });
+}
+
 }  // extern "C"

@@ -59,6 +59,9 @@ ASRB_API int asrbt_gemm_plan(int M, int N, int K, int a_mode, int epi, int sms, 
                              int* plan_out);
 ASRB_API int asrbt_gemm(const asrbt_gemm_args* a, int* plan_out);
 ASRB_API int asrbt_attention(const asrbt_attn_args* a);
+/* the alignment DTW kernel (DESIGN.md 4.10) on one caller matrix M [N][T]: start_tok_out[N] = the least column of the
+ * path in each row.  The trace goes to shared memory when it fits, else to global memory, as in asrb_align_ids. */
+ASRB_API int asrbt_dtw(const float* M, int N, int T, int32_t* start_tok_out);
 
 #ifdef __cplusplus
 }

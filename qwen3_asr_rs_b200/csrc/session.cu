@@ -120,6 +120,13 @@ struct Session {
         float* lp = nullptr; int* tk_ids = nullptr; float* tk_lp = nullptr;
         int* h_int = nullptr; int* d_int = nullptr; size_t int_cap = 0;   // row plan | per-slot arrays | score rows
     } sc;
+    // word-timing alignment (asrb_align_ids, DESIGN.md 4.10): scratch allocated, and grown, all or none by the alignment
+    // calls; the last call's M and dims stay readable (asrb_align_matrix_read / asrb_last_align_dims) until the next one
+    struct AlignBufs {
+        size_t p_cap = 0, m_cap = 0, trace_cap = 0, start_cap = 0;   // floats / floats / words / ints
+        float *P = nullptr, *M = nullptr; uint32_t* trace = nullptr; int* start = nullptr;
+        std::vector<int> N, T; std::vector<long long> moff;   // of the last alignment call (empty: none)
+    } al;
     // streaming (asrb_stream_*, DESIGN.md 4.9): stream b lives in KV slot b; its buffers are allocated by the first open
     struct Stream {
         int64_t n = 0;                  // samples received, in str_samples row b
@@ -689,16 +696,25 @@ static int plan_prompt_rows(const std::vector<int>& pid, const std::vector<int>&
     return r;
 }
 
+// an alignment call's work inside the prefill: run(l) after layer l's q / k normalisation and RoPE, while s->qrot
+// holds that layer's q and the K cache that layer's keys
+struct LayerHook {
+    virtual void run(int layer) = 0;
+    virtual ~LayerHook() = default;
+};
+
 // embed + inject and the decoder layers over the planned rows (s->d_ids ..., totS rows; sequence q's rows are its
-// segment of the attention, in KV slot q); audio rows are read from `audio`
+// segment of the attention, in KV slot q); audio rows are read from `audio`.  n_layers < 0: every layer; else the
+// layers 0 .. n_layers - 1, the last of them stopping after `hook` (an alignment call, which needs no later work)
 static void prefill_layers(Session* s, int totS, int nseq, int maxrows, const FanOut* fan, const int* d_qpos0,
-                           const float* audio) {
+                           const float* audio, int n_layers = -1, LayerHook* hook = nullptr) {
     Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
     cudaStream_t st = s->st; const int np = s->nplanes;
     launch_embed_inject(m.embed, c.hidden_size, s->d_ids, s->d_audio_row, audio, totS, s->hid, st);
     s->launches += 1;
     const int H = c.hidden_size; const float eps = (float)c.rms_norm_eps;
-    for (int l = 0; l < c.num_hidden_layers; ++l) {
+    const int L = n_layers < 0 ? c.num_hidden_layers : n_layers;
+    for (int l = 0; l < L; ++l) {
         const DecLayerW& w = m.dec[l];
         float* kc = s->kcache + (size_t)l * s->cache_layer_stride;
         float* vc = s->vcache + (size_t)l * s->cache_layer_stride;
@@ -709,6 +725,10 @@ static void prefill_layers(Session* s, int totS, int nseq, int maxrows, const Fa
         launch_qk_norm_rope(s->dqkv, totS, s->d_row_seq, s->d_row_pos, w.qnorm, w.knorm, eps, m.rope_cos, m.rope_sin,
                             c.num_attention_heads, c.num_key_value_heads, c.head_dim, s->qrot, kc, vc, s->cache_seq_stride,
                             s->max_ctx, st, fan);
+        if (hook) {
+            hook->run(l);
+            if (l == L - 1) { s->launches += 3; break; }
+        }
         { AttnParams p{}; p.q = s->qrot; p.ldq = d.q_dim; p.k = kc; p.v = vc; p.seg_stride = s->cache_seq_stride;
           p.head_stride = (size_t)s->max_ctx * c.head_dim; p.ldk = c.head_dim; p.keys_in_rows = 0;
           p.seg_q0 = s->d_seq_q0; p.seg_len = s->d_seq_len; p.nseg = nseq; p.nheads = c.num_attention_heads;
@@ -1056,23 +1076,30 @@ void session_transcribe_ids(Session* s, const float* const* samples, const int64
     transcribe_impl(s, samples, n_samples, batch, nullptr, lang_ids, n_lang_ids, max_new_tokens, ids_out, lens_out);
 }
 
-// asrb_transcribe_segments: n views [start, end) of the long-audio files as one batch, every argument checked first
+// n views [start, end) of the long-audio files as one batch (asrb_transcribe_segments, asrb_align_segments): their
+// offsets in the long-audio buffer and lengths, every argument checked first
+static void segment_views(const Session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
+                          std::vector<int64_t>& off, std::vector<int64_t>& len, const char* who) {
+    const std::string w(who);
+    ASRB_REQUIRE(!s->long_n.empty(), ASRB_ERR_STATE, w + ": nothing ingested with asrb_ingest_long");
+    ASRB_REQUIRE(n >= 1 && n <= s->max_batch, ASRB_ERR_INVALID, w + ": n must be in [1, max_batch]");
+    off.assign((size_t)n, 0); len.assign((size_t)n, 0);
+    for (int i = 0; i < n; ++i) {
+        const int f = file[i];
+        ASRB_REQUIRE(f >= 0 && f < (int)s->long_n.size(), ASRB_ERR_INVALID, w + ": file index out of range");
+        ASRB_REQUIRE(start[i] >= 0 && start[i] < end[i] && end[i] <= s->long_n[f], ASRB_ERR_INVALID,
+                     w + ": need 0 <= start < end <= the file's samples");
+        len[i] = end[i] - start[i];
+        ASRB_REQUIRE(len[i] >= 201 && len[i] <= s->max_samples, ASRB_ERR_INVALID, w + ": a view must hold 201 .. max_samples samples");
+        off[i] = s->long_off[f] + start[i];
+    }
+}
+
 void session_transcribe_segments(Session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
                                  const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
                                  int32_t* ids_out, int32_t* lens_out) {
-    ASRB_REQUIRE(!s->long_n.empty(), ASRB_ERR_STATE, "transcribe_segments: nothing ingested with asrb_ingest_long");
-    ASRB_REQUIRE(n >= 1 && n <= s->max_batch, ASRB_ERR_INVALID, "transcribe_segments: n must be in [1, max_batch]");
-    std::vector<int64_t> off((size_t)n), len((size_t)n);
-    for (int i = 0; i < n; ++i) {
-        const int f = file[i];
-        ASRB_REQUIRE(f >= 0 && f < (int)s->long_n.size(), ASRB_ERR_INVALID, "transcribe_segments: file index out of range");
-        ASRB_REQUIRE(start[i] >= 0 && start[i] < end[i] && end[i] <= s->long_n[f], ASRB_ERR_INVALID,
-                     "transcribe_segments: need 0 <= start < end <= the file's samples");
-        len[i] = end[i] - start[i];
-        ASRB_REQUIRE(len[i] >= 201 && len[i] <= s->max_samples, ASRB_ERR_INVALID,
-                     "transcribe_segments: a view must hold 201 .. max_samples samples");
-        off[i] = s->long_off[f] + start[i];
-    }
+    std::vector<int64_t> off, len;
+    segment_views(s, n, file, start, end, off, len, "transcribe_segments");
     transcribe_impl(s, nullptr, len.data(), n, off.data(), lang_ids, n_lang_ids, max_new_tokens, ids_out, lens_out);
 }
 
@@ -1145,6 +1172,87 @@ static void ensure_score_bufs(Session* s, size_t rows, int score_rows, size_t pl
     }
 }
 
+// the plan of a teacher-forced prefill (asrb_score_ids, asrb_align_ids): slot q = candidate q; the first candidate of an
+// utterance leads (its prompt and its ids but the last), the others (followers) compute their ids but the last from
+// position S_b on, their prompt K/V fanned out.  Grows the buffers (the score head's only with `head`), uploads the
+// plan and points the session's row arrays at it
+struct TfPlan {
+    int N = 0, totS = 0, maxrows = 0, R = 0;          // slots, prefill rows, most rows of one slot, ids in all
+    std::vector<int> srow0, coff;                     // first row of slot q; first id of candidate q in the id order
+    const int *d_src = nullptr, *d_tgt = nullptr;     // [R]: the row predicting each id, and the id
+    bool fan = false; FanOut fan_plan{}; const int* d_qpos0 = nullptr;
+};
+static TfPlan plan_teacher_forced(Session* s, int B, const int64_t* const* lang_ids, const int32_t* n_lang_ids,
+                                  const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len, int N,
+                                  bool head) {
+    const asrb_dims& c = s->m->d.c;
+    cudaStream_t st = s->st;
+    TfPlan tf;
+    s->S.assign(B, 0);
+    std::vector<int> utt(N), lead(N), rows(N);
+    std::vector<int>& srow0 = tf.srow0; std::vector<int>& coff = tf.coff;
+    srow0.assign(N, 0); coff.assign(N + 1, 0);
+    int totS = 0, maxrows = 0, R = 0;
+    int64_t shared = 0;
+    for (int b = 0, q = 0; b < B; ++b) {
+        const int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
+        s->S[b] = 9 + (int)context_of(s, b).size() + s->T[b] + 6 + nl;
+        for (int j = 0; j < n_cand[b]; ++j, ++q) {
+            utt[q] = b; lead[q] = q - j;
+            rows[q] = (j == 0 ? s->S[b] : 0) + cand_len[q] - 1;
+            srow0[q] = totS; totS += rows[q]; maxrows = std::max(maxrows, rows[q]);
+            coff[q] = R; R += cand_len[q];
+        }
+        shared += (int64_t)(n_cand[b] - 1) * s->S[b];
+    }
+    coff[N] = R;
+    Session::ScoreBufs& sb = s->sc;
+    ensure_score_bufs(s, (size_t)totS, head ? R : 0, 4 * (size_t)totS + 8 * (size_t)N + 2 * (size_t)R + 16);
+    int* hi = sb.h_int;
+    int* ids = hi; int* arow = ids + totS; int* rseq = arow + totS; int* rpos = rseq + totS;
+    int* sq0 = rpos + totS; int* slen = sq0 + N; int* qpos0 = slen + N;
+    int* fan_n = qpos0 + N; int* fan_off = fan_n + N; int* fan_P = fan_off + N; int* fan_slots = fan_P + N;
+    int* src = fan_slots + std::max(N, 1); int* tgt = src + R;
+    const size_t nint = (size_t)(tgt + R - hi);
+    ASRB_REQUIRE(nint <= sb.int_cap && (!head || R <= sb.rows_cap), ASRB_ERR_INVALID, "score: plan exceeds session capacity");
+    std::vector<int> pid, parow;
+    int nf = 0;
+    for (int q = 0; q < N; ++q) {
+        const int b = utt[q], Sb = s->S[b];
+        const bool leader = lead[q] == q;
+        int r = srow0[q];
+        if (leader) {
+            build_prompt(s, b, lang_ids, pid, parow);
+            r = plan_prompt_rows(pid, parow, 0, r, q, ids, arow, rseq, rpos);
+        }
+        for (int i = 0; i + 1 < cand_len[q]; ++i, ++r) { ids[r] = (int)cand_ids[q][i]; arow[r] = -1; rseq[r] = q; rpos[r] = Sb + i; }
+        sq0[q] = srow0[q]; slen[q] = rows[q]; qpos0[q] = leader ? 0 : Sb;
+        fan_off[q] = nf; fan_n[q] = 0; fan_P[q] = 0;
+        if (leader) {
+            fan_P[q] = Sb;
+            for (int f = q + 1; f < N && lead[f] == q; ++f) { fan_slots[nf++] = f; ++fan_n[q]; }
+        }
+        // row map: id 0 from the leader's last prompt row, id i from this candidate's row at position S_b + i - 1
+        const int own0 = leader ? srow0[q] + Sb : srow0[q];
+        for (int i = 0; i < cand_len[q]; ++i) {
+            src[coff[q] + i] = i == 0 ? srow0[lead[q]] + Sb - 1 : own0 + i - 1;
+            tgt[coff[q] + i] = (int)cand_ids[q][i];
+        }
+    }
+    s->pf_rows = totS; s->pf_shared_rows = shared;
+    s->pf_fan_bytes = shared * 2LL * c.num_hidden_layers * c.num_key_value_heads * c.head_dim * (int64_t)sizeof(float);
+    int* di = sb.d_int;
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(di, hi, nint * sizeof(int), cudaMemcpyHostToDevice, st));
+    s->d_ids = di; s->d_audio_row = di + (arow - hi); s->d_row_seq = di + (rseq - hi);
+    s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
+    tf.fan_plan = FanOut{di + (fan_n - hi), di + (fan_off - hi), di + (fan_P - hi), di + (fan_slots - hi)};
+    tf.fan = nf > 0;
+    tf.d_qpos0 = tf.fan ? di + (qpos0 - hi) : nullptr;
+    tf.d_src = di + (src - hi); tf.d_tgt = di + (tgt - hi);
+    tf.N = N; tf.totS = totS; tf.maxrows = maxrows; tf.R = R;
+    return tf;
+}
+
 static void score_impl(Session* s, const float* const* samples, const int64_t* n_samples, int batch,
                        const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int32_t* n_cand,
                        const int64_t* const* cand_ids, const int32_t* cand_len, int max_new_tokens, float* logprob_out,
@@ -1192,69 +1300,12 @@ static void score_impl(Session* s, const float* const* samples, const int64_t* n
     session_encode(s, nullptr);
     ASRB_CUDA_CHECK(cudaEventRecord(s->ev[3], st));
     s->stage = 2;                                     // the KV slots are overwritten: no run to continue after this call
-    // ---- plan: slot q = candidate q; the first candidate of an utterance leads (its prompt and its ids but the last),
-    // the others (followers) compute their ids but the last from position S_b on, their prompt K/V fanned out ----
-    const int B = batch;
-    s->S.assign(B, 0);
-    std::vector<int> utt(N), lead(N), srow0(N), rows(N), coff(N + 1, 0);
-    int totS = 0, maxrows = 0, R = 0;
-    int64_t shared = 0;
-    for (int b = 0, q = 0; b < B; ++b) {
-        const int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
-        s->S[b] = 9 + (int)context_of(s, b).size() + s->T[b] + 6 + nl;
-        for (int j = 0; j < n_cand[b]; ++j, ++q) {
-            utt[q] = b; lead[q] = q - j;
-            rows[q] = (j == 0 ? s->S[b] : 0) + cand_len[q] - 1;
-            srow0[q] = totS; totS += rows[q]; maxrows = std::max(maxrows, rows[q]);
-            coff[q] = R; R += cand_len[q];
-        }
-        shared += (int64_t)(n_cand[b] - 1) * s->S[b];
-    }
-    coff[N] = R;
+    const TfPlan tf = plan_teacher_forced(s, batch, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len, N, true);
+    const int R = tf.R; const std::vector<int>& coff = tf.coff;
     Session::ScoreBufs& sb = s->sc;
-    ensure_score_bufs(s, (size_t)totS, R, 4 * (size_t)totS + 8 * (size_t)N + 2 * (size_t)R + 16);
-    int* hi = sb.h_int;
-    int* ids = hi; int* arow = ids + totS; int* rseq = arow + totS; int* rpos = rseq + totS;
-    int* sq0 = rpos + totS; int* slen = sq0 + N; int* qpos0 = slen + N;
-    int* fan_n = qpos0 + N; int* fan_off = fan_n + N; int* fan_P = fan_off + N; int* fan_slots = fan_P + N;
-    int* src = fan_slots + std::max(N, 1); int* tgt = src + R;
-    const size_t nint = (size_t)(tgt + R - hi);
-    ASRB_REQUIRE(nint <= sb.int_cap && R <= sb.rows_cap, ASRB_ERR_INVALID, "score: plan exceeds session capacity");
-    std::vector<int> pid, parow;
-    int nf = 0;
-    for (int q = 0; q < N; ++q) {
-        const int b = utt[q], Sb = s->S[b];
-        const bool leader = lead[q] == q;
-        int r = srow0[q];
-        if (leader) {
-            build_prompt(s, b, lang_ids, pid, parow);
-            r = plan_prompt_rows(pid, parow, 0, r, q, ids, arow, rseq, rpos);
-        }
-        for (int i = 0; i + 1 < cand_len[q]; ++i, ++r) { ids[r] = (int)cand_ids[q][i]; arow[r] = -1; rseq[r] = q; rpos[r] = Sb + i; }
-        sq0[q] = srow0[q]; slen[q] = rows[q]; qpos0[q] = leader ? 0 : Sb;
-        fan_off[q] = nf; fan_n[q] = 0; fan_P[q] = 0;
-        if (leader) {
-            fan_P[q] = Sb;
-            for (int f = q + 1; f < N && lead[f] == q; ++f) { fan_slots[nf++] = f; ++fan_n[q]; }
-        }
-        // row map: id 0 from the leader's last prompt row, id i from this candidate's row at position S_b + i - 1
-        const int own0 = leader ? srow0[q] + Sb : srow0[q];
-        for (int i = 0; i < cand_len[q]; ++i) {
-            src[coff[q] + i] = i == 0 ? srow0[lead[q]] + Sb - 1 : own0 + i - 1;
-            tgt[coff[q] + i] = (int)cand_ids[q][i];
-        }
-    }
-    s->pf_rows = totS; s->pf_shared_rows = shared;
-    s->pf_fan_bytes = shared * 2LL * c.num_hidden_layers * c.num_key_value_heads * c.head_dim * (int64_t)sizeof(float);
-    int* di = sb.d_int;
-    ASRB_CUDA_CHECK(cudaMemcpyAsync(di, hi, nint * sizeof(int), cudaMemcpyHostToDevice, st));
-    s->d_ids = di; s->d_audio_row = di + (arow - hi); s->d_row_seq = di + (rseq - hi);
-    s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
-    const FanOut fan_plan{di + (fan_n - hi), di + (fan_off - hi), di + (fan_P - hi), di + (fan_slots - hi)};
-    const bool fan = nf > 0;
-    prefill_layers(s, totS, N, maxrows, fan ? &fan_plan : nullptr, fan ? di + (qpos0 - hi) : nullptr, s->audio);
+    prefill_layers(s, tf.totS, N, tf.maxrows, tf.fan ? &tf.fan_plan : nullptr, tf.d_qpos0, s->audio);
     ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
-    launch_score_head(m, s->hid, di + (src - hi), di + (tgt - hi), R, sb.gathered, sb.planes, (size_t)sb.rows_cap * c.hidden_size,
+    launch_score_head(m, s->hid, tf.d_src, tf.d_tgt, R, sb.gathered, sb.planes, (size_t)sb.rows_cap * c.hidden_size,
                       s->nplanes, sb.part, topk, sb.lp, sb.tk_ids, sb.tk_lp, st, &s->launches);
     ASRB_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
     std::vector<float> lp((size_t)R), tlp(topk ? (size_t)R * TK_MAX : 0);
@@ -1286,6 +1337,217 @@ void session_score_ids(Session* s, const float* const* samples, const int64_t* n
                        int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out) {
     score_impl(s, samples, n_samples, batch, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len, max_new_tokens, logprob_out,
                top_ids_out, top_lp_out);
+}
+
+// -------------------------------------------------------------------------------------------------
+// word-timing alignment (asrb_align_ids, DESIGN.md 4.10): a teacher-forced prefill of one candidate per utterance up to
+// the last listed layer, the audio-key probabilities of the listed heads folded into M as each layer passes, then DTW
+// -------------------------------------------------------------------------------------------------
+struct AlignHook : LayerHook {
+    Session* s = nullptr;
+    std::vector<int> first, count;      // per layer: its heads in the sorted list (count 0: not listed)
+    int last = -1, n_heads = 0, B = 0, maxN = 0, maxT = 0, maxNT = 0;
+    const int *d_heads = nullptr, *d_qrow0 = nullptr, *d_N = nullptr, *d_T = nullptr, *d_a0 = nullptr, *d_slot = nullptr;
+    const long long* d_moff = nullptr;
+    size_t plane = 0;
+    void run(int l) override {
+        if (count[l] == 0) return;
+        const asrb_dims& c = s->m->d.c;
+        AlignProbArgs pa{};
+        pa.q = s->qrot; pa.ldq = s->m->d.q_dim;
+        pa.k = s->kcache + (size_t)l * s->cache_layer_stride; pa.seg_stride = s->cache_seq_stride;
+        pa.head_stride = (size_t)s->max_ctx * c.head_dim; pa.hd = c.head_dim; pa.group = c.num_attention_heads / c.num_key_value_heads;
+        pa.qrow0 = d_qrow0; pa.N = d_N; pa.T = d_T; pa.a0 = d_a0; pa.slot = d_slot; pa.moff = d_moff;
+        pa.heads = d_heads + first[l]; pa.nheads = count[l]; pa.P = s->al.P; pa.plane = plane;
+        launch_align_probs(pa, B, maxN, s->st);
+        AlignFoldArgs fa{};
+        fa.N = d_N; fa.T = d_T; fa.moff = d_moff; fa.P = s->al.P; fa.plane = plane; fa.nheads = count[l]; fa.M = s->al.M;
+        fa.count = l == last ? n_heads : 0;
+        launch_align_fold(fa, B, maxT, maxNT, s->st);
+        s->launches += 3;
+    }
+};
+
+// the alignment scratch of a call: every buffer grown to fit first, then the old ones released (all or none)
+static void ensure_align_bufs(Session* s, size_t p_floats, size_t m_floats, size_t trace_words, size_t start_ints) {
+    Session::AlignBufs& b = s->al;
+    const bool grow = p_floats > b.p_cap || m_floats > b.m_cap || trace_words > b.trace_cap || start_ints > b.start_cap;
+    if (!grow) return;
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    AllocAll a;
+    const size_t pc = std::max(p_floats, b.p_cap), mc = std::max(m_floats, b.m_cap);
+    const size_t tc = std::max(trace_words, b.trace_cap), sc = std::max(start_ints, b.start_cap);
+    float* P = a.take<float>(pc); float* M = a.take<float>(mc);
+    uint32_t* trace = a.take<uint32_t>(tc); int* start = a.take<int>(sc);
+    a.commit(s);
+    for (void* p : {(void*)b.P, (void*)b.M, (void*)b.trace, (void*)b.start}) if (p) release_owned(s, p);
+    b.P = P; b.M = M; b.trace = trace; b.start = start;
+    b.p_cap = pc; b.m_cap = mc; b.trace_cap = tc; b.start_cap = sc;
+}
+
+// view_off: as transcribe_impl (asrb_align_segments); samples == view_off == nullptr: the ingested utterances
+static void align_impl(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* view_off,
+                       const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int64_t* const* ids,
+                       const int32_t* n_ids, const int32_t* text_from, const int32_t* heads, int n_heads, int max_ids,
+                       int32_t* start_out, int32_t* end_out) {
+    ASRB_REQUIRE(ids && n_ids && text_from && start_out && end_out, ASRB_ERR_INVALID, "align: null argument");
+    const bool ingested = samples == nullptr && view_off == nullptr;
+    if (ingested) {
+        batch = (int)s->ingested_n.size();
+        ASRB_REQUIRE(batch >= 1, ASRB_ERR_STATE, "align_ingested: no ingested audio");
+    }
+    Model& m = *s->m; const asrb_dims& c = m.d.c;
+    // ---- every argument checked before any work ----
+    ASRB_REQUIRE(batch >= 1 && batch <= s->max_batch, ASRB_ERR_INVALID, "align: batch outside [1, max_batch]");
+    ASRB_REQUIRE(max_ids >= 1, ASRB_ERR_INVALID, "align: max_ids must be >= 1");
+    check_context(s, batch);
+    int maxn = 0;
+    for (int b = 0; b < batch; ++b) {
+        if (!ingested && !view_off) {
+            ASRB_REQUIRE(samples[b] && n_samples[b] > 0 && n_samples[b] <= s->max_samples, ASRB_ERR_INVALID, "n_samples out of session capacity");
+            ASRB_REQUIRE(((n_samples[b] + 159) / 160) * 160 > 200, ASRB_ERR_INVALID, "utterance too short for reflect padding (needs > 200 samples)");
+        }
+        const int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
+        ASRB_REQUIRE(nl >= 0 && nl <= s->max_lang, ASRB_ERR_INVALID, "language prompt exceeds session capacity");
+        for (int i = 0; i < nl; ++i)
+            ASRB_REQUIRE(lang_ids[b][i] >= 0 && lang_ids[b][i] < c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
+        const int n = n_ids[b];
+        ASRB_REQUIRE(n >= 1 && n <= max_ids && n <= s->max_new, ASRB_ERR_INVALID,
+                     "align: n_ids outside [1, min(max_ids, the session's max_new_tokens)]");
+        ASRB_REQUIRE(ids[b], ASRB_ERR_INVALID, "align: null id row");
+        for (int i = 0; i < n; ++i) ASRB_REQUIRE(ids[b][i] >= 0 && ids[b][i] < c.vocab_size, ASRB_ERR_INVALID, "align: id out of vocabulary");
+        ASRB_REQUIRE(text_from[b] >= 0 && text_from[b] <= n - 1, ASRB_ERR_INVALID, "align: text_from outside [0, n_ids - 1]");
+        maxn = std::max(maxn, n);
+    }
+    ASRB_REQUIRE(n_heads >= 0 && (n_heads == 0 || heads), ASRB_ERR_INVALID, "align: bad head list");
+    std::vector<std::pair<int, int>> hs;
+    if (n_heads == 0) {
+        for (int l = c.num_hidden_layers / 2; l < c.num_hidden_layers; ++l)
+            for (int h = 0; h < c.num_attention_heads; ++h) hs.push_back({l, h});
+    } else {
+        for (int k = 0; k < n_heads; ++k) {
+            const int l = heads[2 * k], h = heads[2 * k + 1];
+            ASRB_REQUIRE(l >= 0 && l < c.num_hidden_layers && h >= 0 && h < c.num_attention_heads, ASRB_ERR_INVALID,
+                         "align: head outside the model");
+            hs.push_back({l, h});
+        }
+        std::sort(hs.begin(), hs.end());
+        ASRB_REQUIRE(std::adjacent_find(hs.begin(), hs.end()) == hs.end(), ASRB_ERR_INVALID, "align: duplicate head");
+    }
+    ASRB_REQUIRE(align_dtw_smem(maxn, 0, false) <= m.ctx->smem_optin, ASRB_ERR_INVALID, "align: too many ids for the DTW kernel");
+    ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
+    cudaStream_t st = s->st;
+    s->launches = 0; s->decode_steps = 0;
+    s->nbest_valid = false; s->lp_valid = false; s->tk_valid = 0;
+    s->al.N.clear(); s->al.T.clear(); s->al.moff.clear();
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
+    s->timing = true;
+    try { mel_impl(s, samples, n_samples, batch, view_off, nullptr); } catch (...) { s->timing = false; throw; }
+    s->timing = false;
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
+    session_encode(s, nullptr);
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[3], st));
+    s->stage = 2;                                     // the KV slots are overwritten: no run to continue after this call
+    const int B = batch;
+    // ---- plan: one candidate per utterance (slot b), no score head ----
+    const std::vector<int32_t> ones((size_t)B, 1);
+    const TfPlan tf = plan_teacher_forced(s, B, lang_ids, n_lang_ids, ones.data(), ids, n_ids, B, false);
+    std::vector<int> N(B), T(B), pi(7 * (size_t)B + hs.size());
+    std::vector<long long> moff(B), toff(B);
+    int* qrow0 = pi.data(); int* pN = qrow0 + B; int* pT = pN + B; int* a0 = pT + B; int* slot = a0 + B; int* soff = slot + B;
+    int* in_smem = soff + B; int* hl = in_smem + B;
+    long long sumNT = 0, words = 0; int sumN = 0, maxN = 0, maxT = 0, maxNT = 0; size_t smem = 0;
+    for (int b = 0; b < B; ++b) {
+        N[b] = n_ids[b] - text_from[b]; T[b] = s->T[b];
+        qrow0[b] = tf.srow0[b] + s->S[b] - 1 + text_from[b]; pN[b] = N[b]; pT[b] = T[b];
+        a0[b] = 9 + (int)context_of(s, b).size(); slot[b] = b; soff[b] = sumN;
+        moff[b] = sumNT; sumNT += (long long)N[b] * T[b]; sumN += N[b];
+        in_smem[b] = align_dtw_smem(N[b], T[b], true) <= m.ctx->smem_optin;
+        smem = std::max(smem, align_dtw_smem(N[b], T[b], in_smem[b] != 0));
+        toff[b] = words; if (!in_smem[b]) words += ((long long)N[b] * T[b] + 15) / 16;
+        maxN = std::max(maxN, N[b]); maxT = std::max(maxT, T[b]); maxNT = std::max(maxNT, N[b] * T[b]);
+    }
+    AlignHook hook;
+    hook.s = s; hook.first.assign(c.num_hidden_layers, 0); hook.count.assign(c.num_hidden_layers, 0);
+    int most = 0;
+    for (size_t k = 0; k < hs.size(); ++k) {
+        hl[k] = hs[k].second;
+        if (hook.count[hs[k].first]++ == 0) hook.first[hs[k].first] = (int)k;
+        most = std::max(most, hook.count[hs[k].first]);
+    }
+    hook.last = hs.back().first; hook.n_heads = (int)hs.size();
+    ensure_align_bufs(s, (size_t)most * sumNT, (size_t)sumNT, (size_t)words, (size_t)sumN + pi.size() + 4 * (size_t)B + 2);
+    // the per-utterance plan rides behind the start tokens: [sumN starts | ints | long longs (8-byte aligned)]
+    Session::AlignBufs& ab = s->al;
+    int* d_pi = ab.start + sumN;
+    long long* d_pl = reinterpret_cast<long long*>(ab.start + ((sumN + pi.size() + 1) & ~(size_t)1));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(d_pi, pi.data(), pi.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(d_pl, moff.data(), B * sizeof(long long), cudaMemcpyHostToDevice, st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(d_pl + B, toff.data(), B * sizeof(long long), cudaMemcpyHostToDevice, st));
+    ASRB_CUDA_CHECK(cudaMemsetAsync(ab.M, 0, (size_t)sumNT * sizeof(float), st));
+    if (words) ASRB_CUDA_CHECK(cudaMemsetAsync(ab.trace, 0, (size_t)words * sizeof(uint32_t), st));
+    hook.B = B; hook.maxN = maxN; hook.maxT = maxT; hook.maxNT = maxNT; hook.plane = (size_t)sumNT;
+    hook.d_qrow0 = d_pi + (qrow0 - pi.data()); hook.d_N = d_pi + (pN - pi.data()); hook.d_T = d_pi + (pT - pi.data());
+    hook.d_a0 = d_pi + (a0 - pi.data()); hook.d_slot = d_pi + (slot - pi.data()); hook.d_heads = d_pi + (hl - pi.data());
+    hook.d_moff = d_pl;
+    prefill_layers(s, tf.totS, B, tf.maxrows, tf.fan ? &tf.fan_plan : nullptr, tf.d_qpos0, s->audio, hook.last + 1, &hook);
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
+    AlignDtwArgs da{};
+    da.N = hook.d_N; da.T = hook.d_T; da.moff = d_pl; da.M = ab.M; da.smem_trace = d_pi + (in_smem - pi.data());
+    da.trace = ab.trace; da.toff = d_pl + B; da.start = ab.start; da.soff = d_pi + (soff - pi.data());
+    launch_align_dtw(da, B, smem, st);
+    s->launches += 1;
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
+    std::vector<int> tok((size_t)sumN);
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(tok.data(), ab.start, (size_t)sumN * sizeof(int), cudaMemcpyDeviceToHost, st));
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int i = 0; i < 5; ++i) ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[i], s->ev[i], s->ev[i + 1]));
+    ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[5], s->ev[0], s->ev[5]));
+    ab.N = N; ab.T = T; ab.moff = moff;
+    // ---- frames: audio token t of chunk k starts at frame k * chunk_frames + 8 t ----
+    const int cf = m.d.chunk_frames;
+    for (int b = 0; b < B; ++b) {
+        std::vector<int> frame;
+        for (int k = 0; k < s->C[b]; ++k) {
+            const int fr = (int)std::min<int64_t>(cf, s->F[b] - (int64_t)k * cf);
+            const int valid = conv_out_len(conv_out_len(conv_out_len(fr)));
+            for (int t = 0; t < valid; ++t) frame.push_back(k * cf + 8 * t);
+        }
+        int32_t* so = start_out + (size_t)b * max_ids; int32_t* eo = end_out + (size_t)b * max_ids;
+        for (int x = 0; x < max_ids; ++x) { so[x] = -1; eo[x] = -1; }
+        const int f = text_from[b];
+        for (int i = 0; i < N[b]; ++i) so[f + i] = frame[tok[soff[b] + i]];
+        for (int i = 0; i < N[b]; ++i) eo[f + i] = i + 1 < N[b] ? so[f + i + 1] : (int32_t)s->F[b];
+    }
+}
+
+void session_align_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* const* lang_ids,
+                       const int32_t* n_lang_ids, const int64_t* const* ids, const int32_t* n_ids, const int32_t* text_from,
+                       const int32_t* heads, int n_heads, int max_ids, int32_t* start_out, int32_t* end_out) {
+    align_impl(s, samples, n_samples, batch, nullptr, lang_ids, n_lang_ids, ids, n_ids, text_from, heads, n_heads, max_ids,
+               start_out, end_out);
+}
+
+void session_align_segments(Session* s, int n, const int32_t* file, const int64_t* start, const int64_t* end,
+                            const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int64_t* const* ids,
+                            const int32_t* n_ids, const int32_t* text_from, const int32_t* heads, int n_heads, int max_ids,
+                            int32_t* start_out, int32_t* end_out) {
+    std::vector<int64_t> off, len;
+    segment_views(s, n, file, start, end, off, len, "align_segments");
+    align_impl(s, nullptr, len.data(), n, off.data(), lang_ids, n_lang_ids, ids, n_ids, text_from, heads, n_heads, max_ids,
+               start_out, end_out);
+}
+
+void session_last_align_dims(Session* s, int b, int32_t* n_rows, int32_t* n_tokens) {
+    ASRB_REQUIRE(b >= 0 && b < (int)s->al.N.size(), ASRB_ERR_STATE, "last_align_dims: no alignment for this index");
+    if (n_rows) *n_rows = s->al.N[b];
+    if (n_tokens) *n_tokens = s->al.T[b];
+}
+
+void session_align_matrix_read(Session* s, int b, float* out) {
+    ASRB_REQUIRE(b >= 0 && b < (int)s->al.N.size(), ASRB_ERR_STATE, "align_matrix_read: no alignment for this index");
+    ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));
+    ASRB_CUDA_CHECK(cudaMemcpy(out, s->al.M + s->al.moff[b], (size_t)s->al.N[b] * s->al.T[b] * sizeof(float), cudaMemcpyDeviceToHost));
 }
 
 // -------------------------------------------------------------------------------------------------

@@ -20,6 +20,7 @@ import numpy as np
 
 from . import _lib
 from .config import AsrConfig
+from .text import Word, build_words
 
 EOS_TOKEN_IDS = (151643, 151645)      # inference.rs:154
 MAX_NEW_TOKENS = 4096                 # inference.rs:153
@@ -261,6 +262,8 @@ class TranscribeResult:           # inference.rs:270-274
     nbest: Optional[List[Tuple[str, float]]] = None   # transcribe(beam_size=K > 1): the K hypotheses as (text, score), ranked
     # transcribe(max_segment_s=...): the segments as (start_s, end_s, text), in time order
     segments: Optional[List[Tuple[float, float, str]]] = None
+    # transcribe(word_timestamps=True): the words of the transcript with their times (text.Word), in order
+    words: Optional[List["Word"]] = None
 
 
 @dataclass
@@ -276,6 +279,7 @@ class LongSegment:
     eos_top_logprobs: Optional[List[Tuple[int, float]]] = None
     temperature: Optional[float] = None
     nbest: Optional[List[Tuple[List[int], float, float, int]]] = None
+    words: Optional[List["Word"]] = None            # word_timestamps=True: times absolute in the file
 
 
 @dataclass
@@ -336,6 +340,63 @@ def check_candidates(candidates, batch: int, vocab: int) -> List[List[List[int]]
             rows.append(ids)
         out.append(rows)
     return out
+
+
+@dataclass
+class Alignment:
+    """Word-timing alignment of one utterance (asrb_align_ids): entry k is id text_from + k of the aligned ids, its start
+    and end in 10 ms mel frames (the end is the next id's start, the last id's the utterance's frame count)."""
+    text_from: int
+    start_frames: List[int]
+    end_frames: List[int]
+
+    @property
+    def start_s(self) -> List[float]:
+        return [f * FRAME_S for f in self.start_frames]
+
+    @property
+    def end_s(self) -> List[float]:
+        return [f * FRAME_S for f in self.end_frames]
+
+
+FRAME_S = 0.01                  # one mel frame: 160 samples at 16 kHz
+
+
+def check_align_ids(ids, text_from, batch: int, vocab: int) -> Tuple[List[List[int]], List[int]]:
+    """ids[b]: a non-empty id list per utterance, every id in [0, vocab); text_from: None (all 0) or one int per
+    utterance in [0, len(ids[b]) - 1]."""
+    if len(ids) != batch:
+        raise ValueError(f"need one id list per utterance: {len(ids)} for {batch}")
+    rows = [[int(i) for i in r] for r in ids]
+    for b, r in enumerate(rows):
+        if not r:
+            raise ValueError(f"utterance {b}: no ids to align")
+        if any(i < 0 or i >= vocab for i in r):
+            raise ValueError(f"utterance {b}: id out of [0, {vocab})")
+    tf = [0] * batch if text_from is None else [int(f) for f in text_from]
+    if len(tf) != batch or any(not 0 <= f < len(r) for f, r in zip(tf, rows)):
+        raise ValueError("text_from must be None or one index per utterance in [0, len(ids[b]) - 1]")
+    return rows, tf
+
+
+def check_alignment_heads(heads, layers: int, nq: int) -> List[Tuple[int, int]]:
+    """None -> [] (the library's default: every head of the second half of the layers); else distinct (layer, head)
+    pairs inside the model."""
+    if heads is None:
+        return []
+    out = [(int(l), int(h)) for l, h in heads]
+    if not out:
+        raise ValueError("alignment_heads must be None or a non-empty list of (layer, head) pairs")
+    if any(not (0 <= l < layers and 0 <= h < nq) for l, h in out) or len(set(out)) != len(out):
+        raise ValueError(f"alignment_heads: distinct (layer, head) pairs with layer < {layers} and head < {nq}")
+    return out
+
+
+def text_start(ids: Sequence[int], asr_text_id: Optional[int]) -> int:
+    """Index of the first transcript id: just after the <asr_text> id when it occurs, else 0."""
+    if asr_text_id is not None and asr_text_id in ids:
+        return list(ids).index(asr_text_id) + 1
+    return 0
 
 
 def score_waves(n_cand: Sequence[int], slots: int) -> List[List[int]]:
@@ -911,6 +972,113 @@ class AsrInference:
         r = self.score_pcm([pcm], [rate], [cands])[0]
         return language_probabilities(names, [c.sum_logprob for c in r])
 
+    # ---- word-timing alignment (asrb_align_ids, DESIGN.md 4.10) ---------------------------------------------------
+    def align_ids(self, clips: Sequence[np.ndarray], ids: Sequence[Sequence[int]], text_from: Optional[Sequence[int]] = None,
+                  language_ids: Optional[Sequence] = None, context_ids: Optional[Sequence] = None,
+                  alignment_heads: Optional[Sequence[Tuple[int, int]]] = None) -> List[Alignment]:
+        """Start and end of every id ids[b][text_from[b]:] in clip b, from the decoder's attention over the audio in one
+        teacher-forced pass over the prompt transcribe_ids builds (language ids and context included) and ids[b]
+        (normally the decoded ids followed by EOS).  `alignment_heads`: (layer, query head) pairs, None = every head of
+        the second half of the layers.  More clips than SCORE_SLOTS run in several calls."""
+        B = len(clips)
+        t = self.config.text
+        rows, tf = check_align_ids(ids, text_from, B, t.vocab_size)
+        heads = check_alignment_heads(alignment_heads, t.num_hidden_layers, t.num_attention_heads)
+        ctx = check_context_ids(context_ids, B, t.vocab_size)
+        out: List[Alignment] = [None] * B
+        for wave in score_waves([1] * B, SCORE_SLOTS):
+            arrs, ptrs, lens = self._pack_samples([clips[b] for b in wave])
+            lang = None if language_ids is None else [language_ids[b] for b in wave]
+            keep, lptrs, llens, mx = self._pack_lang(lang, len(wave))
+            wrows = [rows[b] for b in wave]
+            wctx = None if ctx is None else [ctx[b] for b in wave]
+            s = self._ensure_session(len(wave), max(a.shape[0] for a in arrs), mx, max(len(r) for r in wrows), _max_len(wctx))
+            res = self._align(s, wrows, [tf[b] for b in wave], heads, wctx,
+                              lambda *a: self._lib.asrb_align_ids(s, ptrs, lens, len(wave), lptrs, llens, *a))
+            for b, r in zip(wave, res):
+                out[b] = r
+        return out
+
+    def align_pcm(self, pcms: Sequence, rates: Sequence[int], ids: Sequence[Sequence[int]],
+                  text_from: Optional[Sequence[int]] = None, language_ids: Optional[Sequence] = None,
+                  context_ids: Optional[Sequence] = None,
+                  alignment_heads: Optional[Sequence[Tuple[int, int]]] = None) -> List[Alignment]:
+        """align_ids with step 1 on the GPU: raw PCM in (as transcribe_pcm)."""
+        B = len(pcms)
+        t = self.config.text
+        rows, tf = check_align_ids(ids, text_from, B, t.vocab_size)
+        heads = check_alignment_heads(alignment_heads, t.num_hidden_layers, t.num_attention_heads)
+        ctx = check_context_ids(context_ids, B, t.vocab_size)
+        out: List[Alignment] = [None] * B
+        for wave in score_waves([1] * B, SCORE_SLOTS):
+            lang = None if language_ids is None else [language_ids[b] for b in wave]
+            keep, lptrs, llens, mx = self._pack_lang(lang, len(wave))
+            wrows = [rows[b] for b in wave]
+            wctx = None if ctx is None else [ctx[b] for b in wave]
+            s, _arrs, _n = self._ingest([pcms[b] for b in wave], [rates[b] for b in wave], mx, max(len(r) for r in wrows),
+                                        max_context=_max_len(wctx))
+            res = self._align(s, wrows, [tf[b] for b in wave], heads, wctx,
+                              lambda *a: self._lib.asrb_align_ingested(s, lptrs, llens, *a))
+            for b, r in zip(wave, res):
+                out[b] = r
+        return out
+
+    def _align(self, s, rows: List[List[int]], tf: List[int], heads: List[Tuple[int, int]], context_ids,
+               call) -> List[Alignment]:
+        """One alignment call on session s: `call(ids, n_ids, text_from, heads, n_heads, max_ids, start, end)`."""
+        B = len(rows)
+        max_ids = max(len(r) for r in rows)
+        arrs = [np.ascontiguousarray(r, dtype=np.int64) for r in rows]
+        iptrs = (C.POINTER(C.c_int64) * B)(*[a.ctypes.data_as(C.POINTER(C.c_int64)) for a in arrs])
+        n_ids = (C.c_int32 * B)(*[len(r) for r in rows])
+        tfa = (C.c_int32 * B)(*tf)
+        harr = np.ascontiguousarray(np.array(heads, dtype=np.int32).reshape(-1, 2))
+        st = np.empty((B, max_ids), dtype=np.int32)
+        en = np.empty((B, max_ids), dtype=np.int32)
+        try:
+            if context_ids is not None:
+                self._set_context(s, context_ids)
+            _lib.check(call(iptrs, n_ids, tfa, harr.ctypes.data_as(C.POINTER(C.c_int32)) if heads else None, len(heads),
+                            int(max_ids), st.ctypes.data_as(C.POINTER(C.c_int32)), en.ctypes.data_as(C.POINTER(C.c_int32))))
+        finally:
+            if context_ids is not None:
+                self._set_context(s, None)
+        self._B = B
+        return [Alignment(f, [int(v) for v in st[b, f:len(r)]], [int(v) for v in en[b, f:len(r)]])
+                for b, (r, f) in enumerate(zip(rows, tf))]
+
+    def last_align_matrix(self, b: int) -> np.ndarray:
+        """M [N_b][T_b] of utterance b of the last alignment call (asrb_align_matrix_read): the head-mean of the
+        normalised, filtered audio attention that the DTW ran on.  For choosing alignment heads on a checkpoint."""
+        n, t = C.c_int32(), C.c_int32()
+        _lib.check(self._lib.asrb_last_align_dims(self._session, int(b), C.byref(n), C.byref(t)))
+        a = np.empty((n.value, t.value), dtype=np.float32)
+        _lib.check(self._lib.asrb_align_matrix_read(self._session, int(b), a.ctypes.data_as(C.POINTER(C.c_float))))
+        return a
+
+    def _asr_text_id(self) -> Optional[int]:
+        return self.tokenizer.token_to_id("<asr_text>") if self.tokenizer is not None else None
+
+    def _decode_fn(self):
+        return self.tokenizer.decode if self.tokenizer is not None else (lambda ids: "".join(f" {i}" for i in ids))
+
+    def _word_language(self, ids: List[int], language: Optional[str]) -> Optional[str]:
+        """The language that decides the word split: the tag the decoded ids carry, else `language`."""
+        if self.tokenizer is not None:
+            from .text import parse_asr_output
+            tag = parse_asr_output(self.tokenizer.decode(ids), False)[0]
+            if tag != "unknown":
+                return tag
+        return language
+
+    def _words(self, ids: List[int], al: Alignment, logprobs: Optional[List[float]], language: Optional[str],
+               offset_s: float = 0.0) -> List[Word]:
+        """Words of a decoded id list whose ids + [EOS] were aligned from al.text_from on."""
+        f = al.text_from
+        text = ids[f:]
+        lp = logprobs[f:] if logprobs is not None else None
+        return build_words(self._decode_fn(), text, al.start_s[:len(text)], al.start_s[len(text)], lp, language, offset_s)
+
     # ---- GPU-side audio ingest (step 1, src/audio.rs:162-245) -------------------------------------------
     _PCM_FMT = {"int16": 0, "float32": 1, "int32": 2}
 
@@ -1023,13 +1191,19 @@ class AsrInference:
                         temperature: Union[float, Sequence[float]] = 0.0, seed: int = 0,
                         logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
                         length_penalty: Optional[float] = None, context_ids: Optional[Sequence] = None,
-                        no_repeat_ngram_size: int = 0, repetition_penalty: float = 1.0) -> "LongResult":
+                        no_repeat_ngram_size: int = 0, repetition_penalty: float = 1.0, word_timestamps: bool = False,
+                        alignment_heads: Optional[Sequence[Tuple[int, int]]] = None,
+                        language: Optional[str] = None) -> "LongResult":
         """Long recordings: ingest the files (raw PCM, as transcribe_pcm) into the long-audio buffer, cut them on the GPU
         into segments of at most `max_segment_s` at the quietest 100 ms window of the last `search_s` before each limit
         (asrb_segment_long), and decode the segments as views of that buffer (asrb_transcribe_segments) in waves of
         `batch` segments in (file, time) order, `batch // beam_size` with a beam.  `max_new_tokens` applies per segment.
         Every other keyword is that of transcribe_pcm, per segment: the language ids and context of a file apply to each
         of its segments; temperature fallback re-runs only the failing segments, in waves of their own.
+        `word_timestamps`: also align every segment's decoded ids + EOS in place (asrb_align_segments, waves of `batch`)
+        and fill LongSegment.words with times absolute in the file; it records log-probabilities for the word
+        probabilities.  `alignment_heads` as in align_ids; `language`: the forced language's name, which decides how
+        words are split (text.split_words) when the ids carry no language tag.
         Returns per file its segments in time order."""
         max_seg, search = check_segmenting(max_segment_s, search_s)
         n_files = len(pcms)
@@ -1050,7 +1224,9 @@ class AsrInference:
             raise ValueError("language_ids must be None or one entry per file")
         longest = max(-(-a.shape[0] * MEL_SAMPLE_RATE // int(r)) for a, r in zip(arrs, rates))
         mx = _max_len(language_ids)
-        s = self._ensure_session(batch, min(max_seg, max(longest, 201)), mx, max_new_tokens, _max_len(ctx))
+        # word timestamps align the decoded ids and the EOS: one id more than the decode's cap
+        s = self._ensure_session(batch, min(max_seg, max(longest, 201)), mx, max_new_tokens + int(bool(word_timestamps)),
+                                 _max_len(ctx))
         s, n = self._ingest_long(arrs, rates, s)
         self._long_files = n_files
         cuts = self.segment_long(max_seg, search)
@@ -1074,7 +1250,25 @@ class AsrInference:
                                           s, m, fl, st, en, lptrs, llens, int(max_new_tokens), ids, nn), rep))
                 self._long_waves += 1
             return _concat_runs(runs)
-        r = self._sampled(len(segs), once, temperature, seed, logprob_threshold, logprobs, tk, beam_size, length_penalty)
+        heads = check_alignment_heads(alignment_heads, self.config.text.num_hidden_layers,
+                                      self.config.text.num_attention_heads) if word_timestamps else []
+        r = self._sampled(len(segs), once, temperature, seed, logprob_threshold, logprobs or word_timestamps, tk, beam_size,
+                          length_penalty)
+        als: List[Alignment] = []
+        if word_timestamps:
+            asr_text = self._asr_text_id()
+            for w0 in range(0, len(segs), batch):
+                wave = list(range(w0, min(w0 + batch, len(segs))))
+                m = len(wave)
+                fl = (C.c_int32 * m)(*[segs[i][0] for i in wave])
+                st = (C.c_int64 * m)(*[segs[i][1] for i in wave])
+                en = (C.c_int64 * m)(*[segs[i][2] for i in wave])
+                lang = None if language_ids is None else [language_ids[segs[i][0]] for i in wave]
+                keep, lptrs, llens, _ = self._pack_lang(lang, m)
+                wctx = None if ctx is None else [ctx[segs[i][0]] for i in wave]
+                rows = [r.ids[i] + [EOS_ID] for i in wave]
+                als += self._align(s, rows, [text_start(r.ids[i], asr_text) for i in wave], heads, wctx,
+                                   lambda *a: self._lib.asrb_align_segments(s, m, fl, st, en, lptrs, llens, *a))
         out: List[List[LongSegment]] = [[] for _ in range(n_files)]
         for i, (f, a, b) in enumerate(segs):
             seg = LongSegment(a / MEL_SAMPLE_RATE, b / MEL_SAMPLE_RATE, r.ids[i])
@@ -1086,6 +1280,9 @@ class AsrInference:
                 seg.temperature = r.temperatures[i]
             if r.nbest is not None:
                 seg.nbest = r.nbest[i]
+            if word_timestamps:
+                seg.words = self._words(r.ids[i], als[i], r.logprobs[i], self._word_language(r.ids[i], language),
+                                        a / MEL_SAMPLE_RATE)
             out[f].append(seg)
         return LongResult(out, r.stage_ms, r.kernels_launched, r.decode_steps, len(segs), self._long_waves)
 
@@ -1095,7 +1292,8 @@ class AsrInference:
                    logprob_threshold: Optional[float] = -1.0, beam_size: int = 1,
                    length_penalty: Optional[float] = None, context: Optional[str] = None,
                    max_segment_s: Optional[float] = None, no_repeat_ngram_size: int = 0,
-                   repetition_penalty: float = 1.0) -> TranscribeResult:
+                   repetition_penalty: float = 1.0, word_timestamps: bool = False,
+                   alignment_heads: Optional[Sequence[Tuple[int, int]]] = None) -> TranscribeResult:
         """AsrInference::transcribe (inference.rs:89-213): step 1 (WAV payload -> mono 16 kHz; on the GPU by default,
         `gpu_ingest=False` = the host loader) -> steps 2-8 on the GPU -> step 9 (detokenise + parse, host; needs
         tokenizer.json, else raw_output is the id list as text).  `logprobs`: also fill token_logprobs / avg_logprob;
@@ -1105,7 +1303,10 @@ class AsrInference:
         of the kept attempt; `nbest` holds the beam's hypotheses as (text, score).  `context`: text placed in the prompt's
         system turn to bias recognition (keywords, names, related text; needs tokenizer.json; "" = none).
         `max_segment_s`: None decodes the file in one pass; a number of seconds runs transcribe_long with it (search
-        window min(5 s, half of it, in whole 10 ms)) and `max_new_tokens` per segment: see _long_result."""
+        window min(5 s, half of it, in whole 10 ms)) and `max_new_tokens` per segment: see _long_result.
+        `word_timestamps`: also fill `words` (text.Word: start, end, text, probability) by aligning the kept
+        hypothesis + EOS from just after its <asr_text> id (align_ids; per segment with `max_segment_s`), with
+        `alignment_heads` as in align_ids; it records log-probabilities for the word probabilities."""
         from .audio import load_wav, read_wav_pcm
         from .text import context_prompt_ids, language_prompt_ids, parse_asr_output
         lang_ids = language_prompt_ids(self.tokenizer, language)
@@ -1121,17 +1322,30 @@ class AsrInference:
             lr = self.transcribe_long([pcm], [rate], max_segment_s=max_segment_s, search_s=default_search_s(max_segment_s),
                                       language_ids=[lang_ids] if lang_ids is not None else None,
                                       max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs,
-                                      **sampling)
+                                      word_timestamps=word_timestamps, alignment_heads=alignment_heads,
+                                      language=language, **sampling)
             return self._long_result(lr.files[0], language, logprobs, top_logprobs)
+        lang_kw = dict(language_ids=[lang_ids] if lang_ids is not None else None)
+        heads = check_alignment_heads(alignment_heads, self.config.text.num_hidden_layers,
+                                      self.config.text.num_attention_heads) if word_timestamps else None
+        lp = logprobs or word_timestamps
         if gpu_ingest:
             pcm, rate = read_wav_pcm(audio_path)
-            r = self.transcribe_pcm([pcm], [rate], language_ids=[lang_ids] if lang_ids is not None else None,
-                                    max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs, **sampling)
+            r = self.transcribe_pcm([pcm], [rate], max_new_tokens=max_new_tokens, logprobs=lp, top_logprobs=top_logprobs,
+                                    **lang_kw, **sampling)
         else:
             samples = load_wav(audio_path, MEL_SAMPLE_RATE)
-            r = self.transcribe_ids([samples], language_ids=[lang_ids] if lang_ids is not None else None,
-                                    max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs, **sampling)
+            r = self.transcribe_ids([samples], max_new_tokens=max_new_tokens, logprobs=lp, top_logprobs=top_logprobs,
+                                    **lang_kw, **sampling)
         ids = r.ids[0]
+        al = None
+        if word_timestamps:
+            tf = [text_start(ids, self._asr_text_id())]
+            ctx_kw = dict(context_ids=[ctx_ids] if ctx_ids else None, alignment_heads=heads or None)
+            if gpu_ingest:
+                al = self.align_pcm([pcm], [rate], [ids + [EOS_ID]], text_from=tf, **lang_kw, **ctx_kw)[0]
+            else:
+                al = self.align_ids([samples], [ids + [EOS_ID]], text_from=tf, **lang_kw, **ctx_kw)[0]
 
         def parse(ids):
             raw = self.tokenizer.decode(ids) if self.tokenizer is not None else " ".join(str(i) for i in ids)
@@ -1148,6 +1362,8 @@ class AsrInference:
         if top_logprobs:
             res.top_logprobs = r.top_logprobs[0]
             res.eos_top_logprobs = r.eos_top_logprobs[0]
+        if al is not None:
+            res.words = self._words(ids, al, r.logprobs[0], language if language is not None else lang)
         return res
 
     def _long_result(self, segs: List[LongSegment], language: Optional[str], logprobs: bool,
@@ -1183,6 +1399,8 @@ class AsrInference:
         if top_logprobs:
             res.top_logprobs = sum((sg.top_logprobs for sg in segs), [])
             res.eos_top_logprobs = segs[-1].eos_top_logprobs
+        if segs[0].words is not None:
+            res.words = sum((sg.words for sg in segs), [])
         return res
 
     # ---- stage-level calls (the calls transcribe() makes; used by the parity tests) ----

@@ -76,6 +76,19 @@ extern "C" {
     pub fn asrb_score_ingested(s: *mut asrb_session, lang_ids: *const *const i64, n_lang_ids: *const i32, n_cand: *const i32,
                                cand_ids: *const *const i64, cand_len: *const i32, max_new_tokens: c_int, logprob_out: *mut f32,
                                top_ids_out: *mut i32, top_lp_out: *mut f32) -> c_int;
+    pub fn asrb_align_ids(s: *mut asrb_session, samples: *const *const f32, n_samples: *const i64, batch: c_int,
+                          lang_ids: *const *const i64, n_lang_ids: *const i32, ids: *const *const i64, n_ids: *const i32,
+                          text_from: *const i32, heads: *const i32, n_heads: c_int, max_ids: c_int,
+                          start_frame_out: *mut i32, end_frame_out: *mut i32) -> c_int;
+    pub fn asrb_align_ingested(s: *mut asrb_session, lang_ids: *const *const i64, n_lang_ids: *const i32, ids: *const *const i64,
+                               n_ids: *const i32, text_from: *const i32, heads: *const i32, n_heads: c_int, max_ids: c_int,
+                               start_frame_out: *mut i32, end_frame_out: *mut i32) -> c_int;
+    pub fn asrb_align_segments(s: *mut asrb_session, n: c_int, file: *const i32, start: *const i64, end: *const i64,
+                               lang_ids: *const *const i64, n_lang_ids: *const i32, ids: *const *const i64, n_ids: *const i32,
+                               text_from: *const i32, heads: *const i32, n_heads: c_int, max_ids: c_int,
+                               start_frame_out: *mut i32, end_frame_out: *mut i32) -> c_int;
+    pub fn asrb_last_align_dims(s: *mut asrb_session, b: c_int, n_rows_out: *mut i32, n_tokens_out: *mut i32) -> c_int;
+    pub fn asrb_align_matrix_read(s: *mut asrb_session, b: c_int, out: *mut f32) -> c_int;
     pub fn asrb_session_device_ids(s: *mut asrb_session, ids_dev: *mut *const i32, lens_dev: *mut *const i32, row_stride: *mut c_int, batch: *mut c_int) -> c_int;
     pub fn asrb_session_stats(s: *mut asrb_session, out: *mut i64, n: c_int) -> c_int;
     pub fn asrb_session_set_option(s: *mut asrb_session, key: *const c_char, value: *const c_char) -> c_int;

@@ -252,6 +252,32 @@ impl B200Engine {
         run
     }
 
+    /// Word timing (`asrb_align_ids`, `include/asr_b200.h`): the start and end, in 10 ms mel frames, of every id
+    /// `ids[text_from..]` in `samples`, from the decoder's attention over the audio in one teacher-forced pass over the
+    /// prompt and `ids` (normally the decoded ids followed by EOS 151645).  `heads`: (layer, query head) pairs, empty =
+    /// every head of the second half of the layers.  `ids.len()` may not exceed `max_new_tokens`.
+    pub fn align_ids(&self, samples: &[f32], lang_ids: Option<&[i64]>, ids: &[i64], text_from: usize, heads: &[(i32, i32)])
+        -> Result<Vec<(i32, i32)>> {
+        if ids.is_empty() || text_from >= ids.len() { return Err(anyhow!("need text_from < ids.len() and a non-empty ids")); }
+        let n = ids.len();
+        let (mut st, mut en) = (vec![-1i32; n], vec![-1i32; n]);
+        let sp = [samples.as_ptr()];
+        let sl = [samples.len() as i64];
+        let lp = [lang_ids.map_or(ptr::null(), |v| v.as_ptr())];
+        let ll = [lang_ids.map_or(0, |v| v.len() as i32)];
+        let ip = [ids.as_ptr()];
+        let il = [n as i32];
+        let tf = [text_from as i32];
+        let hs: Vec<i32> = heads.iter().flat_map(|&(l, h)| [l, h]).collect();
+        let session = self.session_for(samples.len())?;
+        check(unsafe {
+            ffi::asrb_align_ids(session, sp.as_ptr(), sl.as_ptr(), 1, lp.as_ptr(), ll.as_ptr(), ip.as_ptr(), il.as_ptr(),
+                                tf.as_ptr(), if hs.is_empty() { ptr::null() } else { hs.as_ptr() }, heads.len() as i32,
+                                n as i32, st.as_mut_ptr(), en.as_mut_ptr())
+        })?;
+        Ok((text_from..n).map(|i| (st[i], en[i])).collect())
+    }
+
     /// One live stream on a session of its own (dropped with the returned handle): push 16 kHz mono f32 audio as it
     /// arrives and get the hypothesis of everything received so far (`asrb_stream_push`, one stream).  `max_samples`
     /// bounds the stream's length; the forced prefix may hold up to 8 ids per second of audio plus `max_new_tokens`.
