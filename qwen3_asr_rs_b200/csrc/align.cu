@@ -1,7 +1,8 @@
 // align.cu -- word-timing alignment from the decoder's audio attention (asrb_align_ids, DESIGN.md 4.10).
 //
 //   align_probs_kernel   softmax over the utterance's audio keys of each aligned row, one listed head of one layer
-//   align_zscore_kernel  per (head, column) mean / population std over the rows, z-scores in place (std = 0: z = 0)
+//   align_zscore_kernel  per (head, column) mean / population std over the rows, z-scores in place (std = 0: z = 0;
+//                        a column of equal values has std exactly 0)
 //   align_median_kernel  per element: width-7 median along the columns (mirror padding) of every listed head of the
 //                        layer, added into M in list order; the last listed layer divides by the head count
 //   align_dtw_kernel     one CTA per utterance: DTW on -M over anti-diagonals, 2-bit trace, backtrace on the device
@@ -80,9 +81,12 @@ __global__ void align_zscore_kernel(AlignFoldArgs a) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= T) return;
     float* P = a.P + (size_t)hl * a.plane + a.moff[b] + j;
+    // the mean as P[0] + mean(P - P[0]): a column of equal values has mean == P[0] exactly, so std = 0 and z = 0 (a
+    // plain fp32 sum of N equal values rounds, which left such columns at z = +-1)
+    const float p0 = P[0];
     float sum = 0.f;
-    for (int i = 0; i < N; ++i) sum += P[(size_t)i * T];
-    const float mean = sum / (float)N;
+    for (int i = 0; i < N; ++i) sum += P[(size_t)i * T] - p0;
+    const float mean = p0 + sum / (float)N;
     float var = 0.f;
     for (int i = 0; i < N; ++i) { const float d = P[(size_t)i * T] - mean; var = fmaf(d, d, var); }
     const float sd = sqrtf(var / (float)N);
@@ -179,9 +183,11 @@ __global__ void __launch_bounds__(DTW_THREADS) align_dtw_kernel(AlignDtwArgs a) 
 
 }  // namespace
 
+size_t align_probs_smem(int hd) { return (size_t)(PROB_ROWS * hd + PROB_KEYS * (hd + 1)) * sizeof(float); }
+
 void launch_align_probs(const AlignProbArgs& a, int B, int maxN, cudaStream_t st) {
-    const size_t smem = (size_t)(PROB_ROWS * a.hd + PROB_KEYS * (a.hd + 1)) * sizeof(float);
-    ASRB_REQUIRE(smem <= 64 * 1024, ASRB_ERR_INVALID, "align: head_dim too large for the probability kernel");
+    const size_t smem = align_probs_smem(a.hd);
+    ASRB_REQUIRE(smem <= ALIGN_PROBS_SMEM_MAX, ASRB_ERR_INVALID, "align: head_dim too large for the probability kernel");
     ASRB_CUDA_CHECK(cudaFuncSetAttribute(align_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((maxN + PROB_ROWS - 1) / PROB_ROWS, a.nheads, B);
     align_probs_kernel<<<grid, PROB_THREADS, smem, st>>>(a);

@@ -271,9 +271,17 @@ struct ScorePart {                  // one (row, column slice): max logit, sum o
     float m, s, t;
     float tv[TK_MAX]; int ti[TK_MAX];   // TOPK: the slice's best (logit, id), best first
 };
+struct ScoreHeadPlan { int tiles_m = 0, tiles_n = 0, nslices = 0, grid = 0; };
+// the head's work items (M tile, column slice) and persistent grid on `sms` SMs; grid_cap > 0 caps the grid further
+ScoreHeadPlan plan_score_head(int rows, int V, int sms, int grid_cap);
 int score_slices(const Model& m);
 void check_score_head(const Model& m);   // throws ASRB_ERR_INVALID for a shape the wgmma head cannot take
-// rows r of hid[d_src[r]] -> final norm -> lm_head; lp_out[r] = log p(d_target[r]), with topk the 8 best of each row
+// rows r of hid[d_src[r]] -> final norm -> lm_head; lp_out[r] = log p(d_target[r]), with topk the 8 best of each row.
+// The first form takes the head's weights and dims explicitly (the probes); the second is the model's, on all its SMs
+void launch_score_head(const bf16* lm_head, const float* final_norm, int H, int V, float eps, int sms, int grid_cap,
+                       const float* hid, const int* d_src, const int* d_target, int rows, float* gathered, bf16* planes,
+                       size_t plane_stride, int nplanes, ScorePart* part, bool topk, float* lp_out, int* tk_ids,
+                       float* tk_lp, cudaStream_t st, int64_t* launches);
 void launch_score_head(const Model& m, const float* hid, const int* d_src, const int* d_target, int rows, float* gathered,
                        bf16* planes, size_t plane_stride, int nplanes, ScorePart* part, bool topk, float* lp_out,
                        int* tk_ids, float* tk_lp, cudaStream_t st, int64_t* launches);
@@ -300,6 +308,8 @@ struct AlignDtwArgs {
     uint32_t* trace; const long long* toff;
     int* start; const int* soff;               // start[soff[b] + i]: least column of the path in row i
 };
+constexpr size_t ALIGN_PROBS_SMEM_MAX = 64 * 1024;
+size_t align_probs_smem(int hd);   // dynamic shared memory of align_probs_kernel; refused above ALIGN_PROBS_SMEM_MAX
 void launch_align_probs(const AlignProbArgs& a, int B, int maxN, cudaStream_t st);
 void launch_align_fold(const AlignFoldArgs& a, int B, int maxT, int maxNT, cudaStream_t st);
 size_t align_dtw_smem(int N, int T, bool trace_in_smem);

@@ -72,6 +72,22 @@ GemmA plan_operand(int M, int K, int a_mode, int OH, int OW, int cpad, size_t pl
 }
 size_t round8(size_t n) { return (n + 7) / 8 * 8; }
 
+void write_score_plan(const ScoreHeadPlan& p, int* out) {
+    const int items = p.tiles_m * p.nslices;
+    int lo = p.tiles_n, hi = 0;
+    for (int s = 0; s < p.nslices; ++s) {   // slice s covers tiles [s * tiles_n / nslices, (s + 1) * tiles_n / nslices)
+        const int w = (int)((long long)(s + 1) * p.tiles_n / p.nslices - (long long)s * p.tiles_n / p.nslices);
+        lo = std::min(lo, w); hi = std::max(hi, w);
+    }
+    out[0] = p.tiles_m; out[1] = p.tiles_n; out[2] = p.nslices; out[3] = p.grid;
+    out[4] = (items + p.grid - 1) / p.grid; out[5] = lo; out[6] = hi;
+}
+
+void check_score_dims(int rows, int V, int H, int grid_cap) {
+    ASRB_REQUIRE(rows >= 1 && V >= 1 && H > 0 && H % 64 == 0 && grid_cap >= 0, ASRB_ERR_INVALID,
+                 "asrbt_score: rows >= 1, V >= 1, H % 64 == 0 and grid_cap >= 0");
+}
+
 }  // namespace
 }  // namespace asrb
 
@@ -242,6 +258,110 @@ int asrbt_dtw(const float* M, int N, int T, int32_t* start_tok_out) {
         a.start = d_start;
         launch_align_dtw(a, 1, smem, s.st);
         s.download(start_tok_out, d_start, (size_t)N);
+        s.sync();
+    });
+}
+
+int asrbt_score_plan(int rows, int V, int H, int sms, int grid_cap, int* plan_out) {
+    return run_guarded([&] {
+        ASRB_REQUIRE(plan_out && sms > 0, ASRB_ERR_INVALID, "asrbt_score_plan: bad arguments");
+        check_score_dims(rows, V, H, grid_cap);
+        write_score_plan(plan_score_head(rows, V, sms, grid_cap), plan_out);
+    });
+}
+
+int asrbt_score_head(const asrbt_score_args* a, int* plan_out) {
+    return run_guarded([&] {
+        ASRB_REQUIRE(a && plan_out && a->hid && a->norm_w && a->lm_head && a->target && a->lp_out, ASRB_ERR_INVALID,
+                     "asrbt_score_head: bad arguments");
+        check_score_dims(a->rows, a->V, a->H, a->grid_cap);
+        ASRB_REQUIRE(a->nplanes >= 1 && a->nplanes <= 3 && (a->topk == 0 || a->topk == 1), ASRB_ERR_INVALID,
+                     "asrbt_score_head: nplanes is 1..3, topk 0 or 1");
+        ASRB_REQUIRE(!a->topk || (a->tk_ids_out && a->tk_lp_out), ASRB_ERR_INVALID, "asrbt_score_head: no top-k output");
+        ASRB_REQUIRE(a->src ? a->n_hid >= 1 : a->n_hid == a->rows, ASRB_ERR_INVALID, "asrbt_score_head: bad n_hid");
+        std::vector<int> src(a->rows);
+        for (int r = 0; r < a->rows; ++r) {
+            src[r] = a->src ? a->src[r] : r;
+            ASRB_REQUIRE(src[r] >= 0 && src[r] < a->n_hid, ASRB_ERR_INVALID, "asrbt_score_head: src out of range");
+            ASRB_REQUIRE(a->target[r] >= 0 && a->target[r] < a->V, ASRB_ERR_INVALID, "asrbt_score_head: target out of range");
+        }
+        Scope s;
+        const int rows = a->rows, H = a->H, V = a->V;
+        const float* d_hid = s.upload(a->hid, (size_t)a->n_hid * H);
+        const int* d_src = s.upload(src.data(), (size_t)rows);
+        const int* d_tgt = s.upload(a->target, (size_t)rows);
+        const float* d_w = s.upload(a->norm_w, (size_t)H);
+        const bf16* d_head = reinterpret_cast<const bf16*>(s.upload(a->lm_head, (size_t)V * H));
+        const size_t plane_stride = round8((size_t)rows * H);
+        float* d_gathered = s.alloc<float>((size_t)rows * H);
+        bf16* d_planes = s.alloc<bf16>(3 * plane_stride);
+        const ScoreHeadPlan p = plan_score_head(rows, V, device_sms(), a->grid_cap);
+        ScorePart* d_part = s.alloc<ScorePart>((size_t)rows * p.nslices, 0xff);   // NaN: a partial never written
+        float* d_lp = s.alloc<float>((size_t)rows, 0xff);
+        int* d_tki = a->topk ? s.alloc<int>((size_t)rows * TK_MAX, 0xff) : nullptr;
+        float* d_tkl = a->topk ? s.alloc<float>((size_t)rows * TK_MAX, 0xff) : nullptr;
+        launch_score_head(d_head, d_w, H, V, a->eps, device_sms(), a->grid_cap, d_hid, d_src, d_tgt, rows, d_gathered,
+                          d_planes, plane_stride, a->nplanes, d_part, a->topk != 0, d_lp, d_tki, d_tkl, s.st, nullptr);
+        write_score_plan(p, plan_out);
+        s.download(a->lp_out, d_lp, (size_t)rows);
+        if (a->topk) {
+            s.download(a->tk_ids_out, d_tki, (size_t)rows * TK_MAX);
+            s.download(a->tk_lp_out, d_tkl, (size_t)rows * TK_MAX);
+        }
+        s.sync();
+    });
+}
+
+int asrbt_align(const asrbt_align_args* a) {
+    return run_guarded([&] {
+        ASRB_REQUIRE(a && a->heads && a->qrow0 && a->N && a->T && a->a0 && a->slot && a->q && a->k && a->P_out &&
+                         a->Z_out && a->M_out, ASRB_ERR_INVALID, "asrbt_align: bad arguments");
+        ASRB_REQUIRE(a->B >= 1 && a->hd >= 1 && a->group >= 1 && a->nheads >= 1 && a->count >= 0 && a->ldq >= 1 &&
+                         a->q_rows >= 1 && a->k_elems >= 1 && a->seg_stride >= 0 && a->head_stride >= 0,
+                     ASRB_ERR_INVALID, "asrbt_align: bad dims");
+        ASRB_REQUIRE(align_probs_smem(a->hd) <= ALIGN_PROBS_SMEM_MAX, ASRB_ERR_INVALID, "asrbt_align: head_dim too large");
+        int maxG = 0;
+        for (int i = 0; i < a->nheads; ++i) {
+            ASRB_REQUIRE(a->heads[i] >= 0 && (int64_t)(a->heads[i] + 1) * a->hd <= a->ldq, ASRB_ERR_INVALID,
+                         "asrbt_align: head outside the q row");
+            maxG = std::max(maxG, a->heads[i] / a->group);
+        }
+        std::vector<long long> moff(a->B);
+        long long total = 0;
+        int maxN = 0, maxT = 0, maxNT = 0;
+        for (int b = 0; b < a->B; ++b) {
+            const int N = a->N[b], T = a->T[b];
+            ASRB_REQUIRE(N >= 1 && T >= 1 && (int64_t)N * T <= INT32_MAX && a->qrow0[b] >= 0 && a->a0[b] >= 0 && a->slot[b] >= 0,
+                         ASRB_ERR_INVALID, "asrbt_align: bad utterance");
+            ASRB_REQUIRE((int64_t)a->qrow0[b] + N <= a->q_rows, ASRB_ERR_INVALID, "asrbt_align: q rows out of range");
+            ASRB_REQUIRE(a->slot[b] * a->seg_stride + (int64_t)maxG * a->head_stride + ((int64_t)a->a0[b] + T) * a->hd <= a->k_elems,
+                         ASRB_ERR_INVALID, "asrbt_align: keys out of range");
+            moff[b] = total; total += (long long)N * T;
+            maxN = std::max(maxN, N); maxT = std::max(maxT, T); maxNT = std::max(maxNT, N * T);
+        }
+        Scope s;
+        const size_t plane = (size_t)total, nP = (size_t)a->nheads * plane;
+        std::vector<int> ints;
+        for (const int* v : {a->qrow0, a->N, a->T, a->a0, a->slot}) ints.insert(ints.end(), v, v + a->B);
+        ints.insert(ints.end(), a->heads, a->heads + a->nheads);
+        const int* d_int = s.upload(ints.data(), ints.size());
+        const long long* d_moff = s.upload(moff.data(), moff.size());
+        AlignProbArgs pa{};
+        pa.q = s.upload(a->q, (size_t)a->q_rows * a->ldq); pa.ldq = a->ldq;
+        pa.k = s.upload(a->k, (size_t)a->k_elems); pa.seg_stride = (size_t)a->seg_stride; pa.head_stride = (size_t)a->head_stride;
+        pa.hd = a->hd; pa.group = a->group;
+        pa.qrow0 = d_int; pa.N = d_int + a->B; pa.T = d_int + 2 * a->B; pa.a0 = d_int + 3 * a->B; pa.slot = d_int + 4 * a->B;
+        pa.moff = d_moff; pa.heads = d_int + 5 * a->B; pa.nheads = a->nheads;
+        pa.P = s.alloc<float>(nP, 0xff); pa.plane = plane;                  // NaN: an element never written
+        float* d_M = a->M_in ? s.upload(a->M_in, plane) : s.alloc<float>(plane);
+        launch_align_probs(pa, a->B, maxN, s.st);
+        s.download(a->P_out, pa.P, nP);
+        AlignFoldArgs fa{};
+        fa.N = pa.N; fa.T = pa.T; fa.moff = d_moff; fa.P = pa.P; fa.plane = plane; fa.nheads = a->nheads; fa.M = d_M;
+        fa.count = a->count;
+        launch_align_fold(fa, a->B, maxT, maxNT, s.st);
+        s.download(a->Z_out, pa.P, nP);
+        s.download(a->M_out, d_M, plane);
         s.sync();
     });
 }

@@ -4,9 +4,9 @@
 //   gather + final RMSNorm -> split3 planes -> wgmma GEMM against lm_head with a folding epilogue -> per-row merge
 //
 // The GEMM is gemm_tc.cu's (TMA ring of 3 stages, warpgroup 0 the producer, warpgroups 1-2 the wgmma consumers, CH
-// k-blocks per tensor-core accumulation, three planes), but its work item is (M tile, column slice): a CTA walks the
-// contiguous N tiles of one slice for one M tile and folds each finished 128 x 128 logit tile into per-row running
-// state held in registers.  Lane l of a consumer warp owns row l & 15 of the warp's 16 rows and 16 of every 32
+// k-blocks per tensor-core accumulation -- 1 here, 4 there -- three planes), but its work item is (M tile, column
+// slice): a CTA walks the contiguous N tiles of one slice for one M tile and folds each finished 128 x 128 logit tile
+// into per-row running state held in registers.  Lane l of a consumer warp owns row l & 15 of the warp's 16 rows and 16 of every 32
 // columns; the two lanes of a row merge at the end of the slice and write one partial (max m, sum of exp(l - m), the
 // target's logit when it lies in the slice, and with TOPK the slice's 8 best (logit, id)).  At most SCORE_SLICES
 // slices per row, so the workspace is rows x 64 partials whatever the vocabulary.  Columns >= vocab (the zero-filled
@@ -27,7 +27,10 @@ static constexpr int STAGE_BYTES = 3 * TILE_A_BYTES + TILE_B_BYTES;
 static constexpr int NTHREADS = 384;
 static constexpr int CONS_WARPS = 8;
 static constexpr int SLAB_LD = 40;
-static constexpr int CH = 4;
+// one k-block (3 planes x 4 k16 steps) per tensor-core accumulation, then a round-to-nearest add into the fp32 sums.
+// The tensor core truncates its running sum at every k16 step; gemm_tc.cu's 4-block chunks (48 truncations) put a
+// peaked row's log-probabilities (every product of the winning logit one sign) at up to 12 x the fp32 error
+static constexpr int CH = 1;
 
 template <bool TOPK>
 __global__ void __launch_bounds__(NTHREADS, 1)
@@ -188,22 +191,28 @@ void check_score_head(const Model& m) {
                  "score: the wgmma score head needs hidden_size % 64 == 0, got " + std::to_string(c.hidden_size));
 }
 
-int score_slices(const Model& m) {
-    const int tiles_n = (m.d.c.vocab_size + score::BN - 1) / score::BN;
-    return std::min(SCORE_SLICES, tiles_n);
+ScoreHeadPlan plan_score_head(int rows, int V, int sms, int grid_cap) {
+    using namespace score;
+    ScoreHeadPlan p;
+    p.tiles_m = (rows + BM - 1) / BM; p.tiles_n = (V + BN - 1) / BN;
+    p.nslices = std::min(SCORE_SLICES, p.tiles_n);
+    p.grid = std::min(p.tiles_m * p.nslices, sms);
+    if (grid_cap > 0) p.grid = std::min(p.grid, grid_cap);
+    return p;
 }
 
-void launch_score_head(const Model& m, const float* hid, const int* d_src, const int* d_target, int rows, float* gathered,
-                       bf16* planes, size_t plane_stride, int nplanes, ScorePart* part, bool topk, float* lp_out,
-                       int* tk_ids, float* tk_lp, cudaStream_t st, int64_t* launches) {
+int score_slices(const Model& m) { return plan_score_head(1, m.d.c.vocab_size, 1, 0).nslices; }
+
+void launch_score_head(const bf16* lm_head, const float* final_norm, int H, int V, float eps, int sms, int grid_cap,
+                       const float* hid, const int* d_src, const int* d_target, int rows, float* gathered, bf16* planes,
+                       size_t plane_stride, int nplanes, ScorePart* part, bool topk, float* lp_out, int* tk_ids,
+                       float* tk_lp, cudaStream_t st, int64_t* launches) {
     using namespace score;
-    check_score_head(m);
-    const asrb_dims& c = m.d.c;
-    const int H = c.hidden_size, V = c.vocab_size;
+    ASRB_REQUIRE(H > 0 && H % BK == 0 && V >= 1 && sms >= 1 && grid_cap >= 0, ASRB_ERR_INVALID, "score: bad head dims");
     ASRB_REQUIRE(rows >= 1 && nplanes >= 1 && nplanes <= 3, ASRB_ERR_INVALID, "score: bad head shape");
     gather_rows_kernel<<<rows, 128, 0, st>>>(hid, d_src, H, gathered);
     ASRB_CUDA_CHECK(cudaGetLastError());
-    launch_rmsnorm_s3(gathered, m.final_norm, rows, H, (float)c.rms_norm_eps, planes, plane_stride, st);
+    launch_rmsnorm_s3(gathered, final_norm, rows, H, eps, planes, plane_stride, st);
     cuuint64_t ad[3] = {(cuuint64_t)H, (cuuint64_t)rows, 3};
     cuuint64_t as[2] = {(cuuint64_t)H * 2, (cuuint64_t)plane_stride * 2};
     cuuint32_t ab[3] = {(cuuint32_t)BK, (cuuint32_t)BM, 1};
@@ -211,9 +220,9 @@ void launch_score_head(const Model& m, const float* hid, const int* d_src, const
     cuuint64_t bd[2] = {(cuuint64_t)H, (cuuint64_t)V};
     cuuint64_t bs[1] = {(cuuint64_t)H * 2};
     cuuint32_t bb[2] = {(cuuint32_t)BK, (cuuint32_t)BN};
-    const CUtensorMap mapB = tc_cached_map(m.lm_head, 2, bd, bs, bb);
-    const int tiles_m = (rows + BM - 1) / BM, tiles_n = (V + BN - 1) / BN, nslices = score_slices(m);
-    const int grid = std::min(tiles_m * nslices, m.ctx->sm_count);
+    const CUtensorMap mapB = tc_cached_map(lm_head, 2, bd, bs, bb);
+    const ScoreHeadPlan p = plan_score_head(rows, V, sms, grid_cap);
+    const int tiles_m = p.tiles_m, tiles_n = p.tiles_n, nslices = p.nslices, grid = p.grid;
     const size_t smem = smem_bytes();
     if (topk) {
         ASRB_CUDA_CHECK(cudaFuncSetAttribute(score_head_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -228,6 +237,16 @@ void launch_score_head(const Model& m, const float* hid, const int* d_src, const
     }
     ASRB_CUDA_CHECK(cudaGetLastError());
     if (launches) *launches += 4;
+}
+
+void launch_score_head(const Model& m, const float* hid, const int* d_src, const int* d_target, int rows, float* gathered,
+                       bf16* planes, size_t plane_stride, int nplanes, ScorePart* part, bool topk, float* lp_out,
+                       int* tk_ids, float* tk_lp, cudaStream_t st, int64_t* launches) {
+    check_score_head(m);
+    const asrb_dims& c = m.d.c;
+    launch_score_head(m.lm_head, m.final_norm, c.hidden_size, c.vocab_size, (float)c.rms_norm_eps, m.ctx->sm_count, 0, hid,
+                      d_src, d_target, rows, gathered, planes, plane_stride, nplanes, part, topk, lp_out, tk_ids, tk_lp, st,
+                      launches);
 }
 
 }  // namespace asrb
