@@ -26,6 +26,12 @@ void ingest_pcm(IngestState* st, cudaStream_t stream, const void* const* pcm, co
 static const int kPromptHead[9] = {151644, 8948, 198, 151645, 198, 151644, 872, 198, 151669};
 static const int kPromptTail[6] = {151670, 151645, 198, 151644, 77091, 198};
 static const int kAudioPad = 151676;
+// the prompt's layout (build_prompt): 3 head ids, the context, 6 more head ids, the audio pads, the tail, the language
+// ids, the forced ids
+static int audio_start(int ctx) { return 3 + ctx + 6; }
+static int prompt_len(int ctx, int T, int nl, int nforced) { return audio_start(ctx) + T + 6 + nl + nforced; }
+// audio tokens of a chunk of `frames` mel frames: three stride-2 convolutions (feat_extract_output_length)
+static int chunk_tokens(int frames) { return conv_out_len(conv_out_len(conv_out_len(frames))); }
 
 struct Session {
     Model* m = nullptr;
@@ -42,10 +48,10 @@ struct Session {
     int stage = 0;         // 0 idle, 1 mel, 2 encoded, 3 prefilled
     int B = 0;
     std::vector<int64_t> n, npad, F, foff, soff;
-    std::vector<int> C, T, toff, S, srow0;
-    int totF = 0, totC = 0, totT = 0, totS = 0, maxlenS = 0, maxwin = 0, nwin = 0;
-    // ---- device buffers ----
-    std::vector<void*> owned;
+    std::vector<int> C, T, toff, S;
+    int totF = 0, totC = 0, totT = 0, maxlenS = 0, maxwin = 0, nwin = 0;
+    // ---- buffers: device (cudaMalloc) and pinned host (cudaMallocHost) memory, freed with the session ----
+    std::vector<void*> owned, owned_host;
     float *h_samples = nullptr, *d_samples = nullptr, *d_mel = nullptr;
     int64_t* d_i64 = nullptr;      // soff | n | npad | foff | frames  (5 * max_batch)
     int64_t* h_i64 = nullptr;
@@ -156,22 +162,10 @@ struct Session {
 };
 
 Session::~Session() {
-    if (d_long) cudaFree(d_long);
-    if (d_seg_blk) cudaFree(d_seg_blk);
-    if (d_seg_i64) cudaFree(d_seg_i64);
     if (step_graph) cudaGraphExecDestroy(step_graph);
     for (auto& e : ev) if (e) cudaEventDestroy(e);
     for (void* p : owned) cudaFree(p);
-    if (h_samples) cudaFreeHost(h_samples);
-    if (h_i64) cudaFreeHost(h_i64);
-    if (h_int) cudaFreeHost(h_int);
-    if (h_done) cudaFreeHost(h_done);
-    if (h_ids) cudaFreeHost(h_ids);
-    if (h_nout) cudaFreeHost(h_nout);
-    if (h_next) cudaFreeHost(h_next);
-    if (sc.h_int) cudaFreeHost(sc.h_int);
-    if (h_str_stats) cudaFreeHost(h_str_stats);
-    if (h_str_int) cudaFreeHost(h_str_int);
+    for (void* p : owned_host) cudaFreeHost(p);
     if (ingest) ingest_state_free(ingest);
     if (st) cudaStreamDestroy(st);
 }
@@ -182,6 +176,22 @@ template <typename T> static T* salloc(Session* s, size_t n, bool zero = false) 
     s->owned.push_back(p);
     if (zero) ASRB_CUDA_CHECK(cudaMemset(p, 0, std::max<size_t>(n, 1) * sizeof(T)));
     return p;
+}
+template <typename T> static T* halloc(Session* s, size_t n) {     // pinned host memory
+    T* p = nullptr;
+    ASRB_CUDA_CHECK(cudaMallocHost(&p, std::max<size_t>(n, 1) * sizeof(T)));
+    s->owned_host.push_back(p);
+    return p;
+}
+// frees a buffer of the session's (device or pinned host); null or not the session's: nothing
+static void release_owned(Session* s, void* p) {
+    for (auto* list : {&s->owned, &s->owned_host}) {
+        auto it = std::find(list->begin(), list->end(), p);
+        if (it == list->end()) continue;
+        if (list == &s->owned) cudaFree(p); else cudaFreeHost(p);
+        list->erase(it);
+        return;
+    }
 }
 
 Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_lang, int max_context, int max_new) {
@@ -201,7 +211,7 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
         s->maxF = (int)(s->max_npad / 160);
         s->maxC = (s->maxF + d.chunk_frames - 1) / d.chunk_frames;
         s->maxT = s->maxC * d.tok_per_chunk;
-        s->maxS = s->maxT + 15 + max_lang + max_context;
+        s->maxS = prompt_len(max_context, s->maxT, max_lang, 0);
         s->max_ctx = s->maxS + max_new;
         ASRB_REQUIRE(s->max_ctx <= m->rope_max_pos, ASRB_ERR_INVALID, "context exceeds RoPE table");
         // the per-phase decode step (asrb_decode_step with logits, any model or context the fused steps decline) holds a
@@ -214,16 +224,16 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
         ASRB_CUDA_CHECK(cudaStreamCreateWithFlags(&s->st, cudaStreamNonBlocking));
         for (auto& e : s->ev) ASRB_CUDA_CHECK(cudaEventCreate(&e));
         const size_t Bm = max_batch;
-        ASRB_CUDA_CHECK(cudaMallocHost(&s->h_samples, Bm * s->max_npad * sizeof(float)));
+        s->h_samples = halloc<float>(s, Bm * s->max_npad);
         s->d_samples = salloc<float>(s, Bm * s->max_npad);
         s->d_mel = salloc<float>(s, Bm * c.num_mel_bins * s->maxF);
-        ASRB_CUDA_CHECK(cudaMallocHost(&s->h_i64, 5 * Bm * sizeof(int64_t)));
+        s->h_i64 = halloc<int64_t>(s, 5 * Bm);
         s->d_i64 = salloc<int64_t>(s, 5 * Bm);
         s->d_maxkey = salloc<int>(s, Bm);
         const size_t totC = Bm * s->maxC, totT = Bm * s->maxT, totS = Bm * s->maxS;
         s->enc_int_cap = 2 * totC + totC * d.tok_per_chunk + 2 * (totC + Bm) + 16;
-        s->int_cap = s->enc_int_cap + 4 * totS + 16 * Bm + 16;   // rows, then per-utterance plan and fan-out arrays
-        ASRB_CUDA_CHECK(cudaMallocHost(&s->h_int, s->int_cap * sizeof(int)));
+        s->int_cap = s->enc_int_cap + 4 * totS + 10 * Bm;   // rows, per-sequence plan and fan-out, lastrow | pos0 | done0
+        s->h_int = halloc<int>(s, s->int_cap);
         s->d_int = salloc<int>(s, s->int_cap);
         // encoder activations
         s->act1_ps = totC * 4 * d.conv_h[2] * d.conv_w[2] * d.cpad;
@@ -305,10 +315,8 @@ Session* session_create(Model* m, int max_batch, int64_t max_samples, int max_la
         }
         s->mega.hq_stats = salloc<unsigned long long>(s, 4, true);
         if (getenv("ASRB_MEGA_DEBUG")) s->mega.dbg = salloc<long long>(s, decode_mega_dbg_slots(), true);
-        ASRB_CUDA_CHECK(cudaMallocHost(&s->h_done, Bm * sizeof(int)));
-        ASRB_CUDA_CHECK(cudaMallocHost(&s->h_nout, Bm * sizeof(int)));
-        ASRB_CUDA_CHECK(cudaMallocHost(&s->h_next, Bm * sizeof(int)));
-        ASRB_CUDA_CHECK(cudaMallocHost(&s->h_ids, Bm * max_new * sizeof(int)));
+        s->h_done = halloc<int>(s, Bm); s->h_nout = halloc<int>(s, Bm); s->h_next = halloc<int>(s, Bm);
+        s->h_ids = halloc<int>(s, Bm * max_new);
         ASRB_CUDA_CHECK(cudaDeviceSynchronize());
     } catch (...) { delete s; throw; }
     return s;
@@ -382,12 +390,13 @@ void session_ingested_read(Session* s, int b, float* out) {
     ASRB_CUDA_CHECK(cudaMemcpy(out, s->d_samples + so, (size_t)s->ingested_n[b] * sizeof(float), cudaMemcpyDeviceToHost));
 }
 
-// (re)allocate a session scratch buffer that is not in `owned` to at least `bytes`; its contents are not kept
+// (re)allocate a session scratch buffer to at least `n` elements; its contents are not kept.  The old buffer is freed
+// first: the long-audio buffer can take hundreds of MB
 template <typename T> static void grow(Session* s, T** p, size_t* cap, size_t n) {
     if (n <= *cap && *p) return;
     ASRB_CUDA_CHECK(cudaStreamSynchronize(s->st));      // the old buffer may still be read
-    if (*p) { cudaFree(*p); *p = nullptr; *cap = 0; }
-    ASRB_CUDA_CHECK(cudaMalloc(p, std::max<size_t>(n, 1) * sizeof(T)));
+    release_owned(s, *p); *p = nullptr; *cap = 0;
+    *p = salloc<T>(s, n);
     *cap = n;
 }
 
@@ -492,7 +501,7 @@ void session_encode(Session* s, int64_t* n_tokens_out) {
         for (int k = 0; k < s->C[b]; ++k, ++ci) {
             chunk_clip[ci] = b; chunk_f0[ci] = k * cf;
             int frames = (int)std::min<int64_t>(cf, s->F[b] - (int64_t)k * cf);
-            int valid = conv_out_len(conv_out_len(conv_out_len(frames)));                // feat_extract_output_length
+            int valid = chunk_tokens(frames);
             for (int t = 0; t < tpc; ++t) rowmap[(size_t)ci * tpc + t] = t < valid ? totT + t : -1;
             totT += valid; wtok += valid;
             bool close = d.chunks_per_window > 0 && ((k + 1) % d.chunks_per_window == 0);
@@ -668,6 +677,17 @@ void session_last_prefill_stats(Session* s, int64_t* out, int n) {
     for (int i = 0; i < n && i < 3; ++i) out[i] = v[i];
 }
 
+// language ids of utterance b: their count (0 when none are given), checked against the session's max_lang less
+// `reserved` (a stream's forced prefix) and against the vocabulary
+static int lang_count(const Session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, int b, int reserved = 0,
+                      const char* over = "language prompt exceeds session capacity") {
+    const int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
+    ASRB_REQUIRE(nl >= 0 && nl + reserved <= s->max_lang, ASRB_ERR_INVALID, over);
+    for (int i = 0; i < nl; ++i)
+        ASRB_REQUIRE(lang_ids[b][i] >= 0 && lang_ids[b][i] < s->m->d.c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
+    return nl;
+}
+
 // a whole prompt, position by position: ids, and the audio row of each audio position (-1 elsewhere).  Head, context,
 // end of the system turn and start of the user turn, T audio pads reading rows arow0 .. arow0 + T - 1, the tail, the nl
 // language ids, then the forced prefix of a stream
@@ -682,18 +702,70 @@ static void build_prompt(const std::vector<int>& ctx, int T, int arow0, const in
     for (int i = 0; i < nl; ++i) { pid.push_back((int)lang[i]); parow.push_back(-1); }
     for (int id : forced) { pid.push_back(id); parow.push_back(-1); }
 }
-// utterance b's prompt of the current offline batch (s->S[b] positions)
-static void build_prompt(const Session* s, int b, const int64_t* const* lang_ids, std::vector<int>& pid, std::vector<int>& parow) {
-    const std::vector<int>& cb = context_of(s, b);
-    const int nl = s->S[b] - (15 + (int)cb.size() + s->T[b]);
-    build_prompt(cb, s->T[b], s->toff[b], nl > 0 ? lang_ids[b] : nullptr, nl, {}, pid, parow);
+// utterance b's prompt of the current offline batch, with its nl language ids
+static void build_prompt(const Session* s, int b, const int64_t* const* lang_ids, int nl, std::vector<int>& pid, std::vector<int>& parow) {
+    build_prompt(context_of(s, b), s->T[b], s->toff[b], nl > 0 ? lang_ids[b] : nullptr, nl, {}, pid, parow);
 }
-// positions [from, |pid|) of a prompt into the row plan from row r0, as rows of sequence (KV slot) q; returns the next row
-static int plan_prompt_rows(const std::vector<int>& pid, const std::vector<int>& parow, int from, int r0, int q, int* ids,
-                            int* arow, int* rseq, int* rpos) {
-    int r = r0;
-    for (int i = from; i < (int)pid.size(); ++i, ++r) { ids[r] = pid[i]; arow[r] = parow[i]; rseq[r] = q; rpos[r] = i; }
-    return r;
+
+// one sequence (KV slot) of a prefill: all its positions (ids, and audio rows as build_prompt gives them), the first one
+// it computes, and the slot whose K/V holds positions [0, from): an earlier slot, a leader that fans them out to this
+// follower as it computes them; this slot itself, which kept them from an earlier call; or none (-1, from = 0)
+struct PrefillSeq {
+    std::vector<int> pid, parow;
+    int from = 0, lead = -1;
+};
+struct PrefillPlan {
+    int totS = 0, nseq = 0, maxrows = 0;      // rows, sequences, most rows of one sequence
+    std::vector<int> srow0;                   // first row of each sequence
+    bool fan = false; FanOut fan_plan{};      // fan: some sequence follows a leader
+    const int* d_qpos0 = nullptr;             // first computed position per sequence; null: no sequence has a lead
+    const int* d_tail = nullptr;              // the caller's ints behind the plan
+};
+// the row plan of a prefill, sequence-major, in the int region (hi, di) of `cap` ints: ids | arow | rseq | rpos per row,
+// sq0 | slen | qpos0 | fan_n | fan_off | fan_P per sequence, the follower slots grouped by leader, then `extra` ints of
+// the caller's that fill_tail(tail, plan) writes.  Uploads it, points the session's row arrays at it and records the
+// prefill stats
+template <typename FillTail>
+static PrefillPlan plan_prefill(Session* s, const std::vector<PrefillSeq>& seq, int* hi, int* di, size_t cap, int extra,
+                                FillTail fill_tail) {
+    const asrb_dims& c = s->m->d.c;
+    PrefillPlan p;
+    const int N = (int)seq.size();
+    p.nseq = N; p.srow0.assign(N, 0);
+    int nf = 0; int64_t shared = 0; bool led = false;
+    for (int q = 0; q < N; ++q) {
+        const int rows = (int)seq[q].pid.size() - seq[q].from;
+        p.srow0[q] = p.totS; p.totS += rows; p.maxrows = std::max(p.maxrows, rows);
+        led = led || seq[q].lead >= 0;
+        if (seq[q].lead >= 0 && seq[q].lead != q) { ++nf; shared += seq[q].from; }
+    }
+    const int totS = p.totS;
+    const size_t nint = 4 * (size_t)totS + 6 * (size_t)N + std::max(nf, 1) + extra;
+    ASRB_REQUIRE(nint <= cap, ASRB_ERR_INVALID, "plan exceeds session capacity");
+    int* ids = hi; int* arow = ids + totS; int* rseq = arow + totS; int* rpos = rseq + totS;
+    int* sq0 = rpos + totS; int* slen = sq0 + N; int* qpos0 = slen + N;
+    int* fan_n = qpos0 + N; int* fan_off = fan_n + N; int* fan_P = fan_off + N; int* fan_slots = fan_P + N;
+    int* tail = fan_slots + std::max(nf, 1);
+    for (int q = 0, r = 0, f = 0; q < N; ++q) {
+        const PrefillSeq& x = seq[q];
+        // position = index in the prompt (build_position_ids, inference.rs:259-266)
+        for (int i = x.from; i < (int)x.pid.size(); ++i, ++r) { ids[r] = x.pid[i]; arow[r] = x.parow[i]; rseq[r] = q; rpos[r] = i; }
+        sq0[q] = p.srow0[q]; slen[q] = (int)x.pid.size() - x.from; qpos0[q] = x.from;
+        fan_off[q] = f; fan_n[q] = 0; fan_P[q] = 0;
+        for (int b = q + 1; b < N; ++b)
+            if (seq[b].lead == q) { fan_slots[f++] = b; ++fan_n[q]; fan_P[q] = seq[b].from; }
+    }
+    fill_tail(tail, p);
+    s->pf_rows = totS; s->pf_shared_rows = shared;
+    s->pf_fan_bytes = shared * 2LL * c.num_hidden_layers * c.num_key_value_heads * c.head_dim * (int64_t)sizeof(float);
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(di, hi, nint * sizeof(int), cudaMemcpyHostToDevice, s->st));
+    s->d_ids = di; s->d_audio_row = di + (arow - hi); s->d_row_seq = di + (rseq - hi);
+    s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
+    p.fan = nf > 0;
+    p.fan_plan = FanOut{di + (fan_n - hi), di + (fan_off - hi), di + (fan_P - hi), di + (fan_slots - hi)};
+    p.d_qpos0 = led ? di + (qpos0 - hi) : nullptr;   // none: the kernels of a call without contexts
+    p.d_tail = di + (tail - hi);
+    return p;
 }
 
 // an alignment call's work inside the prefill: run(l) after layer l's q / k normalisation and RoPE, while s->qrot
@@ -703,13 +775,14 @@ struct LayerHook {
     virtual ~LayerHook() = default;
 };
 
-// embed + inject and the decoder layers over the planned rows (s->d_ids ..., totS rows; sequence q's rows are its
-// segment of the attention, in KV slot q); audio rows are read from `audio`.  n_layers < 0: every layer; else the
-// layers 0 .. n_layers - 1, the last of them stopping after `hook` (an alignment call, which needs no later work)
-static void prefill_layers(Session* s, int totS, int nseq, int maxrows, const FanOut* fan, const int* d_qpos0,
-                           const float* audio, int n_layers = -1, LayerHook* hook = nullptr) {
+// embed + inject and the decoder layers over the rows of plan `pf` (sequence q's rows are its segment of the attention,
+// in KV slot q); audio rows are read from `audio`.  n_layers < 0: every layer; else the layers 0 .. n_layers - 1, the
+// last of them stopping after `hook` (an alignment call, which needs no later work)
+static void prefill_layers(Session* s, const PrefillPlan& pf, const float* audio, int n_layers = -1, LayerHook* hook = nullptr) {
     Model& m = *s->m; const Dims& d = m.d; const asrb_dims& c = d.c;
     cudaStream_t st = s->st; const int np = s->nplanes;
+    const int totS = pf.totS;
+    const FanOut* fan = pf.fan ? &pf.fan_plan : nullptr;
     launch_embed_inject(m.embed, c.hidden_size, s->d_ids, s->d_audio_row, audio, totS, s->hid, st);
     s->launches += 1;
     const int H = c.hidden_size; const float eps = (float)c.rms_norm_eps;
@@ -731,8 +804,8 @@ static void prefill_layers(Session* s, int totS, int nseq, int maxrows, const Fa
         }
         { AttnParams p{}; p.q = s->qrot; p.ldq = d.q_dim; p.k = kc; p.v = vc; p.seg_stride = s->cache_seq_stride;
           p.head_stride = (size_t)s->max_ctx * c.head_dim; p.ldk = c.head_dim; p.keys_in_rows = 0;
-          p.seg_q0 = s->d_seq_q0; p.seg_len = s->d_seq_len; p.nseg = nseq; p.nheads = c.num_attention_heads;
-          p.group = c.num_attention_heads / c.num_key_value_heads; p.causal = 1; p.max_len = maxrows; p.seg_pos0 = d_qpos0;
+          p.seg_q0 = s->d_seq_q0; p.seg_len = s->d_seq_len; p.nseg = pf.nseq; p.nheads = c.num_attention_heads;
+          p.group = c.num_attention_heads / c.num_key_value_heads; p.causal = 1; p.max_len = pf.maxrows; p.seg_pos0 = pf.d_qpos0;
           p.out_s3 = s->dattn; p.plane_stride = s->dattn_ps; p.ldo = d.q_dim;
           launch_attention(p, c.head_dim, st); }
         { GemmA A = plainA(s->dattn, s->dattn_ps, totS, d.q_dim, np);
@@ -749,7 +822,7 @@ static void prefill_layers(Session* s, int totS, int nseq, int maxrows, const Fa
     }
 }
 
-static void begin_run(Session* s, int B, const int* d_done0);
+static void begin_run(Session* s, int B, const int* d_start);
 static void first_token(Session* s, int B, bool write_logits, const int* pos0);
 
 void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* n_lang_ids, int64_t* seq_lens_out,
@@ -760,69 +833,31 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     check_context(s, s->B);
     Model& m = *s->m; const asrb_dims& c = m.d.c;
     const int B = s->B; cudaStream_t st = s->st;
-    for (int b = 0; b < B; ++b) {
-        int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
-        ASRB_REQUIRE(nl >= 0 && nl <= s->max_lang, ASRB_ERR_INVALID, "language prompt exceeds session capacity");
-        for (int i = 0; i < nl; ++i)
-            ASRB_REQUIRE(lang_ids[b][i] >= 0 && lang_ids[b][i] < c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
-    }
+    std::vector<int> nl((size_t)B);
+    for (int b = 0; b < B; ++b) nl[b] = lang_count(s, lang_ids, n_lang_ids, b);
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
     s->run_k = s->beam_k; s->run_alpha = s->length_penalty; s->nslots = B * s->run_k; s->nbest_valid = false;
     if (s->run_k > 1) { ensure_beam_bufs(s); s->beam_steps = 0; }
-    // shared contexts: an utterance whose non-empty context equals that of an earlier leader follows it; its first
-    // P = L + 9 positions (head, context, end of the system turn, user turn up to the audio start) are the leader's
-    std::vector<int> lead((size_t)B, -1), skip((size_t)B, 0);
-    bool fan = false;
+    // shared contexts: an utterance whose non-empty context equals that of an earlier leader follows it; its positions
+    // before the audio (head, context, end of the system turn, user turn up to the audio start) are the leader's
+    std::vector<PrefillSeq> seq((size_t)B);
+    s->S.assign(B, 0); s->maxlenS = 0;
     for (int b = 0; b < B; ++b) {
+        build_prompt(s, b, lang_ids, nl[b], seq[b].pid, seq[b].parow);
+        s->S[b] = (int)seq[b].pid.size(); s->maxlenS = std::max(s->maxlenS, s->S[b]);
         const std::vector<int>& cb = context_of(s, b);
         if (cb.empty()) continue;
         for (int a = 0; a < b; ++a)
-            if (lead[a] < 0 && context_of(s, a) == cb) { lead[b] = a; skip[b] = (int)cb.size() + 9; fan = true; break; }
+            if (seq[a].lead < 0 && context_of(s, a) == cb) { seq[b].lead = a; seq[b].from = audio_start((int)cb.size()); break; }
     }
-    s->S.assign(B, 0); s->srow0.assign(B, 0);
-    int totS = 0, maxlen = 0, maxrows = 0;     // totS: rows computed; maxlen: longest prompt; maxrows: most rows of one utterance
-    for (int b = 0; b < B; ++b) {
-        int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
-        const int L = (int)context_of(s, b).size();
-        s->srow0[b] = totS; s->S[b] = 9 + L + s->T[b] + 6 + nl; totS += s->S[b] - skip[b];
-        maxlen = std::max(maxlen, s->S[b]); maxrows = std::max(maxrows, s->S[b] - skip[b]);
-    }
-    s->totS = totS; s->maxlenS = maxlen;
-    int* hi = s->h_int + s->enc_int_cap;      // separate region: the encoder plan upload may still be in flight
-    int* di = s->d_int + s->enc_int_cap;
-    int* ids = hi; int* arow = ids + totS; int* rseq = arow + totS; int* rpos = rseq + totS;
-    int* sq0 = rpos + totS; int* slen = sq0 + B; int* lastrow = slen + B; int* pos0 = lastrow + B;
-    int* qpos0 = pos0 + B; int* fan_n = qpos0 + B; int* fan_off = fan_n + B; int* fan_P = fan_off + B; int* fan_slots = fan_P + B;
-    int64_t shared = 0;
-    std::vector<int> pid, parow;
-    for (int b = 0; b < B; ++b) {
-        build_prompt(s, b, lang_ids, pid, parow);
-        // rows from position skip[b] on (build_position_ids :259-266: position = index in the prompt)
-        plan_prompt_rows(pid, parow, skip[b], s->srow0[b], b, ids, arow, rseq, rpos);
-        const int rows = s->S[b] - skip[b];
-        sq0[b] = s->srow0[b]; slen[b] = rows; lastrow[b] = s->srow0[b] + rows - 1; pos0[b] = s->S[b] - 1; qpos0[b] = skip[b];
-        shared += skip[b];
-    }
-    int nf = 0;                                // followers grouped by leader, ascending
-    for (int a = 0; a < B; ++a) {
-        fan_off[a] = nf; fan_n[a] = 0; fan_P[a] = 0;
-        for (int b = a + 1; b < B; ++b)
-            if (lead[b] == a) { fan_slots[nf++] = b; ++fan_n[a]; fan_P[a] = skip[b]; }
-    }
-    const size_t nint = (size_t)(fan_slots + std::max(nf, 1) - hi);
-    ASRB_REQUIRE(s->enc_int_cap + nint <= s->int_cap, ASRB_ERR_INVALID, "plan exceeds session capacity");
-    s->pf_rows = totS; s->pf_shared_rows = shared;
-    s->pf_fan_bytes = shared * 2LL * c.num_hidden_layers * c.num_key_value_heads * c.head_dim * (int64_t)sizeof(float);
-    ASRB_CUDA_CHECK(cudaMemcpyAsync(di, hi, nint * sizeof(int), cudaMemcpyHostToDevice, st));
-    s->d_ids = di; s->d_audio_row = di + (arow - hi); s->d_row_seq = di + (rseq - hi);
-    s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
-    const FanOut fan_plan{di + (fan_n - hi), di + (fan_off - hi), di + (fan_P - hi), di + (fan_slots - hi)};
-    const int* d_qpos0 = fan ? di + (qpos0 - hi) : nullptr;   // no follower: the plan and kernels of a call without contexts
-    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_lastrow, di + (lastrow - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.pos, di + (pos0 - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    begin_run(s, B, nullptr);
-    prefill_layers(s, totS, B, maxrows, fan ? &fan_plan : nullptr, d_qpos0, s->audio);
-    first_token(s, B, last_logits != nullptr, di + (pos0 - hi));
+    // separate region: the encoder plan upload may still be in flight
+    const PrefillPlan pf = plan_prefill(s, seq, s->h_int + s->enc_int_cap, s->d_int + s->enc_int_cap, s->int_cap - s->enc_int_cap,
+                                        3 * B, [&](int* t, const PrefillPlan& p) {   // lastrow | pos0 | done0
+        for (int b = 0; b < B; ++b) { t[b] = p.srow0[b] + s->S[b] - seq[b].from - 1; t[B + b] = s->S[b] - 1; t[2 * B + b] = 0; }
+    });
+    begin_run(s, B, pf.d_tail);
+    prefill_layers(s, pf, s->audio);
+    first_token(s, B, last_logits != nullptr, pf.d_tail + B);
     if (seq_lens_out) for (int b = 0; b < B; ++b) seq_lens_out[b] = s->S[b];
     if (last_logits) {
         ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -831,12 +866,14 @@ void session_prefill(Session* s, const int64_t* const* lang_ids, const int32_t* 
     s->stage = 3;
 }
 
-// the result rows of the run's B sequences reset (done from d_done0 when given, else 0) and its record, sampling and
+// the run's B sequences started from the device ints lastrow | pos0 | done0 at d_start (each sequence's last prefill row,
+// its decode position and whether it is done from the start), its result rows reset and its record, sampling and
 // top-k options latched; before the prefill
-static void begin_run(Session* s, int B, const int* d_done0) {
+static void begin_run(Session* s, int B, const int* d_start) {
     cudaStream_t st = s->st;
-    if (d_done0) ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.done, d_done0, B * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    else ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.done, 0, B * sizeof(int), st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_lastrow, d_start, B * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.pos, d_start + B, B * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.done, d_start + 2 * B, B * sizeof(int), cudaMemcpyDeviceToDevice, st));
     ASRB_CUDA_CHECK(cudaMemsetAsync(s->db.n_out, 0, B * sizeof(int), st));
     s->lp_valid = s->opt_logprobs || s->top_k > 0;   // latched here: a run records log-probabilities only if it starts with the option on
     if (s->db.logprobs) {                  // all NaN (0xFFFFFFFF): no EOS seen, nothing appended
@@ -1045,6 +1082,25 @@ void session_generate(Session* s, int max_new_tokens, int32_t* ids_out, int32_t*
     }
 }
 
+// the stage clock of a call, ev[0] .. ev[5]: the mel (ev[1] after its H2D copy) and the encoder here, then the
+// caller's two stages, closed by stage_times
+static void timed_mel_encode(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* view_off) {
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[0], s->st));
+    s->timing = true;
+    try { mel_impl(s, samples, n_samples, batch, view_off, nullptr); } catch (...) { s->timing = false; throw; }
+    s->timing = false;
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[2], s->st));
+    session_encode(s, nullptr);
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[3], s->st));
+}
+// ev[5] recorded and waited for: last_ms[i] = ev[i] .. ev[i + 1], last_ms[5] the whole call
+static void stage_times(Session* s) {
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[5], s->st));
+    ASRB_CUDA_CHECK(cudaEventSynchronize(s->ev[5]));
+    for (int i = 0; i < 5; ++i) ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[i], s->ev[i], s->ev[i + 1]));
+    ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[5], s->ev[0], s->ev[5]));
+}
+
 static void transcribe_impl(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* view_off,
                             const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
                             int32_t* ids_out, int32_t* lens_out) {
@@ -1053,22 +1109,12 @@ static void transcribe_impl(Session* s, const float* const* samples, const int64
     check_sampling_options(s, batch);
     check_context(s, batch);
     ASRB_REQUIRE(max_new_tokens >= 1 && max_new_tokens <= s->max_new, ASRB_ERR_INVALID, "max_new_tokens exceeds session capacity");
-    cudaStream_t st = s->st;
     s->launches = 0; s->decode_steps = 0;
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
-    s->timing = true;
-    try { mel_impl(s, samples, n_samples, batch, view_off, nullptr); } catch (...) { s->timing = false; throw; }   // records ev[1] after the H2D
-    s->timing = false;
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
-    session_encode(s, nullptr);
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[3], st));
+    timed_mel_encode(s, samples, n_samples, batch, view_off);
     session_prefill(s, lang_ids, n_lang_ids, nullptr, nullptr);
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
+    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], s->st));
     session_generate(s, max_new_tokens, ids_out, lens_out);
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
-    ASRB_CUDA_CHECK(cudaEventSynchronize(s->ev[5]));
-    for (int i = 0; i < 5; ++i) ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[i], s->ev[i], s->ev[i + 1]));
-    ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[5], s->ev[0], s->ev[5]));
+    stage_times(s);
 }
 void session_transcribe_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch,
                             const int64_t* const* lang_ids, const int32_t* n_lang_ids, int max_new_tokens,
@@ -1110,20 +1156,20 @@ void session_transcribe_segments(Session* s, int n, const int32_t* file, const i
 // device buffers taken all or none: a failed cudaMalloc frees the ones already taken and throws, and nothing of the
 // session has changed; commit() hands them to the session
 struct AllocAll {
-    std::vector<void*> got;
-    ~AllocAll() { for (void* p : got) cudaFree(p); }
-    template <typename T> T* take(size_t n) {
+    std::vector<void*> got, got_host;
+    ~AllocAll() { for (void* p : got) cudaFree(p); for (void* p : got_host) cudaFreeHost(p); }
+    template <typename T> T* take(size_t n, bool pinned = false) {     // pinned: host memory
         void* p = nullptr;
-        ASRB_CUDA_CHECK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)));
-        got.push_back(p);
+        if (pinned) ASRB_CUDA_CHECK(cudaMallocHost(&p, std::max<size_t>(n, 1) * sizeof(T)));
+        else ASRB_CUDA_CHECK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)));
+        (pinned ? got_host : got).push_back(p);
         return static_cast<T*>(p);
     }
-    void commit(Session* s) { for (void* p : got) s->owned.push_back(p); got.clear(); }
+    void commit(Session* s) {
+        s->owned.insert(s->owned.end(), got.begin(), got.end()); got.clear();
+        s->owned_host.insert(s->owned_host.end(), got_host.begin(), got_host.end()); got_host.clear();
+    }
 };
-static void release_owned(Session* s, void* p) {
-    auto it = std::find(s->owned.begin(), s->owned.end(), p);
-    if (it != s->owned.end()) { cudaFree(p); s->owned.erase(it); }
-}
 
 // a scoring call's prefill of `rows` rows, `score_rows` head rows and a plan of `plan_ints` ints: every buffer is grown
 // to fit first, then the old ones are released, so a failed allocation leaves the session as it was
@@ -1148,10 +1194,7 @@ static void ensure_score_bufs(Session* s, size_t rows, int score_rows, size_t pl
         tk_ids = a.take<int>(R * TK_MAX); tk_lp = a.take<float>(R * TK_MAX);
     }
     int *d_int = nullptr, *h_int = nullptr;
-    if (plan) {
-        d_int = a.take<int>(plan_ints);
-        ASRB_CUDA_CHECK(cudaMallocHost(&h_int, plan_ints * sizeof(int)));
-    }
+    if (plan) { d_int = a.take<int>(plan_ints); h_int = a.take<int>(plan_ints, true); }
     // every allocation succeeded: swap in, release the old buffers
     a.commit(s);
     if (act) {
@@ -1166,97 +1209,48 @@ static void ensure_score_bufs(Session* s, size_t rows, int score_rows, size_t pl
         b.rows_cap = (int)R;
     }
     if (plan) {
-        release_owned(s, b.d_int);
-        if (b.h_int) cudaFreeHost(b.h_int);
+        release_owned(s, b.d_int); release_owned(s, b.h_int);
         b.d_int = d_int; b.h_int = h_int; b.int_cap = plan_ints;
     }
 }
 
 // the plan of a teacher-forced prefill (asrb_score_ids, asrb_align_ids): slot q = candidate q; the first candidate of an
 // utterance leads (its prompt and its ids but the last), the others (followers) compute their ids but the last from
-// position S_b on, their prompt K/V fanned out.  Grows the buffers (the score head's only with `head`), uploads the
-// plan and points the session's row arrays at it
-struct TfPlan {
-    int N = 0, totS = 0, maxrows = 0, R = 0;          // slots, prefill rows, most rows of one slot, ids in all
-    std::vector<int> srow0, coff;                     // first row of slot q; first id of candidate q in the id order
-    const int *d_src = nullptr, *d_tgt = nullptr;     // [R]: the row predicting each id, and the id
-    bool fan = false; FanOut fan_plan{}; const int* d_qpos0 = nullptr;
-};
-static TfPlan plan_teacher_forced(Session* s, int B, const int64_t* const* lang_ids, const int32_t* n_lang_ids,
-                                  const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len, int N,
-                                  bool head) {
-    const asrb_dims& c = s->m->d.c;
-    cudaStream_t st = s->st;
-    TfPlan tf;
+// position S_b on, their prompt K/V fanned out.  Grows the buffers (the score head's only with `head`).  Behind the plan,
+// for each id in candidate order (candidate q's from coff[q] on): the row predicting it (src), then the ids (tgt)
+static PrefillPlan plan_teacher_forced(Session* s, int B, const int64_t* const* lang_ids, const std::vector<int>& nl,
+                                       const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len, int N,
+                                       bool head, std::vector<int>& coff) {
     s->S.assign(B, 0);
-    std::vector<int> utt(N), lead(N), rows(N);
-    std::vector<int>& srow0 = tf.srow0; std::vector<int>& coff = tf.coff;
-    srow0.assign(N, 0); coff.assign(N + 1, 0);
-    int totS = 0, maxrows = 0, R = 0;
-    int64_t shared = 0;
-    for (int b = 0, q = 0; b < B; ++b) {
-        const int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
-        s->S[b] = 9 + (int)context_of(s, b).size() + s->T[b] + 6 + nl;
+    std::vector<PrefillSeq> seq((size_t)N);
+    coff.assign(N + 1, 0);
+    size_t totS = 0;
+    for (int b = 0, q = 0; b < B; ++b)
         for (int j = 0; j < n_cand[b]; ++j, ++q) {
-            utt[q] = b; lead[q] = q - j;
-            rows[q] = (j == 0 ? s->S[b] : 0) + cand_len[q] - 1;
-            srow0[q] = totS; totS += rows[q]; maxrows = std::max(maxrows, rows[q]);
-            coff[q] = R; R += cand_len[q];
+            PrefillSeq& x = seq[q];
+            build_prompt(s, b, lang_ids, nl[b], x.pid, x.parow);
+            s->S[b] = (int)x.pid.size();
+            if (j > 0) { x.lead = q - j; x.from = s->S[b]; }
+            for (int i = 0; i + 1 < cand_len[q]; ++i) { x.pid.push_back((int)cand_ids[q][i]); x.parow.push_back(-1); }
+            totS += x.pid.size() - x.from;
+            coff[q + 1] = coff[q] + cand_len[q];
         }
-        shared += (int64_t)(n_cand[b] - 1) * s->S[b];
-    }
-    coff[N] = R;
-    Session::ScoreBufs& sb = s->sc;
-    ensure_score_bufs(s, (size_t)totS, head ? R : 0, 4 * (size_t)totS + 8 * (size_t)N + 2 * (size_t)R + 16);
-    int* hi = sb.h_int;
-    int* ids = hi; int* arow = ids + totS; int* rseq = arow + totS; int* rpos = rseq + totS;
-    int* sq0 = rpos + totS; int* slen = sq0 + N; int* qpos0 = slen + N;
-    int* fan_n = qpos0 + N; int* fan_off = fan_n + N; int* fan_P = fan_off + N; int* fan_slots = fan_P + N;
-    int* src = fan_slots + std::max(N, 1); int* tgt = src + R;
-    const size_t nint = (size_t)(tgt + R - hi);
-    ASRB_REQUIRE(nint <= sb.int_cap && (!head || R <= sb.rows_cap), ASRB_ERR_INVALID, "score: plan exceeds session capacity");
-    std::vector<int> pid, parow;
-    int nf = 0;
-    for (int q = 0; q < N; ++q) {
-        const int b = utt[q], Sb = s->S[b];
-        const bool leader = lead[q] == q;
-        int r = srow0[q];
-        if (leader) {
-            build_prompt(s, b, lang_ids, pid, parow);
-            r = plan_prompt_rows(pid, parow, 0, r, q, ids, arow, rseq, rpos);
-        }
-        for (int i = 0; i + 1 < cand_len[q]; ++i, ++r) { ids[r] = (int)cand_ids[q][i]; arow[r] = -1; rseq[r] = q; rpos[r] = Sb + i; }
-        sq0[q] = srow0[q]; slen[q] = rows[q]; qpos0[q] = leader ? 0 : Sb;
-        fan_off[q] = nf; fan_n[q] = 0; fan_P[q] = 0;
-        if (leader) {
-            fan_P[q] = Sb;
-            for (int f = q + 1; f < N && lead[f] == q; ++f) { fan_slots[nf++] = f; ++fan_n[q]; }
-        }
-        // row map: id 0 from the leader's last prompt row, id i from this candidate's row at position S_b + i - 1
-        const int own0 = leader ? srow0[q] + Sb : srow0[q];
-        for (int i = 0; i < cand_len[q]; ++i) {
-            src[coff[q] + i] = i == 0 ? srow0[lead[q]] + Sb - 1 : own0 + i - 1;
-            tgt[coff[q] + i] = (int)cand_ids[q][i];
-        }
-    }
-    s->pf_rows = totS; s->pf_shared_rows = shared;
-    s->pf_fan_bytes = shared * 2LL * c.num_hidden_layers * c.num_key_value_heads * c.head_dim * (int64_t)sizeof(float);
-    int* di = sb.d_int;
-    ASRB_CUDA_CHECK(cudaMemcpyAsync(di, hi, nint * sizeof(int), cudaMemcpyHostToDevice, st));
-    s->d_ids = di; s->d_audio_row = di + (arow - hi); s->d_row_seq = di + (rseq - hi);
-    s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
-    tf.fan_plan = FanOut{di + (fan_n - hi), di + (fan_off - hi), di + (fan_P - hi), di + (fan_slots - hi)};
-    tf.fan = nf > 0;
-    tf.d_qpos0 = tf.fan ? di + (qpos0 - hi) : nullptr;
-    tf.d_src = di + (src - hi); tf.d_tgt = di + (tgt - hi);
-    tf.N = N; tf.totS = totS; tf.maxrows = maxrows; tf.R = R;
-    return tf;
+    const int R = coff[N];
+    ensure_score_bufs(s, totS, head ? R : 0, 4 * totS + 7 * (size_t)N + 2 * (size_t)R);
+    return plan_prefill(s, seq, s->sc.h_int, s->sc.d_int, s->sc.int_cap, 2 * R, [&](int* src, const PrefillPlan& p) {
+        for (int b = 0, q = 0; b < B; ++b)
+            for (int j = 0; j < n_cand[b]; ++j, ++q)
+                for (int i = 0; i < cand_len[q]; ++i) {
+                    const int o = i == 0 ? q - j : q;     // id i is predicted at position S_b + i - 1: the leader's for id 0
+                    src[coff[q] + i] = p.srow0[o] + s->S[b] + i - 1 - seq[o].from;
+                    src[R + coff[q] + i] = (int)cand_ids[q][i];
+                }
+    });
 }
 
-static void score_impl(Session* s, const float* const* samples, const int64_t* n_samples, int batch,
-                       const int64_t* const* lang_ids, const int32_t* n_lang_ids, const int32_t* n_cand,
-                       const int64_t* const* cand_ids, const int32_t* cand_len, int max_new_tokens, float* logprob_out,
-                       int32_t* top_ids_out, float* top_lp_out) {
+void session_score_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* const* lang_ids,
+                       const int32_t* n_lang_ids, const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
+                       int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out) {
     ASRB_REQUIRE(logprob_out && n_cand && cand_ids && cand_len, ASRB_ERR_INVALID, "score: null argument");
     if (samples == nullptr) {
         batch = (int)s->ingested_n.size();          // asrb_score_ingested
@@ -1269,13 +1263,11 @@ static void score_impl(Session* s, const float* const* samples, const int64_t* n
     check_context(s, batch);
     check_score_head(m);
     int64_t n_total = 0;
+    std::vector<int> nl((size_t)batch);
     for (int b = 0; b < batch; ++b) {
         ASRB_REQUIRE(n_cand[b] >= 1, ASRB_ERR_INVALID, "score: every utterance needs at least one candidate");
         n_total += n_cand[b];
-        const int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
-        ASRB_REQUIRE(nl >= 0 && nl <= s->max_lang, ASRB_ERR_INVALID, "language prompt exceeds session capacity");
-        for (int i = 0; i < nl; ++i)
-            ASRB_REQUIRE(lang_ids[b][i] >= 0 && lang_ids[b][i] < c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
+        nl[b] = lang_count(s, lang_ids, n_lang_ids, b);
     }
     ASRB_REQUIRE(n_total <= s->max_batch, ASRB_ERR_INVALID,
                  "score: " + std::to_string(n_total) + " candidates exceed the session's max_batch (one KV slot each)");
@@ -1292,22 +1284,17 @@ static void score_impl(Session* s, const float* const* samples, const int64_t* n
     cudaStream_t st = s->st;
     s->launches = 0; s->decode_steps = 0;
     s->nbest_valid = false; s->lp_valid = false; s->tk_valid = 0;
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
-    s->timing = true;
-    try { mel_impl(s, samples, n_samples, batch, nullptr, nullptr); } catch (...) { s->timing = false; throw; }
-    s->timing = false;
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
-    session_encode(s, nullptr);
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[3], st));
+    timed_mel_encode(s, samples, n_samples, batch, nullptr);
     s->stage = 2;                                     // the KV slots are overwritten: no run to continue after this call
-    const TfPlan tf = plan_teacher_forced(s, batch, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len, N, true);
-    const int R = tf.R; const std::vector<int>& coff = tf.coff;
+    std::vector<int> coff;
+    const PrefillPlan pf = plan_teacher_forced(s, batch, lang_ids, nl, n_cand, cand_ids, cand_len, N, true, coff);
+    const int R = coff[N];
     Session::ScoreBufs& sb = s->sc;
-    prefill_layers(s, tf.totS, N, tf.maxrows, tf.fan ? &tf.fan_plan : nullptr, tf.d_qpos0, s->audio);
+    prefill_layers(s, pf, s->audio);
     ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
-    launch_score_head(m, s->hid, tf.d_src, tf.d_tgt, R, sb.gathered, sb.planes, (size_t)sb.rows_cap * c.hidden_size,
+    launch_score_head(m, s->hid, pf.d_tail, pf.d_tail + R, R, sb.gathered, sb.planes, (size_t)sb.rows_cap * c.hidden_size,
                       s->nplanes, sb.part, topk, sb.lp, sb.tk_ids, sb.tk_lp, st, &s->launches);
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
+    stage_times(s);
     std::vector<float> lp((size_t)R), tlp(topk ? (size_t)R * TK_MAX : 0);
     std::vector<int> tid(tlp.size());
     ASRB_CUDA_CHECK(cudaMemcpyAsync(lp.data(), sb.lp, lp.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -1316,8 +1303,6 @@ static void score_impl(Session* s, const float* const* samples, const int64_t* n
         ASRB_CUDA_CHECK(cudaMemcpyAsync(tlp.data(), sb.tk_lp, tlp.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
     }
     ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
-    for (int i = 0; i < 5; ++i) ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[i], s->ev[i], s->ev[i + 1]));
-    ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[5], s->ev[0], s->ev[5]));
     const float nan = std::numeric_limits<float>::quiet_NaN();
     for (int q = 0; q < N; ++q)
         for (int i = 0; i < max_new_tokens; ++i) {
@@ -1330,13 +1315,6 @@ static void score_impl(Session* s, const float* const* samples, const int64_t* n
                     top_lp_out[o * k + j] = in ? tlp[r * TK_MAX + j] : nan;
                 }
         }
-}
-
-void session_score_ids(Session* s, const float* const* samples, const int64_t* n_samples, int batch, const int64_t* const* lang_ids,
-                       const int32_t* n_lang_ids, const int32_t* n_cand, const int64_t* const* cand_ids, const int32_t* cand_len,
-                       int max_new_tokens, float* logprob_out, int32_t* top_ids_out, float* top_lp_out) {
-    score_impl(s, samples, n_samples, batch, lang_ids, n_lang_ids, n_cand, cand_ids, cand_len, max_new_tokens, logprob_out,
-               top_ids_out, top_lp_out);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1402,15 +1380,13 @@ static void align_impl(Session* s, const float* const* samples, const int64_t* n
     ASRB_REQUIRE(max_ids >= 1, ASRB_ERR_INVALID, "align: max_ids must be >= 1");
     check_context(s, batch);
     int maxn = 0;
+    std::vector<int> nl((size_t)batch);
     for (int b = 0; b < batch; ++b) {
         if (!ingested && !view_off) {
             ASRB_REQUIRE(samples[b] && n_samples[b] > 0 && n_samples[b] <= s->max_samples, ASRB_ERR_INVALID, "n_samples out of session capacity");
             ASRB_REQUIRE(((n_samples[b] + 159) / 160) * 160 > 200, ASRB_ERR_INVALID, "utterance too short for reflect padding (needs > 200 samples)");
         }
-        const int nl = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
-        ASRB_REQUIRE(nl >= 0 && nl <= s->max_lang, ASRB_ERR_INVALID, "language prompt exceeds session capacity");
-        for (int i = 0; i < nl; ++i)
-            ASRB_REQUIRE(lang_ids[b][i] >= 0 && lang_ids[b][i] < c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
+        nl[b] = lang_count(s, lang_ids, n_lang_ids, b);
         const int n = n_ids[b];
         ASRB_REQUIRE(n >= 1 && n <= max_ids && n <= s->max_new, ASRB_ERR_INVALID,
                      "align: n_ids outside [1, min(max_ids, the session's max_new_tokens)]");
@@ -1440,18 +1416,13 @@ static void align_impl(Session* s, const float* const* samples, const int64_t* n
     s->launches = 0; s->decode_steps = 0;
     s->nbest_valid = false; s->lp_valid = false; s->tk_valid = 0;
     s->al.N.clear(); s->al.T.clear(); s->al.moff.clear();
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[0], st));
-    s->timing = true;
-    try { mel_impl(s, samples, n_samples, batch, view_off, nullptr); } catch (...) { s->timing = false; throw; }
-    s->timing = false;
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[2], st));
-    session_encode(s, nullptr);
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[3], st));
+    timed_mel_encode(s, samples, n_samples, batch, view_off);
     s->stage = 2;                                     // the KV slots are overwritten: no run to continue after this call
     const int B = batch;
     // ---- plan: one candidate per utterance (slot b), no score head ----
     const std::vector<int32_t> ones((size_t)B, 1);
-    const TfPlan tf = plan_teacher_forced(s, B, lang_ids, n_lang_ids, ones.data(), ids, n_ids, B, false);
+    std::vector<int> coff;
+    const PrefillPlan pf = plan_teacher_forced(s, B, lang_ids, nl, ones.data(), ids, n_ids, B, false, coff);
     std::vector<int> N(B), T(B), pi(7 * (size_t)B + hs.size());
     std::vector<long long> moff(B), toff(B);
     int* qrow0 = pi.data(); int* pN = qrow0 + B; int* pT = pN + B; int* a0 = pT + B; int* slot = a0 + B; int* soff = slot + B;
@@ -1459,8 +1430,8 @@ static void align_impl(Session* s, const float* const* samples, const int64_t* n
     long long sumNT = 0, words = 0; int sumN = 0, maxN = 0, maxT = 0, maxNT = 0; size_t smem = 0;
     for (int b = 0; b < B; ++b) {
         N[b] = n_ids[b] - text_from[b]; T[b] = s->T[b];
-        qrow0[b] = tf.srow0[b] + s->S[b] - 1 + text_from[b]; pN[b] = N[b]; pT[b] = T[b];
-        a0[b] = 9 + (int)context_of(s, b).size(); slot[b] = b; soff[b] = sumN;
+        qrow0[b] = pf.srow0[b] + s->S[b] - 1 + text_from[b]; pN[b] = N[b]; pT[b] = T[b];
+        a0[b] = audio_start((int)context_of(s, b).size()); slot[b] = b; soff[b] = sumN;
         moff[b] = sumNT; sumNT += (long long)N[b] * T[b]; sumN += N[b];
         in_smem[b] = align_dtw_smem(N[b], T[b], true) <= m.ctx->smem_optin;
         smem = std::max(smem, align_dtw_smem(N[b], T[b], in_smem[b] != 0));
@@ -1490,27 +1461,24 @@ static void align_impl(Session* s, const float* const* samples, const int64_t* n
     hook.d_qrow0 = d_pi + (qrow0 - pi.data()); hook.d_N = d_pi + (pN - pi.data()); hook.d_T = d_pi + (pT - pi.data());
     hook.d_a0 = d_pi + (a0 - pi.data()); hook.d_slot = d_pi + (slot - pi.data()); hook.d_heads = d_pi + (hl - pi.data());
     hook.d_moff = d_pl;
-    prefill_layers(s, tf.totS, B, tf.maxrows, tf.fan ? &tf.fan_plan : nullptr, tf.d_qpos0, s->audio, hook.last + 1, &hook);
+    prefill_layers(s, pf, s->audio, hook.last + 1, &hook);
     ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
     AlignDtwArgs da{};
     da.N = hook.d_N; da.T = hook.d_T; da.moff = d_pl; da.M = ab.M; da.smem_trace = d_pi + (in_smem - pi.data());
     da.trace = ab.trace; da.toff = d_pl + B; da.start = ab.start; da.soff = d_pi + (soff - pi.data());
     launch_align_dtw(da, B, smem, st);
     s->launches += 1;
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
+    stage_times(s);
     std::vector<int> tok((size_t)sumN);
     ASRB_CUDA_CHECK(cudaMemcpyAsync(tok.data(), ab.start, (size_t)sumN * sizeof(int), cudaMemcpyDeviceToHost, st));
     ASRB_CUDA_CHECK(cudaStreamSynchronize(st));
-    for (int i = 0; i < 5; ++i) ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[i], s->ev[i], s->ev[i + 1]));
-    ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[5], s->ev[0], s->ev[5]));
     ab.N = N; ab.T = T; ab.moff = moff;
     // ---- frames: audio token t of chunk k starts at frame k * chunk_frames + 8 t ----
     const int cf = m.d.chunk_frames;
     for (int b = 0; b < B; ++b) {
         std::vector<int> frame;
         for (int k = 0; k < s->C[b]; ++k) {
-            const int fr = (int)std::min<int64_t>(cf, s->F[b] - (int64_t)k * cf);
-            const int valid = conv_out_len(conv_out_len(conv_out_len(fr)));
+            const int valid = chunk_tokens((int)std::min<int64_t>(cf, s->F[b] - (int64_t)k * cf));
             for (int t = 0; t < valid; ++t) frame.push_back(k * cf + 8 * t);
         }
         int32_t* so = start_out + (size_t)b * max_ids; int32_t* eo = end_out + (size_t)b * max_ids;
@@ -1589,9 +1557,8 @@ void session_stream_open(Session* s, int n_streams, int rollback, int unfixed) {
         float* tok = a.take<float>(Bm * s->maxT * d.c.output_dim);
         float* stats = a.take<float>(Bm * s->str_stats_ld);
         int* pi = a.take<int>(s->str_int_cap);
-        float* hs = nullptr; int* hi = nullptr;
-        ASRB_CUDA_CHECK(cudaMallocHost(&hs, Bm * s->str_stats_ld * sizeof(float)));
-        if (cudaMallocHost(&hi, s->str_int_cap * sizeof(int)) != cudaSuccess) { cudaFreeHost(hs); throw Error(ASRB_ERR_CUDA, "stream_open: out of host memory"); }
+        float* hs = a.take<float>(Bm * s->str_stats_ld, true);
+        int* hi = a.take<int>(s->str_int_cap, true);
         a.commit(s);
         s->str_samples = smp; s->str_raw = raw; s->str_tok = tok; s->str_stats = stats; s->str_int = pi;
         s->h_str_stats = hs; s->h_str_int = hi;
@@ -1640,11 +1607,8 @@ void session_stream_push(Session* s, int nst, const float* const* samples, const
         ASRB_REQUIRE(!x.closed, ASRB_ERR_STATE, "stream_push: stream " + std::to_string(b) + " is closed (asrb_stream_reset reopens it)");
         ASRB_REQUIRE(x.n + nb <= s->max_samples, ASRB_ERR_INVALID, "stream_push: samples past the session's max_samples");
         ASRB_REQUIRE(((x.n + nb + 159) / 160) * 160 > 200, ASRB_ERR_INVALID, "stream_push: a stream needs > 160 samples before its first push");
-        nl[b] = (lang_ids && lang_ids[b] && n_lang_ids) ? n_lang_ids[b] : 0;
-        ASRB_REQUIRE(nl[b] >= 0 && nl[b] + (int)x.p.size() <= s->max_lang, ASRB_ERR_INVALID,
-                     "stream_push: language ids + forced prefix exceed the session's max_lang_ids");
-        for (int i = 0; i < nl[b]; ++i)
-            ASRB_REQUIRE(lang_ids[b][i] >= 0 && lang_ids[b][i] < c.vocab_size, ASRB_ERR_INVALID, "language id out of vocabulary");
+        nl[b] = lang_count(s, lang_ids, n_lang_ids, b, (int)x.p.size(),
+                           "stream_push: language ids + forced prefix exceed the session's max_lang_ids");
         ASRB_REQUIRE((int)x.p.size() + max_new_tokens <= max_ids, ASRB_ERR_INVALID, "stream_push: max_ids < forced prefix + max_new_tokens");
     }
     ASRB_CUDA_CHECK(cudaSetDevice(m.ctx->device));
@@ -1705,7 +1669,7 @@ void session_stream_push(Session* s, int nst, const float* const* samples, const
         for (int w = 0; w < W; ++w) {
             const int f0 = w * Wf, f1 = std::min(F[b], (w + 1) * Wf);
             int wt = 0;
-            for (int k = f0 / cf; k * cf < f1; ++k) wt += conv_out_len(conv_out_len(conv_out_len(std::min(cf, F[b] - k * cf))));
+            for (int k = f0 / cf; k * cf < f1; ++k) wt += chunk_tokens(std::min(cf, F[b] - k * cf));
             const bool finished = f1 <= Ffin[b];
             const bool was_final = x.win_final[w];
             const bool floor_ok = phi == x.win_phi[w] || row[2 + w] >= fmaxf(phi, x.win_phi[w]);
@@ -1722,7 +1686,7 @@ void session_stream_push(Session* s, int nst, const float* const* samples, const
         T[b] = tok;
         x.phi = phi; x.Ffin = Ffin[b]; x.T = tok;
         // P_b: head, context and the pads of the windows before the first re-encoded one (0 before the first prefill)
-        P[b] = std::min(9 + (int)x.ctx.size() + (tok_re < 0 ? tok : tok_re), x.kv_valid);
+        P[b] = std::min(audio_start((int)x.ctx.size()) + (tok_re < 0 ? tok : tok_re), x.kv_valid);
     }
     s->str_counts[0] = (int64_t)utts.size();
     // ---- encoder: the re-encoded windows as pseudo-utterances of at most one window each, in waves of max_batch ----
@@ -1758,63 +1722,44 @@ void session_stream_push(Session* s, int nst, const float* const* samples, const
     // ---- prefill: stream b's rows from position P_b on, attending to the K/V its slot keeps below P_b ----
     const int B = nst;
     s->B = B; s->run_k = 1; s->run_alpha = -1.0; s->nslots = B;
-    s->S.assign(B, 0); s->srow0.assign(B, 0);
-    int totS = 0, maxlen = 0, maxrows = 0;
-    for (int b = 0; b < B; ++b) {
-        const Session::Stream& x = s->streams[b];
-        maxlen = std::max(maxlen, x.kv_valid + 1);     // an idle row's decode position (below)
-        if (!act[b]) continue;
-        s->srow0[b] = totS; s->S[b] = 9 + (int)x.ctx.size() + T[b] + 6 + nl[b] + (int)x.p.size();
-        totS += s->S[b] - P[b];
-        maxlen = std::max(maxlen, s->S[b]); maxrows = std::max(maxrows, s->S[b] - P[b]);
-    }
-    s->totS = totS; s->maxlenS = maxlen;
-    int* hi = s->h_int + s->enc_int_cap;
-    int* di = s->d_int + s->enc_int_cap;
-    int* ids = hi; int* arow = ids + totS; int* rseq = arow + totS; int* rpos = rseq + totS;
-    int* sq0 = rpos + totS; int* slen = sq0 + B; int* lastrow = slen + B; int* pos0 = lastrow + B; int* qpos0 = pos0 + B;
-    int* done0 = qpos0 + B;
-    const size_t nint = (size_t)(done0 + B - hi);
-    ASRB_REQUIRE(s->enc_int_cap + nint <= s->int_cap, ASRB_ERR_INVALID, "plan exceeds session capacity");
+    s->S.assign(B, 0); s->maxlenS = 0;
+    std::vector<PrefillSeq> seq((size_t)B);
     int64_t kept = 0;
     for (int b = 0; b < B; ++b) {
         const Session::Stream& x = s->streams[b];
-        // idle: no rows, done.  The batched decode step still writes a done row's K/V at its position: kv_valid, the
-        // first position the stream's next prefill recomputes
-        sq0[b] = 0; slen[b] = 0; lastrow[b] = 0; pos0[b] = x.kv_valid; qpos0[b] = 0; done0[b] = 1;
+        seq[b].lead = b;                                          // its slot keeps positions [0, from)
+        s->maxlenS = std::max(s->maxlenS, x.kv_valid + 1);       // an idle row's decode position (below)
         if (!act[b]) continue;
-        std::vector<int> pid, parow;
-        build_prompt(x.ctx, T[b], b * s->maxT, nl[b] > 0 ? lang_ids[b] : nullptr, nl[b], x.p, pid, parow);
-        plan_prompt_rows(pid, parow, P[b], s->srow0[b], b, ids, arow, rseq, rpos);
-        const int rows = s->S[b] - P[b];
-        sq0[b] = s->srow0[b]; slen[b] = rows; lastrow[b] = s->srow0[b] + rows - 1; pos0[b] = s->S[b] - 1; qpos0[b] = P[b]; done0[b] = 0;
-        kept += P[b];
+        build_prompt(x.ctx, T[b], b * s->maxT, nl[b] > 0 ? lang_ids[b] : nullptr, nl[b], x.p, seq[b].pid, seq[b].parow);
+        seq[b].from = P[b]; kept += P[b];
+        s->S[b] = (int)seq[b].pid.size(); s->maxlenS = std::max(s->maxlenS, s->S[b]);
     }
-    s->str_counts[3] = totS; s->str_counts[4] = kept;
-    s->pf_rows = totS; s->pf_shared_rows = 0; s->pf_fan_bytes = 0;
-    ASRB_CUDA_CHECK(cudaMemcpyAsync(di, hi, nint * sizeof(int), cudaMemcpyHostToDevice, st));
-    s->d_ids = di; s->d_audio_row = di + (arow - hi); s->d_row_seq = di + (rseq - hi);
-    s->d_row_pos = di + (rpos - hi); s->d_seq_q0 = di + (sq0 - hi); s->d_seq_len = di + (slen - hi);
-    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->d_lastrow, di + (lastrow - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    ASRB_CUDA_CHECK(cudaMemcpyAsync(s->db.pos, di + (pos0 - hi), B * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    begin_run(s, B, di + (done0 - hi));
-    prefill_layers(s, totS, B, maxrows, nullptr, di + (qpos0 - hi), s->str_tok);
+    // idle: no rows, done.  The batched decode step still writes a done row's K/V at its position: kv_valid, the first
+    // position the stream's next prefill recomputes
+    const PrefillPlan pf = plan_prefill(s, seq, s->h_int + s->enc_int_cap, s->d_int + s->enc_int_cap, s->int_cap - s->enc_int_cap,
+                                        3 * B, [&](int* t, const PrefillPlan& p) {   // lastrow | pos0 | done0
+        for (int b = 0; b < B; ++b) {
+            t[b] = act[b] ? p.srow0[b] + s->S[b] - P[b] - 1 : 0;
+            t[B + b] = act[b] ? s->S[b] - 1 : s->streams[b].kv_valid;
+            t[2 * B + b] = !act[b];
+        }
+    });
+    s->str_counts[3] = pf.totS; s->str_counts[4] = kept;
+    begin_run(s, B, pf.d_tail);
+    prefill_layers(s, pf, s->str_tok);
     first_token(s, B, false, nullptr);
     s->stage = 3;
     ASRB_CUDA_CHECK(cudaEventRecord(s->ev[4], st));
     // ---- decode: the offline batch's paths; idle streams are done from the start ----
     std::vector<int32_t> g((size_t)B * max_new_tokens), glen((size_t)B);
     session_generate(s, max_new_tokens, g.data(), glen.data());
-    ASRB_CUDA_CHECK(cudaEventRecord(s->ev[5], st));
-    ASRB_CUDA_CHECK(cudaEventSynchronize(s->ev[5]));
-    for (int i = 0; i < 5; ++i) ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[i], s->ev[i], s->ev[i + 1]));
-    ASRB_CUDA_CHECK(cudaEventElapsedTime(&s->last_ms[5], s->ev[0], s->ev[5]));
+    stage_times(s);
     s->stream_run = true;
     // ---- hypotheses and the next forced prefixes ----
     for (int b = 0; b < B; ++b) {
         if (!act[b]) continue;
         Session::Stream& x = s->streams[b];
-        x.kv_valid = 9 + (int)x.ctx.size() + T[b];
+        x.kv_valid = audio_start((int)x.ctx.size()) + T[b];
         std::vector<int> hyp = x.p;
         hyp.insert(hyp.end(), g.begin() + (size_t)b * max_new_tokens, g.begin() + (size_t)b * max_new_tokens + glen[b]);
         if (fin[b]) { x.p = hyp; x.closed = true; }
