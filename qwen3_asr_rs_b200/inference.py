@@ -13,7 +13,8 @@ from __future__ import annotations
 import ctypes as C
 import math
 import os
-from dataclasses import dataclass
+from contextlib import contextmanager
+from dataclasses import dataclass, replace
 from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -223,13 +224,95 @@ def default_search_s(max_segment_s: float) -> float:
     return min(5.0, math.floor(float(max_segment_s) * 100 / 2) / 100)
 
 
+_PCM_FMT = {"int16": 0, "float32": 1, "int32": 2}
+
+
 def _pcm_arrays(pcms) -> List[np.ndarray]:
     """PCM arrays as contiguous [frames, channels] of a supported dtype, else ValueError."""
     arrs = [np.ascontiguousarray(a if a.ndim == 2 else a.reshape(-1, 1)) for a in pcms]
     for a in arrs:
-        if a.dtype.name not in AsrInference._PCM_FMT:
+        if a.dtype.name not in _PCM_FMT:
             raise ValueError(f"PCM dtype must be int16 / int32 / float32, got {a.dtype}")
     return arrs
+
+
+def _pcm_args(arrs: Sequence[np.ndarray], rates: Sequence[int]):
+    """The per-file arrays of asrb_ingest_pcm / asrb_ingest_long: data pointers, frames, channels, rates, formats."""
+    B = len(arrs)
+    return ((C.c_void_p * B)(*[a.ctypes.data for a in arrs]), (C.c_int64 * B)(*[a.shape[0] for a in arrs]),
+            (C.c_int32 * B)(*[a.shape[1] for a in arrs]), (C.c_int32 * B)(*[int(r) for r in rates]),
+            (C.c_int32 * B)(*[_PCM_FMT[a.dtype.name] for a in arrs]))
+
+
+# the library's value of every per-call session option (include/asr_b200.h)
+_OPTION_DEFAULTS = {"logprobs": "0", "top_logprobs": "0", "temperature": "0", "seed": "0", "beam_size": "1",
+                    "length_penalty": "none", "no_repeat_ngram_size": "0", "repetition_penalty": "1"}
+
+
+def _decode_options(logprobs: bool, top_logprobs: int, temperature: Optional[float], seed: int,
+                    beam: Optional[Tuple[int, Optional[float]]], rep: Tuple[int, float]) -> Dict[str, str]:
+    """The session options of one decode call, in the order they are set: the records asked for, temperature and seed
+    when sampling (temperature not None), beam_size and, for K > 1, length_penalty (beam = (K, length penalty); None:
+    neither), and the repetition controls rep = (N, penalty)."""
+    opts = {}
+    if logprobs:
+        opts["logprobs"] = "1"
+    if top_logprobs:
+        opts["top_logprobs"] = str(top_logprobs)
+    if temperature is not None:
+        opts.update(temperature=temperature_option(temperature), seed=str(seed))
+    if beam is not None:
+        opts["beam_size"] = str(beam[0])
+        if beam[0] > 1:
+            opts["length_penalty"] = length_penalty_option(beam[1])
+    opts.update(no_repeat_ngram_size=str(rep[0]), repetition_penalty=repetition_penalty_option(rep[1]))
+    return opts
+
+
+@dataclass
+class _Audio:
+    """The audio of one call's items, in one of three forms, so that the transcribe, score and align bodies need not
+    know which: "ids" = host f32 clips at 16 kHz; "ingested" = PCM arrays at `rates`, brought to mono 16 kHz on the GPU
+    (asrb_ingest_pcm); "segments" = (file, start, end) views into the session's long-audio buffer.  `lang` / `ctx`: per
+    item its language ids and its context (for a segment, those of its file; None: none for every item)."""
+    form: str
+    items: list
+    rates: Optional[list] = None
+    lang: Optional[list] = None
+    ctx: Optional[list] = None
+
+    def __len__(self) -> int:
+        return len(self.items)
+
+    def subset(self, idx: Sequence[int]) -> "_Audio":
+        """The items `idx`, in that order."""
+        pick = (lambda xs: None if xs is None else [xs[i] for i in idx])
+        return _Audio(self.form, pick(self.items), pick(self.rates), pick(self.lang), pick(self.ctx))
+
+    def prepare(self, eng: "AsrInference", slots: int, max_new: int):
+        """Make the engine's session ready for these items and return it.  Clips and PCM grow it to max(items, slots)
+        KV slots and `max_new` ids, and PCM is ingested; segment views keep the session as it is, since re-creating it
+        would drop the long-audio buffer."""
+        B = len(self.items)
+        langs, lptrs, llens, mx = eng._pack_lang(self.lang, B)
+        if self.form == "ids":
+            arrs, ptrs, lens = eng._pack_samples(self.items)
+            s = eng._ensure_session(max(B, slots), max(a.shape[0] for a in arrs), mx, max_new, _max_len(self.ctx))
+            lead = (ptrs, lens, B)
+        elif self.form == "ingested":
+            s, arrs, _ = eng._ingest(self.items, self.rates, mx, max_new, slots, _max_len(self.ctx))
+            lead = ()
+        else:
+            s, arrs = eng._session, None
+            lead = (B, (C.c_int32 * B)(*[f for f, _, _ in self.items]), (C.c_int64 * B)(*[a for _, a, _ in self.items]),
+                    (C.c_int64 * B)(*[b for _, _, b in self.items]))
+        self._keep = (arrs, langs)                   # the host arrays the pointers below refer to
+        self._args = (s, *lead, lptrs, llens)
+        return s
+
+    def call(self, lib, family: str, *rest) -> int:
+        """asrb_<family>_<form> (family: transcribe, score or align) on the prepared items; returns its status."""
+        return getattr(lib, f"asrb_{family}_{self.form}")(*self._args, *rest)
 
 
 def _concat_runs(runs: Sequence["TranscribeIds"]) -> "TranscribeIds":
@@ -564,14 +647,41 @@ class AsrInference:
         """asrb_session_set_context on the current session: None clears the contexts; else one entry per utterance of
         the next runs (None or an empty sequence: no context), or a single entry for all of them.  For the stage-level
         calls; transcribe_ids / transcribe_pcm / transcribe set their own contexts for the call."""
-        self._set_context(self._session, context_ids)
-
-    def _set_context(self, s, context_ids) -> None:
         if not context_ids:
-            _lib.check(self._lib.asrb_session_set_context(s, 0, None, None))
+            _lib.check(self._lib.asrb_session_set_context(self._session, 0, None, None))
             return
         keep, ptrs, lens, _ = self._pack_lang(context_ids, len(context_ids))
-        _lib.check(self._lib.asrb_session_set_context(s, len(context_ids), ptrs, lens))
+        _lib.check(self._lib.asrb_session_set_context(self._session, len(context_ids), ptrs, lens))
+
+    @contextmanager
+    def _call_scope(self, s, options: Dict[str, str], context_ids=None):
+        """One call on session s with `options` and, unless None, `context_ids` (as set_context).  An option is set
+        only where it differs from the engine's configured value (the library default when none is configured), since
+        setting one drops the captured per-phase step graph.  On exit, also on an exception, the context is cleared
+        and every option set goes back to that value.  Results that depend on the options are read inside the scope."""
+        undo = []
+        try:
+            for key, val in options.items():
+                conf = self._options.get(key, _OPTION_DEFAULTS[key])
+                if conf != val:
+                    _lib.check(self._lib.asrb_session_set_option(s, key.encode(), val.encode()))
+                    undo.append((key, conf))
+            if context_ids is not None:
+                keep, ptrs, lens, _ = self._pack_lang(context_ids, len(context_ids))
+                _lib.check(self._lib.asrb_session_set_context(s, len(context_ids), ptrs, lens))
+            yield
+        finally:
+            if context_ids is not None:
+                _lib.check(self._lib.asrb_session_set_context(s, 0, None, None))
+            for key, conf in undo:
+                _lib.check(self._lib.asrb_session_set_option(s, key.encode(), conf.encode()))
+
+    def _last_batch(self) -> Tuple[int, int]:
+        """(the session's batch capacity, the utterances of its last run) for the asrb_last_* reads; AsrbError
+        (ASRB_ERR_STATE) before anything has run."""
+        if self._session is None:
+            raise _lib.AsrbError(4, "no session: nothing has run yet")
+        return self._cap[0], getattr(self, "_B", self._cap[0])
 
     def last_prefill_stats(self) -> Dict[str, int]:
         """asrb_last_prefill_stats: rows computed, rows taken from a leader's shared context, KV bytes fanned out."""
@@ -580,22 +690,14 @@ class AsrInference:
         return dict(zip(("rows_computed", "rows_shared", "fanout_kv_bytes"), [int(v) for v in out]))
 
     # ---- per-token log-probabilities (session option "logprobs") ----------------------------
-    def _record_logprobs(self, s, on: bool) -> None:
-        """Switch recording on for one call (True) or back to the engine's configured value (False)."""
-        if self._options.get("logprobs") != "1":
-            _lib.check(self._lib.asrb_session_set_option(s, b"logprobs", b"1" if on else b"0"))
-
     def last_logprobs(self, max_new_tokens: int):
         """asrb_last_logprobs: (per-utterance log-probabilities of the ids of the last run, EOS log-probability or None).
         Raises AsrbError (ASRB_ERR_STATE) when the last run did not record them."""
-        if self._session is None:
-            raise _lib.AsrbError(4, "no session: nothing has run yet")
-        cap = self._cap[0]                                   # the library writes one row per utterance of the last run
+        cap, B = self._last_batch()                          # the library writes one row per utterance of the last run
         lp = np.full((cap, max_new_tokens), np.nan, dtype=np.float32)
         eos = np.full(cap, np.nan, dtype=np.float32)
         _lib.check(self._lib.asrb_last_logprobs(self._session, int(max_new_tokens), lp.ctypes.data_as(C.POINTER(C.c_float)),
                                                 eos.ctypes.data_as(C.POINTER(C.c_float))))
-        B = getattr(self, "_B", cap)
         rows = []
         for r in lp[:B]:                                     # each row: the finite prefix (NaN from the utterance's length on)
             nan = np.flatnonzero(np.isnan(r))
@@ -603,21 +705,12 @@ class AsrInference:
         return rows, [None if np.isnan(e) else float(e) for e in eos[:B]]
 
     # ---- top-k alternatives (session option "top_logprobs") ------------------------------------
-    def _record_top_logprobs(self, s, k: int, on: bool) -> None:
-        """Record k >= 1 alternatives for one call (True) or go back to the engine's configured value (False).  Nothing
-        is set when the two agree (setting an option drops the captured per-phase step graph)."""
-        conf = self._options.get("top_logprobs", "0")
-        if conf != str(k):
-            _lib.check(self._lib.asrb_session_set_option(s, b"top_logprobs", (str(k) if on else conf).encode()))
-
     def last_top_logprobs(self, max_new_tokens: int, k: int):
         """asrb_last_top_logprobs: (per utterance, per id of the last run, the k best candidates of its step as
         (id, log p) pairs, best first; per utterance the same for the step that selected the ending EOS, or None).
         Raises AsrbError: ASRB_ERR_STATE when the last run did not record them, ASRB_ERR_INVALID when k is outside
         [1, the recorded top_logprobs]."""
-        if self._session is None:
-            raise _lib.AsrbError(4, "no session: nothing has run yet")
-        cap = self._cap[0]
+        cap, B = self._last_batch()
         ids = np.full((cap, max_new_tokens, max(k, 1)), -1, dtype=np.int32)
         lp = np.full(ids.shape, np.nan, dtype=np.float32)
         eids = np.full((cap, max(k, 1)), -1, dtype=np.int32)
@@ -626,7 +719,6 @@ class AsrInference:
             self._session, int(max_new_tokens), int(k), ids.ctypes.data_as(C.POINTER(C.c_int32)),
             lp.ctypes.data_as(C.POINTER(C.c_float)), eids.ctypes.data_as(C.POINTER(C.c_int32)),
             elp.ctypes.data_as(C.POINTER(C.c_float))))
-        B = getattr(self, "_B", cap)
         rows = []
         for b in range(B):                                   # the rows before the utterance's length (-1 from there on)
             n = int(np.count_nonzero(ids[b, :, 0] >= 0))
@@ -639,9 +731,7 @@ class AsrInference:
         """asrb_last_nbest: per utterance of the last beam run, its k best hypotheses ranked as (ids, sum_logprob,
         score, eos_id; -1 = stopped by the cap).  Raises AsrbError: ASRB_ERR_STATE when the last run was not a beam
         run, ASRB_ERR_INVALID when k is outside [1, beam_size]."""
-        if self._session is None:
-            raise _lib.AsrbError(4, "no session: nothing has run yet")
-        B = getattr(self, "_B", self._cap[0])
+        _, B = self._last_batch()
         kk = max(int(k), 1)
         ids = np.full((B, kk, max_new_tokens), -1, dtype=np.int32)
         lens = np.zeros((B, kk), dtype=np.int32)
@@ -661,18 +751,6 @@ class AsrInference:
         _lib.check(self._lib.asrb_last_beam_stats(self._session, out, 4))
         return dict(zip(("beam_steps", "slots_reassigned", "expand_kv_bytes", "reorder_kv_bytes"), [int(v) for v in out]))
 
-    def _set_beam(self, s, k: int, length_penalty: Optional[float]) -> List[Tuple[str, str]]:
-        """Set beam_size k and the length penalty for one call; returns the (option, configured value) pairs to
-        restore.  Nothing is set when they agree (setting an option drops the captured per-phase step graph)."""
-        undo = []
-        vals = (("beam_size", str(k)), ("length_penalty", length_penalty_option(length_penalty))) if k > 1 else (("beam_size", "1"),)
-        for key, val in vals:
-            conf = self._options.get(key, {"beam_size": "1", "length_penalty": "none"}[key])
-            if conf != val:
-                _lib.check(self._lib.asrb_session_set_option(s, key.encode(), val.encode()))
-                undo.append((key, conf))
-        return undo
-
     def _finish(self, s, B: int, ids, n, max_new_tokens: int, logprobs: bool, top_logprobs: int = 0,
                 beam_size: int = 1) -> TranscribeIds:
         ms = (C.c_float * 6)()
@@ -690,33 +768,6 @@ class AsrInference:
         return r
 
     # ---- seeded temperature sampling (session options "temperature" / "seed") ---------------------------
-    def _set_sampling(self, s, t: Optional[float], seed: int) -> List[Tuple[str, str]]:
-        """Set temperature t and seed for one call; returns the (option, configured value) pairs to restore."""
-        undo = []
-        if t is None:
-            return undo
-        for key, val in (("temperature", temperature_option(t)), ("seed", str(seed))):
-            conf = self._options.get(key, "0")
-            if conf != val:
-                _lib.check(self._lib.asrb_session_set_option(s, key.encode(), val.encode()))
-                undo.append((key, conf))
-        return undo
-
-    # ---- repetition controls (session options "no_repeat_ngram_size" / "repetition_penalty") ------------------
-    def _set_repetition(self, s, rep: Tuple[int, float]) -> List[Tuple[str, str]]:
-        """Set N and the penalty for one call; returns the (option, configured value) pairs to restore."""
-        undo = []
-        for key, val in (("no_repeat_ngram_size", str(rep[0])), ("repetition_penalty", repetition_penalty_option(rep[1]))):
-            conf = self._options.get(key, {"no_repeat_ngram_size": "0", "repetition_penalty": "1"}[key])
-            if conf != val:
-                _lib.check(self._lib.asrb_session_set_option(s, key.encode(), val.encode()))
-                undo.append((key, conf))
-        return undo
-
-    def _restore(self, s, undo) -> None:
-        for key, conf in undo:
-            _lib.check(self._lib.asrb_session_set_option(s, key.encode(), conf.encode()))
-
     def _sampled(self, B: int, once, temperature, seed, logprob_threshold, logprobs: bool, top_logprobs: int,
                  beam_size: int = 1, length_penalty: Optional[float] = None) -> TranscribeIds:
         """One call of transcribe_ids / transcribe_pcm.  `once(indices, logprobs, top_logprobs, t, beam)` runs the
@@ -775,56 +826,33 @@ class AsrInference:
         `no_repeat_ngram_size` N >= 1 bans every id that would repeat an N-gram of the ids generated so far, and
         `repetition_penalty` > 1 divides the positive (multiplies the negative) logits of ids generated so far, in every
         attempt, beam and path (include/asr_b200.h); the prompt and context never count."""
-        ctx = check_context_ids(context_ids, len(clips), self.config.text.vocab_size)
+        return self._transcribe(_Audio("ids", clips, None, language_ids), max_new_tokens, logprobs, top_logprobs,
+                                temperature, seed, logprob_threshold, beam_size, length_penalty, context_ids,
+                                no_repeat_ngram_size, repetition_penalty)
+
+    def _transcribe(self, src: _Audio, max_new_tokens: int, logprobs: bool, top_logprobs: int, temperature, seed: int,
+                    logprob_threshold: Optional[float], beam_size: int, length_penalty: Optional[float], context_ids,
+                    no_repeat_ngram_size: int, repetition_penalty: float) -> TranscribeIds:
+        """transcribe_ids / transcribe_pcm on the items of `src`."""
+        src = replace(src, ctx=check_context_ids(context_ids, len(src), self.config.text.vocab_size))
         rep = check_repetition(no_repeat_ngram_size, repetition_penalty)
+        return self._sampled(len(src), lambda idx, lp, k, t, beam: self._run(src.subset(idx), max_new_tokens, lp, k, t,
+                                                                             seed, beam, rep),
+                             temperature, seed, logprob_threshold, logprobs, top_logprobs, beam_size, length_penalty)
 
-        def once(idx, lp, k, t, beam):
-            sub = clips if len(idx) == len(clips) else [clips[i] for i in idx]
-            lang = None if language_ids is None else [language_ids[i] for i in idx]
-            return self._ids_once(sub, lang, max_new_tokens, lp, k, t, seed, beam,
-                                  None if ctx is None else [ctx[i] for i in idx], rep)
-        return self._sampled(len(clips), once, temperature, seed, logprob_threshold, logprobs, top_logprobs,
-                             beam_size, length_penalty)
-
-    def _ids_once(self, clips, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
-                  temperature: Optional[float], seed: int, beam=None, context_ids=None, rep=(0, 1.0)) -> TranscribeIds:
-        B = len(clips)
-        K = beam[0] if beam else 1
-        arrs, ptrs, lens = self._pack_samples(clips)
-        keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
-        s = self._ensure_session(B * K, max(a.shape[0] for a in arrs), mx, max_new_tokens, _max_len(context_ids))
-        return self._run(s, B, max_new_tokens, logprobs, top_logprobs, temperature, seed, beam, context_ids,
-                         lambda ids, n: self._lib.asrb_transcribe_ids(s, ptrs, lens, B, lptrs, llens, int(max_new_tokens),
-                                                                      ids, n), rep)
-
-    def _run(self, s, B: int, max_new_tokens: int, logprobs: bool, top_logprobs: int, temperature: Optional[float],
-             seed: int, beam, context_ids, call, rep=(0, 1.0)) -> TranscribeIds:
-        """One decode call on session s with this call's options set and restored around it: `call(ids_out, lens_out)`
-        runs the library's transcribe entry point for B utterances and returns its status; `rep` = (N, penalty)."""
-        K = beam[0] if beam else 1
+    def _run(self, src: _Audio, max_new_tokens: int, logprobs: bool, top_logprobs: int, temperature: Optional[float],
+             seed: int, beam, rep: Tuple[int, float]) -> TranscribeIds:
+        """One decode call of the items of `src` at `temperature` (None: the session's configured options) with
+        beam = (K, length penalty) (None: greedy or sampling) and rep = (N, penalty)."""
+        B, K = len(src), beam[0] if beam else 1
+        s = src.prepare(self, B * K, max_new_tokens)
         ids = np.zeros((B, max_new_tokens), dtype=np.int32)
         n = np.zeros(B, dtype=np.int32)
-        if logprobs:
-            self._record_logprobs(s, True)
-        if top_logprobs:
-            self._record_top_logprobs(s, top_logprobs, True)
-        undo = []
-        try:
-            undo = self._set_sampling(s, temperature, seed)
-            undo += self._set_beam(s, K, beam[1] if beam else None)
-            undo += self._set_repetition(s, rep)
-            if context_ids is not None:
-                self._set_context(s, context_ids)
-            _lib.check(call(ids.ctypes.data_as(C.POINTER(C.c_int32)), n.ctypes.data_as(C.POINTER(C.c_int32))))
+        with self._call_scope(s, _decode_options(logprobs, top_logprobs, temperature, seed, beam or (1, None), rep),
+                              src.ctx):
+            _lib.check(src.call(self._lib, "transcribe", int(max_new_tokens), ids.ctypes.data_as(C.POINTER(C.c_int32)),
+                                n.ctypes.data_as(C.POINTER(C.c_int32))))
             return self._finish(s, B, ids, n, max_new_tokens, logprobs, top_logprobs, K)
-        finally:
-            if context_ids is not None:
-                self._set_context(s, None)
-            self._restore(s, undo)
-            if logprobs:
-                self._record_logprobs(s, False)
-            if top_logprobs:
-                self._record_top_logprobs(s, top_logprobs, False)
 
     # ---- streaming (asrb_stream_*) ------------------------------------------------------------------------------------
     def open_streams(self, n: int, max_seconds: float, language: Optional[str] = None, context: Optional[str] = None,
@@ -857,51 +885,32 @@ class AsrInference:
         and context included).  The candidates of a clip share its prompt's prefill.  With `top_logprobs` = k in 1..8,
         also the k best ids of every position and the greedy prefix.  More candidates than SCORE_SLOTS run in several
         calls of whole utterances."""
-        B = len(clips)
-        cands = check_candidates(candidates, B, self.config.text.vocab_size)
-        k = check_top_logprobs(top_logprobs)
-        ctx = check_context_ids(context_ids, B, self.config.text.vocab_size)
-        out: List[List[ScoredCandidate]] = [None] * B
-        for wave in score_waves([len(c) for c in cands], SCORE_SLOTS):
-            sub = [clips[b] for b in wave]
-            arrs, ptrs, lens = self._pack_samples(sub)
-            lang = None if language_ids is None else [language_ids[b] for b in wave]
-            keep, lptrs, llens, mx = self._pack_lang(lang, len(wave))
-            wc = [cands[b] for b in wave]
-            n_total = sum(len(c) for c in wc)
-            max_new = max(len(c) for cs in wc for c in cs)
-            wctx = None if ctx is None else [ctx[b] for b in wave]
-            s = self._ensure_session(n_total, max(a.shape[0] for a in arrs), mx, max_new, _max_len(wctx))
-            res = self._score(s, wc, max_new, k, wctx, lambda *a: self._lib.asrb_score_ids(s, ptrs, lens, len(wave), lptrs, llens, *a))
-            for b, r in zip(wave, res):
-                out[b] = r
-        return out
+        return self._score_waves(_Audio("ids", clips, None, language_ids), candidates, context_ids, top_logprobs)
 
     def score_pcm(self, pcms: Sequence, rates: Sequence[int], candidates: Sequence[Sequence[Sequence[int]]],
                   language_ids: Optional[Sequence] = None, context_ids: Optional[Sequence] = None,
                   top_logprobs: int = 0) -> List[List[ScoredCandidate]]:
         """score_ids with step 1 on the GPU: raw PCM in (as transcribe_pcm)."""
-        B = len(pcms)
+        return self._score_waves(_Audio("ingested", pcms, rates, language_ids), candidates, context_ids, top_logprobs)
+
+    def _score_waves(self, src: _Audio, candidates, context_ids, top_logprobs: int) -> List[List[ScoredCandidate]]:
+        """score_ids / score_pcm on the items of `src`: one _score call per wave of whole utterances."""
+        B = len(src)
         cands = check_candidates(candidates, B, self.config.text.vocab_size)
         k = check_top_logprobs(top_logprobs)
-        ctx = check_context_ids(context_ids, B, self.config.text.vocab_size)
+        src = replace(src, ctx=check_context_ids(context_ids, B, self.config.text.vocab_size))
         out: List[List[ScoredCandidate]] = [None] * B
         for wave in score_waves([len(c) for c in cands], SCORE_SLOTS):
-            lang = None if language_ids is None else [language_ids[b] for b in wave]
-            keep, lptrs, llens, mx = self._pack_lang(lang, len(wave))
-            wc = [cands[b] for b in wave]
-            max_new = max(len(c) for cs in wc for c in cs)
-            wctx = None if ctx is None else [ctx[b] for b in wave]
-            s, _arrs, _n = self._ingest([pcms[b] for b in wave], [rates[b] for b in wave], mx, max_new,
-                                        slots=sum(len(c) for c in wc), max_context=_max_len(wctx))
-            res = self._score(s, wc, max_new, k, wctx, lambda *a: self._lib.asrb_score_ingested(s, lptrs, llens, *a))
-            for b, r in zip(wave, res):
+            for b, r in zip(wave, self._score(src.subset(wave), [cands[b] for b in wave], k)):
                 out[b] = r
         return out
 
-    def _score(self, s, cands: List[List[List[int]]], max_new: int, k: int, context_ids, call) -> List[List[ScoredCandidate]]:
+    def _score(self, src: _Audio, cands: List[List[List[int]]], k: int) -> List[List[ScoredCandidate]]:
+        """One scoring call: cands[b] = the candidates of item b of `src`."""
         flat = [c for cs in cands for c in cs]
         N = len(flat)
+        max_new = max(len(c) for c in flat)
+        s = src.prepare(self, N, max_new)
         n_cand = (C.c_int32 * len(cands))(*[len(cs) for cs in cands])
         arrs = [np.ascontiguousarray(c, dtype=np.int64) for c in flat]
         cptrs = (C.POINTER(C.c_int64) * N)(*[a.ctypes.data_as(C.POINTER(C.c_int64)) for a in arrs])
@@ -909,19 +918,11 @@ class AsrInference:
         lp = np.empty((N, max_new), dtype=np.float32)
         tid = np.empty((N, max_new, max(k, 1)), dtype=np.int32)
         tlp = np.empty((N, max_new, max(k, 1)), dtype=np.float32)
-        if k:
-            self._record_top_logprobs(s, k, True)
-        try:
-            if context_ids is not None:
-                self._set_context(s, context_ids)
-            _lib.check(call(n_cand, cptrs, clens, int(max_new), lp.ctypes.data_as(C.POINTER(C.c_float)),
-                            tid.ctypes.data_as(C.POINTER(C.c_int32)) if k else None,
-                            tlp.ctypes.data_as(C.POINTER(C.c_float)) if k else None))
-        finally:
-            if context_ids is not None:
-                self._set_context(s, None)
-            if k:
-                self._record_top_logprobs(s, k, False)
+        with self._call_scope(s, {"top_logprobs": str(k)} if k else {}, src.ctx):
+            _lib.check(src.call(self._lib, "score", n_cand, cptrs, clens, int(max_new),
+                                lp.ctypes.data_as(C.POINTER(C.c_float)),
+                                tid.ctypes.data_as(C.POINTER(C.c_int32)) if k else None,
+                                tlp.ctypes.data_as(C.POINTER(C.c_float)) if k else None))
         res, q = [], 0
         for cs in cands:
             row = []
@@ -980,47 +981,33 @@ class AsrInference:
         teacher-forced pass over the prompt transcribe_ids builds (language ids and context included) and ids[b]
         (normally the decoded ids followed by EOS).  `alignment_heads`: (layer, query head) pairs, None = every head of
         the second half of the layers.  More clips than SCORE_SLOTS run in several calls."""
-        B = len(clips)
-        t = self.config.text
-        rows, tf = check_align_ids(ids, text_from, B, t.vocab_size)
-        heads = check_alignment_heads(alignment_heads, t.num_hidden_layers, t.num_attention_heads)
-        ctx = check_context_ids(context_ids, B, t.vocab_size)
-        out: List[Alignment] = [None] * B
-        for wave in score_waves([1] * B, SCORE_SLOTS):
-            arrs, ptrs, lens = self._pack_samples([clips[b] for b in wave])
-            lang = None if language_ids is None else [language_ids[b] for b in wave]
-            keep, lptrs, llens, mx = self._pack_lang(lang, len(wave))
-            wrows = [rows[b] for b in wave]
-            wctx = None if ctx is None else [ctx[b] for b in wave]
-            s = self._ensure_session(len(wave), max(a.shape[0] for a in arrs), mx, max(len(r) for r in wrows), _max_len(wctx))
-            res = self._align(s, wrows, [tf[b] for b in wave], heads, wctx,
-                              lambda *a: self._lib.asrb_align_ids(s, ptrs, lens, len(wave), lptrs, llens, *a))
-            for b, r in zip(wave, res):
-                out[b] = r
-        return out
+        return self._align_checked(_Audio("ids", clips, None, language_ids), ids, text_from, context_ids, alignment_heads)
 
     def align_pcm(self, pcms: Sequence, rates: Sequence[int], ids: Sequence[Sequence[int]],
                   text_from: Optional[Sequence[int]] = None, language_ids: Optional[Sequence] = None,
                   context_ids: Optional[Sequence] = None,
                   alignment_heads: Optional[Sequence[Tuple[int, int]]] = None) -> List[Alignment]:
         """align_ids with step 1 on the GPU: raw PCM in (as transcribe_pcm)."""
-        B = len(pcms)
+        return self._align_checked(_Audio("ingested", pcms, rates, language_ids), ids, text_from, context_ids,
+                                   alignment_heads)
+
+    def _align_checked(self, src: _Audio, ids, text_from, context_ids, alignment_heads) -> List[Alignment]:
+        """align_ids / align_pcm on the items of `src`, SCORE_SLOTS per call."""
         t = self.config.text
-        rows, tf = check_align_ids(ids, text_from, B, t.vocab_size)
+        rows, tf = check_align_ids(ids, text_from, len(src), t.vocab_size)
         heads = check_alignment_heads(alignment_heads, t.num_hidden_layers, t.num_attention_heads)
-        ctx = check_context_ids(context_ids, B, t.vocab_size)
-        out: List[Alignment] = [None] * B
-        for wave in score_waves([1] * B, SCORE_SLOTS):
-            lang = None if language_ids is None else [language_ids[b] for b in wave]
-            keep, lptrs, llens, mx = self._pack_lang(lang, len(wave))
-            wrows = [rows[b] for b in wave]
-            wctx = None if ctx is None else [ctx[b] for b in wave]
-            s, _arrs, _n = self._ingest([pcms[b] for b in wave], [rates[b] for b in wave], mx, max(len(r) for r in wrows),
-                                        max_context=_max_len(wctx))
-            res = self._align(s, wrows, [tf[b] for b in wave], heads, wctx,
-                              lambda *a: self._lib.asrb_align_ingested(s, lptrs, llens, *a))
-            for b, r in zip(wave, res):
-                out[b] = r
+        src = replace(src, ctx=check_context_ids(context_ids, len(src), t.vocab_size))
+        return self._align_waves(src, rows, tf, heads, SCORE_SLOTS)
+
+    def _align_waves(self, src: _Audio, rows: List[List[int]], tf: List[int], heads: List[Tuple[int, int]],
+                     per_call: int) -> List[Alignment]:
+        """Alignments of the items of `src` (ids rows[b] from tf[b] on), in calls of `per_call` items."""
+        out: List[Alignment] = []
+        for w0 in range(0, len(rows), per_call):
+            wrows, wtf = rows[w0:w0 + per_call], tf[w0:w0 + per_call]
+            sub = src.subset(range(w0, w0 + len(wrows)))
+            s = sub.prepare(self, len(wrows), max(len(r) for r in wrows))
+            out += self._align(s, wrows, wtf, heads, sub.ctx, lambda *a: sub.call(self._lib, "align", *a))
         return out
 
     def _align(self, s, rows: List[List[int]], tf: List[int], heads: List[Tuple[int, int]], context_ids,
@@ -1035,14 +1022,9 @@ class AsrInference:
         harr = np.ascontiguousarray(np.array(heads, dtype=np.int32).reshape(-1, 2))
         st = np.empty((B, max_ids), dtype=np.int32)
         en = np.empty((B, max_ids), dtype=np.int32)
-        try:
-            if context_ids is not None:
-                self._set_context(s, context_ids)
+        with self._call_scope(s, {}, context_ids):
             _lib.check(call(iptrs, n_ids, tfa, harr.ctypes.data_as(C.POINTER(C.c_int32)) if heads else None, len(heads),
                             int(max_ids), st.ctypes.data_as(C.POINTER(C.c_int32)), en.ctypes.data_as(C.POINTER(C.c_int32))))
-        finally:
-            if context_ids is not None:
-                self._set_context(s, None)
         self._B = B
         return [Alignment(f, [int(v) for v in st[b, f:len(r)]], [int(v) for v in en[b, f:len(r)]])
                 for b, (r, f) in enumerate(zip(rows, tf))]
@@ -1080,24 +1062,14 @@ class AsrInference:
         return build_words(self._decode_fn(), text, al.start_s[:len(text)], al.start_s[len(text)], lp, language, offset_s)
 
     # ---- GPU-side audio ingest (step 1, src/audio.rs:162-245) -------------------------------------------
-    _PCM_FMT = {"int16": 0, "float32": 1, "int32": 2}
-
     def _ingest(self, pcms: Sequence, rates: Sequence[int], max_lang: int, max_new: int, slots: int = 0,
                 max_context: int = 0):
-        B = len(pcms)
-        arrs = [np.ascontiguousarray(a if a.ndim == 2 else a.reshape(-1, 1)) for a in pcms]
-        for a in arrs:
-            if a.dtype.name not in self._PCM_FMT:
-                raise ValueError(f"PCM dtype must be int16 / int32 / float32, got {a.dtype}")
+        arrs = _pcm_arrays(pcms)
+        B = len(arrs)
         n_out = [-(-a.shape[0] * MEL_SAMPLE_RATE // int(r)) for a, r in zip(arrs, rates)]
         s = self._ensure_session(max(B, slots), max(n_out), max_lang, max_new, max_context)
-        ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in arrs])
-        frames = (C.c_int64 * B)(*[a.shape[0] for a in arrs])
-        chans = (C.c_int32 * B)(*[a.shape[1] for a in arrs])
-        rts = (C.c_int32 * B)(*[int(r) for r in rates])
-        fmts = (C.c_int32 * B)(*[self._PCM_FMT[a.dtype.name] for a in arrs])
         n = (C.c_int64 * B)()
-        _lib.check(self._lib.asrb_ingest_pcm(s, ptrs, frames, chans, rts, fmts, B, n))
+        _lib.check(self._lib.asrb_ingest_pcm(s, *_pcm_args(arrs, rates), B, n))
         return s, arrs, list(n)
 
     def ingest_pcm(self, pcms: Sequence, rates: Sequence[int]) -> List[np.ndarray]:
@@ -1119,26 +1091,9 @@ class AsrInference:
         """transcribe() steps 1-8 for a batch with step 1 on the GPU: raw PCM in, token ids out (`logprobs`,
         `top_logprobs`, `temperature`, `seed`, `logprob_threshold`, `beam_size`, `length_penalty`, `context_ids`,
         `no_repeat_ngram_size`, `repetition_penalty`: as in transcribe_ids)."""
-        ctx = check_context_ids(context_ids, len(pcms), self.config.text.vocab_size)
-        rep = check_repetition(no_repeat_ngram_size, repetition_penalty)
-
-        def once(idx, lp, k, t, beam):
-            sel = (lambda xs: xs if len(idx) == len(pcms) else [xs[i] for i in idx])
-            lang = None if language_ids is None else sel(language_ids)
-            return self._pcm_once(sel(pcms), sel(rates), lang, max_new_tokens, lp, k, t, seed, beam,
-                                  None if ctx is None else sel(ctx), rep)
-        return self._sampled(len(pcms), once, temperature, seed, logprob_threshold, logprobs, top_logprobs,
-                             beam_size, length_penalty)
-
-    def _pcm_once(self, pcms, rates, language_ids, max_new_tokens: int, logprobs: bool, top_logprobs: int,
-                  temperature: Optional[float], seed: int, beam=None, context_ids=None, rep=(0, 1.0)) -> TranscribeIds:
-        B = len(pcms)
-        K = beam[0] if beam else 1
-        keep, lptrs, llens, mx = self._pack_lang(language_ids, B)
-        s, _arrs, _n = self._ingest(pcms, rates, mx, max_new_tokens, slots=B * K, max_context=_max_len(context_ids))
-        return self._run(s, B, max_new_tokens, logprobs, top_logprobs, temperature, seed, beam, context_ids,
-                         lambda ids, n: self._lib.asrb_transcribe_ingested(s, lptrs, llens, int(max_new_tokens), ids, n),
-                         rep)
+        return self._transcribe(_Audio("ingested", pcms, rates, language_ids), max_new_tokens, logprobs, top_logprobs,
+                                temperature, seed, logprob_threshold, beam_size, length_penalty, context_ids,
+                                no_repeat_ngram_size, repetition_penalty)
 
     # ---- long-form audio: cut at low-energy points on the GPU, decode the pieces in waves -----------------------
     def ingest_long(self, pcms: Sequence, rates: Sequence[int]) -> List[np.ndarray]:
@@ -1155,14 +1110,8 @@ class AsrInference:
 
     def _ingest_long(self, pcms: Sequence, rates: Sequence[int], s):
         arrs = _pcm_arrays(pcms)
-        B = len(arrs)
-        ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in arrs])
-        frames = (C.c_int64 * B)(*[a.shape[0] for a in arrs])
-        chans = (C.c_int32 * B)(*[a.shape[1] for a in arrs])
-        rts = (C.c_int32 * B)(*[int(r) for r in rates])
-        fmts = (C.c_int32 * B)(*[self._PCM_FMT[a.dtype.name] for a in arrs])
-        n = (C.c_int64 * B)()
-        _lib.check(self._lib.asrb_ingest_long(s, ptrs, frames, chans, rts, fmts, B, n))
+        n = (C.c_int64 * len(arrs))()
+        _lib.check(self._lib.asrb_ingest_long(s, *_pcm_args(arrs, rates), len(arrs), n))
         return s, list(n)
 
     def segment_long(self, max_segment_samples: int, search_samples: int) -> List[List[Tuple[int, int]]]:
@@ -1231,24 +1180,17 @@ class AsrInference:
         self._long_files = n_files
         cuts = self.segment_long(max_seg, search)
         segs = [(f, a, b) for f in range(n_files) for a, b in cuts[f]]
-        self._long_waves = 0
+        src = _Audio("segments", segs, None, None if language_ids is None else [language_ids[f] for f, _, _ in segs],
+                     None if ctx is None else [ctx[f] for f, _, _ in segs])
+        n_waves = 0
 
         def once(idx, lp, k, t, beam):
+            nonlocal n_waves
             W = batch // (beam[0] if beam else 1)
             runs = []
             for w0 in range(0, len(idx), W):
-                wave = [segs[i] for i in idx[w0:w0 + W]]
-                m = len(wave)
-                fl = (C.c_int32 * m)(*[x[0] for x in wave])
-                st = (C.c_int64 * m)(*[x[1] for x in wave])
-                en = (C.c_int64 * m)(*[x[2] for x in wave])
-                lang = None if language_ids is None else [language_ids[x[0]] for x in wave]
-                keep, lptrs, llens, _ = self._pack_lang(lang, m)
-                wctx = None if ctx is None else [ctx[x[0]] for x in wave]
-                runs.append(self._run(s, m, max_new_tokens, lp, k, t, seed, beam, wctx,
-                                      lambda ids, nn: self._lib.asrb_transcribe_segments(
-                                          s, m, fl, st, en, lptrs, llens, int(max_new_tokens), ids, nn), rep))
-                self._long_waves += 1
+                runs.append(self._run(src.subset(idx[w0:w0 + W]), max_new_tokens, lp, k, t, seed, beam, rep))
+                n_waves += 1
             return _concat_runs(runs)
         heads = check_alignment_heads(alignment_heads, self.config.text.num_hidden_layers,
                                       self.config.text.num_attention_heads) if word_timestamps else []
@@ -1257,18 +1199,8 @@ class AsrInference:
         als: List[Alignment] = []
         if word_timestamps:
             asr_text = self._asr_text_id()
-            for w0 in range(0, len(segs), batch):
-                wave = list(range(w0, min(w0 + batch, len(segs))))
-                m = len(wave)
-                fl = (C.c_int32 * m)(*[segs[i][0] for i in wave])
-                st = (C.c_int64 * m)(*[segs[i][1] for i in wave])
-                en = (C.c_int64 * m)(*[segs[i][2] for i in wave])
-                lang = None if language_ids is None else [language_ids[segs[i][0]] for i in wave]
-                keep, lptrs, llens, _ = self._pack_lang(lang, m)
-                wctx = None if ctx is None else [ctx[segs[i][0]] for i in wave]
-                rows = [r.ids[i] + [EOS_ID] for i in wave]
-                als += self._align(s, rows, [text_start(r.ids[i], asr_text) for i in wave], heads, wctx,
-                                   lambda *a: self._lib.asrb_align_segments(s, m, fl, st, en, lptrs, llens, *a))
+            als = self._align_waves(src, [ids + [EOS_ID] for ids in r.ids], [text_start(ids, asr_text) for ids in r.ids],
+                                    heads, batch)
         out: List[List[LongSegment]] = [[] for _ in range(n_files)]
         for i, (f, a, b) in enumerate(segs):
             seg = LongSegment(a / MEL_SAMPLE_RATE, b / MEL_SAMPLE_RATE, r.ids[i])
@@ -1284,7 +1216,7 @@ class AsrInference:
                 seg.words = self._words(r.ids[i], als[i], r.logprobs[i], self._word_language(r.ids[i], language),
                                         a / MEL_SAMPLE_RATE)
             out[f].append(seg)
-        return LongResult(out, r.stage_ms, r.kernels_launched, r.decode_steps, len(segs), self._long_waves)
+        return LongResult(out, r.stage_ms, r.kernels_launched, r.decode_steps, len(segs), n_waves)
 
     def transcribe(self, audio_path: str, language: Optional[str] = None,
                    max_new_tokens: int = MAX_NEW_TOKENS, gpu_ingest: bool = True, logprobs: bool = False,
@@ -1311,41 +1243,28 @@ class AsrInference:
         from .text import context_prompt_ids, language_prompt_ids, parse_asr_output
         lang_ids = language_prompt_ids(self.tokenizer, language)
         ctx_ids = context_prompt_ids(self.tokenizer, context)
+        lang = [lang_ids] if lang_ids is not None else None
+        ctx = [ctx_ids] if ctx_ids else None
         sampling = dict(temperature=temperature, seed=seed, logprob_threshold=logprob_threshold, beam_size=beam_size,
-                        length_penalty=length_penalty, context_ids=[ctx_ids] if ctx_ids else None,
-                        no_repeat_ngram_size=no_repeat_ngram_size, repetition_penalty=repetition_penalty)
-        if max_segment_s is not None:
-            if gpu_ingest:
-                pcm, rate = read_wav_pcm(audio_path)
-            else:
-                pcm, rate = load_wav(audio_path, MEL_SAMPLE_RATE), MEL_SAMPLE_RATE
-            lr = self.transcribe_long([pcm], [rate], max_segment_s=max_segment_s, search_s=default_search_s(max_segment_s),
-                                      language_ids=[lang_ids] if lang_ids is not None else None,
-                                      max_new_tokens=max_new_tokens, logprobs=logprobs, top_logprobs=top_logprobs,
-                                      word_timestamps=word_timestamps, alignment_heads=alignment_heads,
-                                      language=language, **sampling)
-            return self._long_result(lr.files[0], language, logprobs, top_logprobs)
-        lang_kw = dict(language_ids=[lang_ids] if lang_ids is not None else None)
+                        length_penalty=length_penalty, context_ids=ctx, no_repeat_ngram_size=no_repeat_ngram_size,
+                        repetition_penalty=repetition_penalty)
+        # checked before the file is read; transcribe_long checks them after its own arguments
         heads = check_alignment_heads(alignment_heads, self.config.text.num_hidden_layers,
-                                      self.config.text.num_attention_heads) if word_timestamps else None
-        lp = logprobs or word_timestamps
-        if gpu_ingest:
-            pcm, rate = read_wav_pcm(audio_path)
-            r = self.transcribe_pcm([pcm], [rate], max_new_tokens=max_new_tokens, logprobs=lp, top_logprobs=top_logprobs,
-                                    **lang_kw, **sampling)
-        else:
-            samples = load_wav(audio_path, MEL_SAMPLE_RATE)
-            r = self.transcribe_ids([samples], max_new_tokens=max_new_tokens, logprobs=lp, top_logprobs=top_logprobs,
-                                    **lang_kw, **sampling)
+                                      self.config.text.num_attention_heads) if word_timestamps and max_segment_s is None else None
+        pcm, rate = read_wav_pcm(audio_path) if gpu_ingest else (load_wav(audio_path, MEL_SAMPLE_RATE), MEL_SAMPLE_RATE)
+        if max_segment_s is not None:
+            lr = self.transcribe_long([pcm], [rate], max_segment_s=max_segment_s, search_s=default_search_s(max_segment_s),
+                                      language_ids=lang, max_new_tokens=max_new_tokens, logprobs=logprobs,
+                                      top_logprobs=top_logprobs, word_timestamps=word_timestamps,
+                                      alignment_heads=alignment_heads, language=language, **sampling)
+            return self._long_result(lr.files[0], language, logprobs, top_logprobs)
+        src = _Audio("ingested", [pcm], [rate], lang) if gpu_ingest else _Audio("ids", [pcm], None, lang)
+        r = self._transcribe(src, max_new_tokens=max_new_tokens, logprobs=logprobs or word_timestamps,
+                             top_logprobs=top_logprobs, **sampling)
         ids = r.ids[0]
         al = None
         if word_timestamps:
-            tf = [text_start(ids, self._asr_text_id())]
-            ctx_kw = dict(context_ids=[ctx_ids] if ctx_ids else None, alignment_heads=heads or None)
-            if gpu_ingest:
-                al = self.align_pcm([pcm], [rate], [ids + [EOS_ID]], text_from=tf, **lang_kw, **ctx_kw)[0]
-            else:
-                al = self.align_ids([samples], [ids + [EOS_ID]], text_from=tf, **lang_kw, **ctx_kw)[0]
+            al = self._align_checked(src, [ids + [EOS_ID]], [text_start(ids, self._asr_text_id())], ctx, heads or None)[0]
 
         def parse(ids):
             raw = self.tokenizer.decode(ids) if self.tokenizer is not None else " ".join(str(i) for i in ids)

@@ -66,7 +66,7 @@ class StreamSet:
     def __init__(self, eng, n: int, max_seconds: float, lang_ids: Optional[List[int]], context_ids: Optional[List[int]],
                  rollback: int, unfixed_pushes: int, max_new_tokens: int, logprobs: bool, top_logprobs: int,
                  temperature: float, seed: int, no_repeat_ngram_size: int, repetition_penalty: float):
-        from .inference import check_repetition, check_seed, check_temperature, check_top_logprobs
+        from .inference import _decode_options, check_repetition, check_seed, check_temperature, check_top_logprobs
         if n < 1:
             raise ValueError("n must be >= 1")
         if max_seconds <= 0:
@@ -75,33 +75,27 @@ class StreamSet:
             raise ValueError("rollback and unfixed_pushes must be >= 0")
         self._eng, self.n = eng, n
         self._lang = list(lang_ids) if lang_ids else []
-        self._ctx = list(context_ids) if context_ids else None
+        self._ctx = [list(context_ids)] if context_ids else None     # one context for every stream (set_context)
         self._max_new = int(max_new_tokens)
         self._top = check_top_logprobs(top_logprobs)
         self._logprobs = bool(logprobs) or self._top > 0
         temps = check_temperature(temperature)
         if len(temps) != 1:
             raise ValueError("streams take one temperature, not a fallback schedule")
-        self._temperature, self._seed = temps[0], check_seed(seed)
-        if self._top and self._temperature > 0.0:
+        t, seed = temps[0], check_seed(seed)
+        if self._top and t > 0.0:
             raise ValueError("temperature > 0 cannot be combined with top_logprobs")
-        self._rep = check_repetition(no_repeat_ngram_size, repetition_penalty)
+        # a push's session options: the records, sampling at t > 0 and the repetition controls (no beam on streams)
+        self._push_options = _decode_options(self._logprobs, self._top, t if t > 0.0 else None, seed, None,
+                                             check_repetition(no_repeat_ngram_size, repetition_penalty))
         self.max_samples = int(round(max_seconds * 16000))
         max_lang = stream_max_lang_ids(max_seconds, len(self._lang), self._max_new)
         self._max_ids = max_lang + self._max_new          # h = p + g
-        s = eng._ensure_session(n, max(self.max_samples, 201), max_lang, self._max_new, len(self._ctx) if self._ctx else 0)
+        s = eng._ensure_session(n, max(self.max_samples, 201), max_lang, self._max_new, len(self._ctx[0]) if self._ctx else 0)
         self._s = s
         self._n = [0] * n                  # samples pushed per stream
-        self._with_context(lambda: _lib.check(eng._lib.asrb_stream_open(s, n, int(rollback), int(unfixed_pushes))))
-
-    def _with_context(self, fn):
-        if self._ctx is None:
-            return fn()
-        self._eng._set_context(self._s, [self._ctx])
-        try:
-            return fn()
-        finally:
-            self._eng._set_context(self._s, None)
+        with eng._call_scope(s, {}, self._ctx):
+            _lib.check(eng._lib.asrb_stream_open(s, n, int(rollback), int(unfixed_pushes)))
 
     def _session(self):
         if self._eng._session is not self._s:
@@ -126,14 +120,7 @@ class StreamSet:
         hyp = np.zeros((n, self._max_ids), dtype=np.int32)
         hl, fl = np.zeros(n, dtype=np.int32), np.zeros(n, dtype=np.int32)
         P = C.POINTER
-        if self._logprobs:
-            eng._record_logprobs(s, True)
-        if self._top:
-            eng._record_top_logprobs(s, self._top, True)
-        undo = []
-        try:
-            undo = eng._set_sampling(s, self._temperature if self._temperature > 0.0 else None, self._seed)
-            undo += eng._set_repetition(s, self._rep)
+        with eng._call_scope(s, self._push_options):
             _lib.check(lib.asrb_stream_push(s, n, ptrs, lens, fins, lptrs, llens, self._max_new, self._max_ids,
                                             hyp.ctypes.data_as(P(C.c_int32)), hl.ctypes.data_as(P(C.c_int32)),
                                             fl.ctypes.data_as(P(C.c_int32))))
@@ -150,12 +137,6 @@ class StreamSet:
                 tk, _ = eng.last_top_logprobs(self._max_new, self._top)
                 for b in range(n):
                     out[b].top_logprobs = tk[b] if active[b] else None
-        finally:
-            eng._restore(s, undo)
-            if self._logprobs:
-                eng._record_logprobs(s, False)
-            if self._top:
-                eng._record_top_logprobs(s, self._top, False)
         if eng.tokenizer is not None:
             from .text import parse_asr_output
             forced = bool(self._lang)
@@ -167,7 +148,8 @@ class StreamSet:
     def reset(self, b: int) -> None:
         """Stream b back to its start (no samples, empty prefix), open again after a final push."""
         s = self._session()
-        self._with_context(lambda: _lib.check(self._eng._lib.asrb_stream_reset(s, int(b))))
+        with self._eng._call_scope(s, {}, self._ctx):
+            _lib.check(self._eng._lib.asrb_stream_reset(s, int(b)))
         self._n[b] = 0
 
     def stats(self) -> Dict[str, int]:
